@@ -1,4 +1,4 @@
-"""Builds the in-tree CUDA shared library (sm_100a only) with nvcc.  Used by __graft_entry__.build()."""
+"""Builds the in-tree CUDA shared library (sm_90a only) with nvcc.  Used by __graft_entry__.build()."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgypsum_b200.so")
 SOURCES = ["kernels.cu", "tracker.cu", "bits.cu", "fused.cu", "engine.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared", "-cudart", "static",
 ]
 

@@ -64,6 +64,10 @@ struct PinnedBuf {
     }
 };
 
+// L2 window of the one-warp correlate kernel: the fastest size for the benchmark's config-2 call and for config 3 on the
+// H100's 50 MB L2 (DESIGN.md §4, L2 windows).
+constexpr int kL2WindowMb = 16;
+
 int env_int(const char* name, int dflt) {
     const char* v = getenv(name);
     return (v && *v) ? atoi(v) : dflt;
@@ -72,7 +76,7 @@ int env_int(const char* name, int dflt) {
 }  // namespace
 
 struct gb200_engine {
-    int device = 0, fs = 0, N = 0, s = 0, num_sms = 148;
+    int device = 0, fs = 0, N = 0, s = 0, num_sms = 132;
     cudaStream_t own_stream = nullptr, stream = nullptr;
     DevBuf<float2> tw1, tw2, crep, iq_own, spec, d_replica;
     DevBuf<uint8_t> chips;
@@ -275,8 +279,7 @@ int pick_rsplit(const gb200_engine* e, int np, long long n_cells) {
 
 // Non-coherent, record-only launches use the one-warp-per-transform kernel: 12 warps per CTA (168 registers) for
 // single-millisecond searches, 8 warps (the 32 accumulators live across the milliseconds: 226 registers) for longer
-// integrations.  With the packed-FP32 codelets it beats the warp-pair kernel everywhere (config 3: 0.219 -> 0.181 ms,
-// profiles/ablation_r2.md), so the pair kernel keeps only the coherent and full-profile launches.
+// integrations; the pair kernel keeps only the coherent and full-profile launches.
 // Returns the warps per CTA, or 0 for the pair kernel.  GB200_W2048=0 disables it, =10 runs single-ms searches with 10 warps.
 int pick_w2048(const gb200_engine* e, int M, int kind, bool profile) {
     if (e->w2048 <= 0 || kind != GB200_NON_COHERENT || profile) return 0;
@@ -394,9 +397,9 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
         ca.cell_probe = nullptr;
         const int grid = std::min(ca.n_groups, e->num_sms);
         // L2 windows of the one-warp kernel (see the kernel): a batch whose spectra exceed L2 is walked in equal runs of units of
-        // about GB200_L2_WINDOW_MB (default 40; 0 = off), as long as a window still gives every CTA at least two groups (config 5's
-        // heavy cells: 2.8 groups per CTA and window; the kernel's round-robin of the extra groups keeps the CTAs together).
-        static const size_t win_bytes = static_cast<size_t>(std::max(0, env_int("GB200_L2_WINDOW_MB", 40))) << 20;
+        // about GB200_L2_WINDOW_MB (default kL2WindowMb; 0 = off), as long as a window still gives every CTA at least two groups
+        // (the kernel's round-robin of the extra groups keeps the CTAs together).
+        static const size_t win_bytes = static_cast<size_t>(std::max(0, env_int("GB200_L2_WINDOW_MB", kL2WindowMb))) << 20;
         ca.win_chunks = 0;
         const size_t batch_bytes = static_cast<size_t>(nbb) * per_block * sizeof(float2);
         if (nw && win_bytes && batch_bytes > win_bytes + win_bytes / 2) {
@@ -442,7 +445,7 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
     if (e->fused < 0 && fused_supports(e->s) && !profile_dev) {
         // Automatic choice.  The split kernels pay off when many cells share a Doppler bin (the PRN-independent half is
         // computed once per bin); lists with mostly distinct Dopplers (the refinement passes of acquisition.py:81-101)
-        // and small lists are faster through the fused block-per-cell kernel (profiles/configs_r1l.jsonl).
+        // and small lists are faster through the fused block-per-cell kernel.
         std::vector<double> u(dop, dop + n_cells);
         std::sort(u.begin(), u.end());
         const long long n_unique = std::unique(u.begin(), u.end()) - u.begin();
@@ -652,9 +655,8 @@ int gb200_create(int device, int fs, int n, gb200_engine** out) {
     e->fs = fs;
     e->N = n;
     e->s = n / kChips;
-    // Spectra scratch per launch pair.  It does not have to stay in L2: a launch writes and re-reads 21 MB per 16.368 Msps block
-    // in ~0.15 ms (< 0.3 TB/s), and launches that carry more cells run the correlate kernel without cross-warp merges and with a
-    // shorter tail (config 5: 99.7 -> 121.6 Msamples/s going from 80 MB to 512 MB; config 2 x 512 blocks +3 %).
+    // Spectra scratch per launch pair.  It does not have to stay in L2 (a launch writes and re-reads 21 MB per 16.368 Msps
+    // block), and launches that carry more cells run the correlate kernel without cross-warp merges and with a shorter tail.
     e->spec_budget_bytes = static_cast<size_t>(env_int("GB200_SPEC_BUDGET_MB", 512)) << 20;
     e->np_override = env_int("GB200_NP", 0);
     e->w2048 = env_int("GB200_W2048", 12);
@@ -669,8 +671,8 @@ int gb200_create(int device, int fs, int n, gb200_engine** out) {
     if ((ce = cudaSetDevice(device)) != cudaSuccess) return fail(ce, "cudaSetDevice");
     cudaDeviceProp prop;
     if ((ce = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return fail(ce, "cudaGetDeviceProperties");
-    if (prop.major != 10) {
-        g_create_error = "this build targets sm_100a (B200) only";
+    if (prop.major != 9 || prop.minor != 0) {
+        g_create_error = "this build targets sm_90a (H100) only";
         delete e;
         return GB200_ECUDA;
     }
@@ -834,8 +836,8 @@ int gb200_acquire_grid_host(gb200_engine* e, const float* iq_host, int n_blocks,
     GB_CUDA(e, e->d_records.ensure(n_rec));
     GB_CUDA(e, e->h_records.ensure(n_rec));
     // Large pinned inputs (a 10-ms window is 327 KB) are copied by the DMA engine straight from the caller's buffer: staging them
-    // would cost a 15-20 us host memcpy.  The copy node of the graph has its source baked in, so those calls launch eagerly
-    // (1.7 us more than a replay on this host, profiles/launch_latency_r2.log).  Small inputs are staged and replayed.
+    // would cost a host memcpy.  The copy node of the graph has its source baked in, so those calls launch eagerly (a few us
+    // more than a replay).  Small inputs are staged and replayed.
     const float2* h2d_src = e->h_iq.p;
     bool eager_src = false;
     if (n_iq * sizeof(float2) > (64u << 10)) {

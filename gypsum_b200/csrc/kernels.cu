@@ -1,4 +1,4 @@
-// sm_100a kernels of the acquisition correlation path (reference: gypsum/utils.py:59-116 driven by
+// sm_90a kernels of the acquisition correlation path (reference: gypsum/utils.py:59-116 driven by
 // gypsum/acquisition.py:154-190).  No cuFFT, no tensor cores, no CPU fallback.
 //
 //   doppler_spectra   per (Doppler, ms): carrier wipe-off (utils.py:93-97), polyphase boxcar, forward warp FFTs.
@@ -67,8 +67,7 @@ constexpr int kCarrierTable = 64;  // >= ceil(N / threads) for every supported r
 
 // When every (branch, parity) task has its own warp (2S <= 8) the transpose tiles take the place of the polyphase rows,
 // which are dead once every warp holds its vector in registers: 35 KB instead of 52 KB per 2.046 Msps CTA and, with the
-// register cap of five CTAs per SM, the 1312 units of a 32-block batch run in two waves instead of three (measured on
-// B200: 30.1 -> 24.0 us per 32-block launch, profiles/ablation_r2.md).
+// register cap of five CTAs per SM, the 1312 units of a 32-block batch run in two waves instead of three.
 __host__ __device__ constexpr bool spec_alias(int s) { return 2 * s <= 8; }
 __host__ __device__ constexpr int spec_f2(int s) {  // float2 of rows + tiles
     return spec_alias(s) ? (s * kFft > spec_warps(s) * kTileF2 ? s * kFft : spec_warps(s) * kTileF2)
@@ -86,9 +85,9 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 5 : 1) k_doppler_
 
     const int unit = blockIdx.x / a.M, i = blockIdx.x % a.M;
     const int b = unit / a.n_doppler, d = unit % a.n_doppler;
-    // (No early griddepcontrol.launch_dependents here: measured on B200 it let the FIRST dependent launch of a fresh
-    // engine read the spectra before they were written; the implicit trigger at grid completion keeps the launch-latency
-    // overlap -- 30.4 -> 27.9 us for a one-block search -- and is correct.)
+    // (No early griddepcontrol.launch_dependents here: it let the FIRST dependent launch of a fresh engine read the
+    // spectra before they were written; the implicit trigger at grid completion keeps the launch-latency overlap and is
+    // correct.)
     const double f = a.doppler[d];
     if (isnan(f)) return;  // slot switched off by the on-device search planner
     const float2* __restrict__ src = a.iq + static_cast<size_t>(b) * a.block_stride + static_cast<size_t>(i) * a.N;
@@ -99,7 +98,7 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 5 : 1) k_doppler_
     // error growth.
     constexpr int kIter = (kChips * S + kSpecThreads - 1) / kSpecThreads;  // samples per thread (16 for every S but 16: 64)
     // coalesced float2 loads of the 1-ms IQ vector, ALL issued before the carrier set-up and the first use (the loop form
-    // stalled on every load: 25 % of the kernel's stall samples, profiles/ablation_r2.md)
+    // stalls on every load)
     constexpr int kBatch = kIter < 16 ? kIter : 16;
     float2 v[kBatch];
 #pragma unroll
@@ -263,7 +262,7 @@ __global__ void __launch_bounds__(NP * 64, 1) k_correlate_cells(const CorrelateA
             parity ^= 1;
             cur_prn = prn;
             // De-phase the pairs after the CTA-wide barrier: warps that restart in step convoy on the shared-memory
-            // pipe (measured: -4 % on config 2, neutral elsewhere; profiles/ablation_r1.md).
+            // pipe.
             __nanosleep(pair * 300);
         }
 
@@ -465,9 +464,8 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
     int g1 = g0 + per_cta + (slot < extra ? 1 : 0);
     if (n_win == 1) {
         // one window (list mode, batches that fit in L2, cells too heavy to window): the proportional split.  Its range starts
-        // c * n_groups / grid fall on only grid / gcd(P, grid) distinct offsets within a PRN's cell list (37 for 32 PRNs on 148
-        // SMs), so four CTAs on different PRNs walk the same units at the same time -- measured 12 % faster on batches larger
-        // than L2 than a split without that property (profiles/ablation_r2.md, r2v).
+        // c * n_groups / grid fall on only grid / gcd(P, grid) distinct offsets within a PRN's cell list (33 for 32 PRNs on 132
+        // SMs), so four CTAs on different PRNs walk the same units at the same time.
         g0 = static_cast<int>(static_cast<long long>(blockIdx.x) * ng_w / n_cta);
         g1 = static_cast<int>(static_cast<long long>(blockIdx.x + 1) * ng_w / n_cta);
     }

@@ -1,4 +1,4 @@
-/* gypsum_b200 -- C ABI of the B200 acquisition / tracking correlation engine.
+/* gypsum_b200 -- C ABI of the H100 acquisition / tracking correlation engine.
  *
  * The reference (codyd51/gypsum) has no FFI: its boundary for this path is two Python classes and one pure
  * function.  Each entry point below names the reference interface it stands behind (paths relative to the

@@ -1,4 +1,4 @@
-"""Secondary measurements on one B200 (not the driver's bench line): BASELINE configs 2 (single block), 3, 5,
+"""Secondary measurements on one H100 (not the driver's bench line): BASELINE configs 2 (single block), 3, 5,
 the real 10-pass detector, and config 4 (tracking).  Prints one JSON line per workload.
 usage: python tools/bench_configs.py [--quick]"""
 import json

@@ -1,6 +1,6 @@
 """Emit gypsum_b200/csrc/fft32_gen.cuh: straight-line split-radix DFT codelets (length 32 and 64, forward and inverse) on
-float2 = (re, im) register arrays, natural order in and out, written with the packed-FP32 helpers of cplx2.cuh (sm_100
-FADD2 / FFMA2: one instruction per complex add, per rotation by +-j and per real-times-complex multiply-add).
+float2 = (re, im) register arrays, natural order in and out, written with the float2 helpers of cplx2.cuh (one
+helper per complex add, per rotation by +-j and per real-times-complex multiply-add).
 
 Twiddle constants are folded (1, -j, (1-j)/sqrt2 ... are special-cased) and every split-radix butterfly with non-trivial
 twiddles is written in the factored ("tangent") form, in which the two twiddle products, their sum / difference and the four

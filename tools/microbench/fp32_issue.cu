@@ -1,5 +1,5 @@
-// Microbenchmark: sustained FP32 warp-instruction issue rate per SM on B200 for the instruction forms the FFT
-// codelets are made of.  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp32_issue fp32_issue.cu && ./fp32_issue
+// Microbenchmark: sustained FP32 warp-instruction issue rate per SM on H100 for the instruction forms the FFT
+// codelets are made of.  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp32_issue fp32_issue.cu && ./fp32_issue
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -31,15 +31,15 @@ __global__ void k(float* out, int iters, float a, float b) {
 template <int MODE>
 void run(const char* name) {
     float* out;
-    cudaMalloc(&out, 148 * 1024 * sizeof(float));
+    cudaMalloc(&out, 132 * 1024 * sizeof(float));
     const int iters = 2000;
     for (int warps : {4, 8, 16, 32}) {
         cudaEvent_t e0, e1;
         cudaEventCreate(&e0);
         cudaEventCreate(&e1);
-        k<MODE><<<148, warps * 32>>>(out, 10, 1.0001f, 0.9999f);
+        k<MODE><<<132, warps * 32>>>(out, 10, 1.0001f, 0.9999f);
         cudaEventRecord(e0);
-        k<MODE><<<148, warps * 32>>>(out, iters, 1.0001f, 0.9999f);
+        k<MODE><<<132, warps * 32>>>(out, iters, 1.0001f, 0.9999f);
         cudaEventRecord(e1);
         cudaEventSynchronize(e1);
         float ms;

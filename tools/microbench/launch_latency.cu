@@ -1,7 +1,7 @@
 // Host-to-host overhead of a small CUDA-graph job (what gb200_acquire_grid_host pays around its two kernels), by variant:
 //   copy node vs a one-CTA loader kernel reading the pinned (device-mapped) source; cudaStreamSynchronize vs polling a flag the
 //   last CTA writes into pinned memory.  Kernels are empty apart from that, so the numbers are pure launch / completion cost.
-// build: nvcc -O2 -gencode arch=compute_100a,code=sm_100a -o launch_latency launch_latency.cu
+// build: nvcc -O2 -gencode arch=compute_90a,code=sm_90a -o launch_latency launch_latency.cu
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <chrono>

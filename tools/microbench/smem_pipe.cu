@@ -1,4 +1,4 @@
-// Microbenchmark: sustained shared-memory data-pipe throughput on B200 for the access patterns of the warp FFT
+// Microbenchmark: sustained shared-memory data-pipe throughput on H100 for the access patterns of the warp FFT
 // (128-bit row reads, 64-bit column writes at row stride 34 float2, pair-interleaved table reads).
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -57,7 +57,7 @@ __global__ void k(float* out, int iters) {
 template <int MODE>
 void run(const char* name, double wf_per_iter) {
     float* out;
-    cudaMalloc(&out, 148 * 1024 * sizeof(float));
+    cudaMalloc(&out, 132 * 1024 * sizeof(float));
     const int iters = 4000;
     for (int warps : {4, 8, 16, 20}) {
         const size_t sm = warps * 32 * kStride * sizeof(float2);
@@ -65,9 +65,9 @@ void run(const char* name, double wf_per_iter) {
         cudaEvent_t e0, e1;
         cudaEventCreate(&e0);
         cudaEventCreate(&e1);
-        k<MODE><<<148, warps * 32, sm>>>(out, 10);
+        k<MODE><<<132, warps * 32, sm>>>(out, 10);
         cudaEventRecord(e0);
-        k<MODE><<<148, warps * 32, sm>>>(out, iters);
+        k<MODE><<<132, warps * 32, sm>>>(out, iters);
         cudaEventRecord(e1);
         cudaEventSynchronize(e1);
         float ms;
