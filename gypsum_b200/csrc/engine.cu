@@ -107,11 +107,8 @@ struct gb200_engine {
     int64_t iq_samples = 0;
     int64_t launches = 0;
     size_t spec_budget_bytes = 512u << 20;
-    int np_override = 0, rsplit_override = 0;
-    int w2048 = 12;  // one-warp-per-transform correlate kernel: warps per CTA for single-ms searches (0 = use the pair kernel)
     bool timing = false;
     int fused = -1;  // acquire_cells kernel choice: -1 automatic, 0 doppler_spectra + correlate_cells, 1 fused block-per-cell
-    bool detect_fused = true;  // gb200_detect: fused block-per-cell kernel (every cell has its own Doppler)
     bool fused_configured = false;
     DevBuf<BestRecord> d_best;
     PinnedBuf<BestRecord> h_best;
@@ -269,32 +266,55 @@ struct TimedLaunch {
 
 int gcd_int(int a, int b) { return b ? gcd_int(b, a % b) : a; }
 
-// How many warp pairs share one cell.  With plenty of cells per pair each pair keeps a whole cell (no cross-pair
-// merge, no CTA-wide barrier); small launches split a cell's polyphase branches over pairs to fill the machine.
-int pick_rsplit(const gb200_engine* e, int np, long long n_cells) {
-    if (e->rsplit_override > 0 && e->s % e->rsplit_override == 0 && np % e->rsplit_override == 0) return e->rsplit_override;
-    if (n_cells >= 8LL * e->num_sms * np) return 1;
-    return gcd_int(e->s, np);
-}
-
-// Non-coherent, record-only launches use the one-warp-per-transform kernel: 12 warps per CTA (168 registers) for
-// single-millisecond searches, 8 warps (the 32 accumulators live across the milliseconds: 226 registers) for longer
-// integrations; the pair kernel keeps only the coherent and full-profile launches.
-// Returns the warps per CTA, or 0 for the pair kernel.  GB200_W2048=0 disables it, =10 runs single-ms searches with 10 warps.
-int pick_w2048(const gb200_engine* e, int M, int kind, bool profile) {
-    if (e->w2048 <= 0 || kind != GB200_NON_COHERENT || profile) return 0;
-    if (M == 1) return e->w2048 == 10 ? 10 : 12;
-    return 8;
-}
-
-// Warp pairs per CTA: 10 (20 warps / SM) for single-millisecond non-coherent searches, 8 otherwise (the
-// multi-millisecond accumulators need the larger register budget).  GB200_NP=8 forces the 8-pair build.
-int pick_np(const gb200_engine* e, int M, int kind, bool profile) {
-    if (e->np_override == 8) return 8;
-    return (M == 1 && kind == GB200_NON_COHERENT && !profile) ? 10 : 8;
+// How many of a CTA's slots (correlate_slots: warps or warp pairs) share one cell.  With plenty of cells per slot each
+// slot keeps a whole cell (no cross-slot merge, no CTA-wide barrier); small launches split a cell's polyphase branches
+// over slots to fill the machine.
+int pick_rsplit(const gb200_engine* e, int slots, long long n_cells) {
+    if (n_cells >= 8LL * e->num_sms * slots) return 1;
+    return gcd_int(e->s, slots);
 }
 
 size_t unit_floats2(const gb200_engine* e, int M) { return static_cast<size_t>(M) * e->s * 2 * kFft; }
+
+// doppler_spectra of n_units (block, Doppler) units, n_doppler per block, blocks of M milliseconds consecutive from iq.
+int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int n_doppler, int n_units) {
+    SpectraArgs sa{};
+    sa.iq = iq;
+    sa.doppler = dop;
+    sa.spec = e->spec.p;
+    sa.tw1 = e->tw1.p;
+    sa.tw2 = e->tw2.p;
+    sa.block_stride = static_cast<long long>(M) * e->N;
+    sa.inv_fs = 1.0 / static_cast<double>(e->fs);
+    sa.N = e->N;
+    sa.s = e->s;
+    sa.M = M;
+    sa.n_doppler = n_doppler;
+    sa.n_units = n_units;
+    {
+        TimedLaunch tl(e, 0);
+        GB_CUDA(e, launch_doppler_spectra(sa, e->stream));
+    }
+    e->launches++;
+    return GB200_OK;
+}
+
+// The correlate arguments every launch sets; the caller adds its grid- or list-mode plan.
+CorrelateArgs correlate_args(const gb200_engine* e, int M, int kind, int rsplit, CellRecord* records, float* profile) {
+    CorrelateArgs ca{};
+    ca.spec = e->spec.p;
+    ca.crep = e->crep.p;
+    ca.tw1 = e->tw1.p;
+    ca.tw2 = e->tw2.p;
+    ca.records = records;
+    ca.profile = profile;
+    ca.N = e->N;
+    ca.s = e->s;
+    ca.M = M;
+    ca.kind = kind;
+    ca.rsplit = rsplit;
+    return ca;
+}
 
 int check_common(gb200_engine* e, int n_ms, int kind) {
     if (!e) return GB200_EINVAL;
@@ -349,44 +369,16 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
     nb = std::min(nb, n_blocks);
     GB_CUDA(e, e->spec.ensure(per_block * nb));
 
-    const int nw = pick_w2048(e, M, kind, false);
-    const int np = nw ? nw : pick_np(e, M, kind, false);  // CTA "slots": warps (one-warp kernel) or warp pairs
-    const int rsplit = pick_rsplit(e, np, static_cast<long long>(nb) * P * D);
-    const int cpg = np / rsplit;
+    const int slots = correlate_slots(kind, M, false);
+    const int rsplit = pick_rsplit(e, slots, static_cast<long long>(nb) * P * D);
+    const int cpg = slots / rsplit;
     for (int b0 = 0; b0 < n_blocks; b0 += nb) {
         const int nbb = std::min(nb, n_blocks - b0);
         const int chunks = (nbb * D + cpg - 1) / cpg;  // groups per PRN: its nbb*D cells in chunks of cpg
-        SpectraArgs sa{};
-        sa.iq = e->iq + static_cast<size_t>(b0) * M * e->N;
-        sa.doppler = e->d_doppler.p;
-        sa.spec = e->spec.p;
-        sa.tw1 = e->tw1.p;
-        sa.tw2 = e->tw2.p;
-        sa.block_stride = static_cast<long long>(M) * e->N;
-        sa.inv_fs = 1.0 / static_cast<double>(e->fs);
-        sa.N = e->N;
-        sa.s = e->s;
-        sa.M = M;
-        sa.n_doppler = D;
-        sa.n_units = nbb * D;
-        {
-            TimedLaunch tl(e, 0);
-            GB_CUDA(e, launch_doppler_spectra(sa, e->stream));
-        }
-        e->launches++;
+        rc = run_spectra(e, e->iq + static_cast<size_t>(b0) * M * e->N, M, e->d_doppler.p, D, nbb * D);
+        if (rc) return rc;
 
-        CorrelateArgs ca{};
-        ca.spec = e->spec.p;
-        ca.crep = e->crep.p;
-        ca.tw1 = e->tw1.p;
-        ca.tw2 = e->tw2.p;
-        ca.records = rec_dev + static_cast<size_t>(b0) * P * D;
-        ca.profile = nullptr;
-        ca.N = e->N;
-        ca.s = e->s;
-        ca.M = M;
-        ca.kind = kind;
-        ca.rsplit = rsplit;
+        CorrelateArgs ca = correlate_args(e, M, kind, rsplit, rec_dev + static_cast<size_t>(b0) * P * D, nullptr);
         ca.n_groups = P * chunks;
         ca.grid_mode = 1;
         ca.P = P;
@@ -394,15 +386,14 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
         ca.n_blocks = nbb;
         ca.chunks = chunks;
         ca.prn_idx = e->d_ints.p;
-        ca.cell_probe = nullptr;
         const int grid = std::min(ca.n_groups, e->num_sms);
-        // L2 windows of the one-warp kernel (see the kernel): a batch whose spectra exceed L2 is walked in equal runs of units of
-        // about GB200_L2_WINDOW_MB (default kL2WindowMb; 0 = off), as long as a window still gives every CTA at least two groups
-        // (the kernel's round-robin of the extra groups keeps the CTAs together).
+        // L2 windows of the one-warp kernel (see the kernel; the pair kernel walks the batch as one window): a batch whose
+        // spectra exceed L2 is walked in equal runs of units of about GB200_L2_WINDOW_MB (default kL2WindowMb; 0 = off), as
+        // long as a window still gives every CTA at least two groups (the kernel's round-robin of the extra groups keeps the
+        // CTAs together).
         static const size_t win_bytes = static_cast<size_t>(std::max(0, env_int("GB200_L2_WINDOW_MB", kL2WindowMb))) << 20;
-        ca.win_chunks = 0;
         const size_t batch_bytes = static_cast<size_t>(nbb) * per_block * sizeof(float2);
-        if (nw && win_bytes && batch_bytes > win_bytes + win_bytes / 2) {
+        if (win_bytes && batch_bytes > win_bytes + win_bytes / 2) {
             const long long n_win = static_cast<long long>((batch_bytes + win_bytes - 1) / win_bytes);
             long long wc = (chunks + n_win - 1) / n_win;
             // a window whose P * wc groups divide evenly among the CTAs, when one exists within a quarter of the target size
@@ -420,8 +411,7 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
         }
         {
             TimedLaunch tl(e, 1);
-            if (nw) GB_CUDA(e, launch_correlate_w2048(ca, nw, grid, e->stream));
-            else GB_CUDA(e, launch_correlate_cells(ca, np, grid, e->stream));
+            GB_CUDA(e, launch_correlate(ca, grid, e->stream));
         }
         e->launches++;
     }
@@ -490,10 +480,9 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
         return GB200_OK;
     }
 
-    const int nw = pick_w2048(e, M, kind, profile_dev != nullptr);
-    const int np = nw ? nw : pick_np(e, M, kind, profile_dev != nullptr);
-    const int rsplit = pick_rsplit(e, np, n_cells);
-    const int cpg = np / rsplit;
+    const int slots = correlate_slots(kind, M, profile_dev != nullptr);
+    const int rsplit = pick_rsplit(e, slots, n_cells);
+    const int cpg = slots / rsplit;
     std::vector<int> order(n_cells);
     std::iota(order.begin(), order.end(), 0);
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return prn_idx[a] < prn_idx[b]; });
@@ -555,39 +544,11 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
         GB_CUDA(e, cudaMemcpyAsync(di, hi, sizeof(int) * (2 * nc + 3 * ng), cudaMemcpyHostToDevice, e->stream));
         GB_CUDA(e, cudaMemcpyAsync(e->d_doppler.p, e->h_doubles.p, sizeof(double) * nu, cudaMemcpyHostToDevice, e->stream));
 
-        SpectraArgs sa{};
-        sa.iq = e->iq;
-        sa.doppler = e->d_doppler.p;
-        sa.spec = e->spec.p;
-        sa.tw1 = e->tw1.p;
-        sa.tw2 = e->tw2.p;
-        sa.block_stride = 0;
-        sa.inv_fs = 1.0 / static_cast<double>(e->fs);
-        sa.N = e->N;
-        sa.s = e->s;
-        sa.M = M;
-        sa.n_doppler = nu;
-        sa.n_units = nu;
-        {
-            TimedLaunch tl(e, 0);
-            GB_CUDA(e, launch_doppler_spectra(sa, e->stream));
-        }
-        e->launches++;
+        rc = run_spectra(e, e->iq, M, e->d_doppler.p, nu, nu);
+        if (rc) return rc;
 
-        CorrelateArgs ca{};
-        ca.spec = e->spec.p;
-        ca.crep = e->crep.p;
-        ca.tw1 = e->tw1.p;
-        ca.tw2 = e->tw2.p;
-        ca.records = rec_dev;
-        ca.profile = profile_dev;
-        ca.N = e->N;
-        ca.s = e->s;
-        ca.M = M;
-        ca.kind = kind;
-        ca.rsplit = rsplit;
+        CorrelateArgs ca = correlate_args(e, M, kind, rsplit, rec_dev, profile_dev);
         ca.n_groups = ng;
-        ca.grid_mode = 0;
         ca.cell_u = di;
         ca.cell_out = di + nc;
         ca.grp_first = di + 2 * nc;
@@ -597,8 +558,7 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
         const int grid = std::min(ng, e->num_sms);
         {
             TimedLaunch tl(e, 1);
-            if (nw) GB_CUDA(e, launch_correlate_w2048(ca, nw, grid, e->stream));
-            else GB_CUDA(e, launch_correlate_cells(ca, np, grid, e->stream));
+            GB_CUDA(e, launch_correlate(ca, grid, e->stream));
         }
         e->launches++;
         c0 = c1;
@@ -658,10 +618,6 @@ int gb200_create(int device, int fs, int n, gb200_engine** out) {
     // Spectra scratch per launch pair.  It does not have to stay in L2 (a launch writes and re-reads 21 MB per 16.368 Msps
     // block), and launches that carry more cells run the correlate kernel without cross-warp merges and with a shorter tail.
     e->spec_budget_bytes = static_cast<size_t>(env_int("GB200_SPEC_BUDGET_MB", 512)) << 20;
-    e->np_override = env_int("GB200_NP", 0);
-    e->w2048 = env_int("GB200_W2048", 12);
-    e->rsplit_override = env_int("GB200_RSPLIT", 0);
-    e->detect_fused = env_int("GB200_DETECT_FUSED", 1) != 0;
     auto fail = [&](cudaError_t c, const char* what) {
         g_create_error = std::string(what) + ": " + cudaGetErrorString(c);
         cudaGetLastError();
@@ -824,8 +780,7 @@ int gb200_acquire_grid_host(gb200_engine* e, const float* iq_host, int n_blocks,
     GB_CUDA(e, cudaSetDevice(e->device));
     const size_t n_iq = static_cast<size_t>(n_blocks) * M * e->N, n_rec = static_cast<size_t>(n_blocks) * P * D;
     const size_t spec_bytes = unit_floats2(e, M) * D * sizeof(float2) * n_blocks;
-    static const bool graphs = env_int("GB200_GRAPH", 1) != 0;
-    if (!graphs || e->timing || spec_bytes > e->spec_budget_bytes) {  // several scratch batches / per-kernel events: plain path
+    if (e->timing || spec_bytes > e->spec_budget_bytes) {  // several scratch batches / per-kernel events: plain path
         int rc = gb200_upload_iq(e, iq_host, static_cast<int64_t>(n_iq));
         if (rc) return rc;
         return gb200_acquire_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, out_host);
@@ -1133,10 +1088,9 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
 
     const int MAXB = kRefineMaxBins;
     const int n_cells = n_sv * MAXB;
-    const int nw = pick_w2048(e, n_ms, GB200_NON_COHERENT, false);
-    const int np = nw ? nw : pick_np(e, n_ms, GB200_NON_COHERENT, false);
-    const int rsplit = pick_rsplit(e, np, n_cells);
-    const int cpg = np / rsplit;
+    const int slots = correlate_slots(GB200_NON_COHERENT, n_ms, false);
+    const int rsplit = pick_rsplit(e, slots, n_cells);
+    const int cpg = slots / rsplit;
     const int gps = (MAXB + cpg - 1) / cpg;  // groups per satellite
     const size_t unit = unit_floats2(e, n_ms);
     int sv_per_chunk = static_cast<int>(std::max<size_t>(1, e->spec_budget_bytes / (unit * sizeof(float2) * MAXB)));
@@ -1190,39 +1144,9 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
     double* d_coh_doppler = e->r_doppler.p + n_cells;
     CellRecord* d_coh_records = e->r_records.p + n_cells;
 
-    auto spectra = [&](const double* dop, int n_units) -> cudaError_t {
-        SpectraArgs sa{};
-        sa.iq = e->iq;
-        sa.doppler = dop;
-        sa.spec = e->spec.p;
-        sa.tw1 = e->tw1.p;
-        sa.tw2 = e->tw2.p;
-        sa.block_stride = 0;
-        sa.inv_fs = 1.0 / static_cast<double>(e->fs);
-        sa.N = e->N;
-        sa.s = e->s;
-        sa.M = n_ms;
-        sa.n_doppler = n_units;
-        sa.n_units = n_units;
-        TimedLaunch tl(e, 0);
-        e->launches++;
-        return launch_doppler_spectra(sa, e->stream);
-    };
-    CorrelateArgs base{};
-    base.spec = e->spec.p;
-    base.crep = e->crep.p;
-    base.tw1 = e->tw1.p;
-    base.tw2 = e->tw2.p;
-    base.profile = nullptr;
-    base.N = e->N;
-    base.s = e->s;
-    base.M = n_ms;
-    base.rsplit = rsplit;
-    base.grid_mode = 0;
-
     // Every (satellite, bin) cell of a refinement pass has its own Doppler, so nothing is shared between PRNs: the
     // fused block-per-cell kernel does the same arithmetic without the spectra round trip through HBM.
-    const bool use_fused = fused_supports(e->s) && e->detect_fused;
+    const bool use_fused = fused_supports(e->s);
     FusedArgs fbase{};
     const int* d_cell_prn = nullptr;
     if (use_fused) {
@@ -1268,22 +1192,19 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
         }
         for (int sv0 = 0; !use_fused && sv0 < n_sv; sv0 += sv_per_chunk) {
             const int nsv = std::min(sv_per_chunk, n_sv - sv0);
-            GB_CUDA(e, spectra(e->r_doppler.p + static_cast<size_t>(sv0) * MAXB, nsv * MAXB));
-            CorrelateArgs ca = base;
-            ca.records = e->r_records.p;
-            ca.kind = GB200_NON_COHERENT;
+            rc = run_spectra(e, e->iq, n_ms, e->r_doppler.p + static_cast<size_t>(sv0) * MAXB, nsv * MAXB, nsv * MAXB);
+            if (rc) return rc;
+            CorrelateArgs ca = correlate_args(e, n_ms, GB200_NON_COHERENT, rsplit, e->r_records.p, nullptr);
             ca.n_groups = nsv * gps;
             ca.cell_u = di;
             ca.cell_out = di + n_cells;
             ca.grp_first = di + 2 * n_cells + sv0 * gps;
             ca.grp_count = di + 2 * n_cells + ng + sv0 * gps;
             ca.grp_prn = di + 2 * n_cells + 2 * ng + sv0 * gps;
-            ca.cell_probe = nullptr;
             ca.cell_gate = e->r_doppler.p;
             {
                 TimedLaunch tl(e, 1);
-                if (nw) GB_CUDA(e, launch_correlate_w2048(ca, nw, std::min(ca.n_groups, e->num_sms), e->stream));
-                else GB_CUDA(e, launch_correlate_cells(ca, np, std::min(ca.n_groups, e->num_sms), e->stream));
+                GB_CUDA(e, launch_correlate(ca, std::min(ca.n_groups, e->num_sms), e->stream));
             }
             e->launches++;
         }
@@ -1306,14 +1227,11 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
         }
         e->launches++;
     } else {
-        GB_CUDA(e, spectra(d_coh_doppler, n_sv));
-    }
-    if (!use_fused) {
+        rc = run_spectra(e, e->iq, n_ms, d_coh_doppler, n_sv, n_sv);
+        if (rc) return rc;
         const int* cbase = di + 2 * n_cells + 3 * ng;
-        CorrelateArgs ca = base;
-        ca.records = d_coh_records;
-        ca.kind = GB200_COHERENT;
-        ca.rsplit = pick_rsplit(e, 8, n_sv);  // the coherent pass always runs on the 8-pair build
+        const int crsplit = pick_rsplit(e, correlate_slots(GB200_COHERENT, n_ms, false), n_sv);
+        CorrelateArgs ca = correlate_args(e, n_ms, GB200_COHERENT, crsplit, d_coh_records, nullptr);
         ca.n_groups = n_sv;
         ca.cell_u = cbase;
         ca.cell_out = cbase + n_sv;
@@ -1321,9 +1239,10 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
         ca.grp_count = cbase + 3 * n_sv;
         ca.grp_prn = cbase + 4 * n_sv;
         ca.cell_probe = d_probe;
-        ca.cell_gate = nullptr;
-        TimedLaunch tl(e, 1);
-        GB_CUDA(e, launch_correlate_cells(ca, 8, std::min(n_sv, e->num_sms), e->stream));
+        {
+            TimedLaunch tl(e, 1);
+            GB_CUDA(e, launch_correlate(ca, std::min(n_sv, e->num_sms), e->stream));
+        }
         e->launches++;
     }
     GB_CUDA(e, launch_refine_finalize(n_sv, e->r_state.p, d_coh_records, e->r_results.p, e->stream));

@@ -7,12 +7,10 @@
 //   correlate_cells   per (PRN, Doppler) cell: x conj(FFT(replica)) (utils.py:69, spectrum staged into shared
 //                     memory with a TMA bulk copy), inverse warp FFTs (utils.py:73), |.| accumulation over ms
 //                     (utils.py:102-104) in registers, peak/argmax/sum/count reduction with REDUX / warp shuffles
-//                     (acquisition.py:181-189, utils.py:111-116).  Two builds: k_correlate_cells (a warp pair per
-//                     transform pair; multi-ms, coherent, profile) and k_correlate_w2048 (one warp per pruned
-//                     inverse FFT-2048; single-ms searches).
+//                     (acquisition.py:181-189, utils.py:111-116).  Two kernels, chosen by launch_correlate:
+//                     k_correlate_w2048 (one warp per pruned inverse FFT-2048; every non-coherent, record-only launch)
+//                     and k_correlate_cells (a warp pair per transform pair; coherent launches, probes, full profiles).
 //   refine_*          planning / selection kernels of the on-device search (acquisition.py:70-152).
-#include <cstdlib>
-
 #include "kernels.cuh"
 #include "ptx_helpers.cuh"
 #include "warp_fft.cuh"
@@ -180,15 +178,17 @@ __device__ __forceinline__ void warp_reduce_peak(Peak& p) {
     for (int off = 16; off > 0; off >>= 1) p.sum += __shfl_xor_sync(0xffffffffu, p.sum, off);
 }
 
-template <int NP, int KIND, bool PROFILE>
-__global__ void __launch_bounds__(NP * 64, 1) k_correlate_cells(const CorrelateArgs a) {
+constexpr int kPairs = 8;  // warp pairs per k_correlate_cells CTA
+
+template <int KIND, bool PROFILE>
+__global__ void __launch_bounds__(kPairs * 64, 1) k_correlate_cells(const CorrelateArgs a) {
     extern __shared__ __align__(16) float2 smem[];
     float2* crep_s = smem;                 // [2][1024]
     float2* tw1_s = crep_s + 2 * kFft;     // [32][32]
     float2* tw2_s = tw1_s + kFft;          // [1024]
-    float2* tiles = tw2_s + kFft;          // [2*NP][kTileF2]
-    PairPartial* partial = reinterpret_cast<PairPartial*>(tiles + 2 * NP * kTileF2);  // [2*NP]
-    uint64_t* mbar = reinterpret_cast<uint64_t*>(partial + 2 * NP);
+    float2* tiles = tw2_s + kFft;          // [2*kPairs][kTileF2]
+    PairPartial* partial = reinterpret_cast<PairPartial*>(tiles + 2 * kPairs * kTileF2);  // [2*kPairs]
+    uint64_t* mbar = reinterpret_cast<uint64_t*>(partial + 2 * kPairs);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int pair = warp >> 1, h = warp & 1;
@@ -205,7 +205,7 @@ __global__ void __launch_bounds__(NP * 64, 1) k_correlate_cells(const CorrelateA
     }
     mbar_wait(mbar, parity);
     parity ^= 1;
-    const int cells_per_group = NP / a.rsplit;
+    const int cells_per_group = kPairs / a.rsplit;
     const int r_per_pair = a.s / a.rsplit;
     const int my_cell = pair / a.rsplit;  // cell slot inside the group
     const int my_r0 = (pair % a.rsplit) * r_per_pair;
@@ -278,9 +278,7 @@ __global__ void __launch_bounds__(NP * 64, 1) k_correlate_cells(const CorrelateA
                 float acc[16];
 #pragma unroll
                 for (int jj = 0; jj < 16; ++jj) acc[jj] = 0.f;
-                // The 10-pair build (20 warps / SM, 96 registers) is only launched for single-millisecond non-coherent work:
-                // with the trip count known the accumulators are not live across the transform and nothing spills.
-                const int n_iter = (KIND == kKindCoherent || NP == 10) ? 1 : a.M;
+                const int n_iter = KIND == kKindCoherent ? 1 : a.M;
                 for (int it = 0; it < n_iter; ++it) {
                     float2 x[32];
                     if (KIND == kKindCoherent) {
@@ -433,7 +431,7 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
     }
     mbar_wait(mbar, parity);
     parity ^= 1;
-    asm volatile("griddepcontrol.wait;" ::: "memory");  // see k_correlate_cells: PDL against doppler_spectra
+    asm volatile("griddepcontrol.wait;" ::: "memory");  // PDL against doppler_spectra, see launch_correlate
 
     const int cells_per_group = NW / a.rsplit;
     const int r_per_warp = a.s / a.rsplit;
@@ -799,8 +797,8 @@ cudaError_t launch_refine_finalize(int n_sv, const RefineState* st, const CellRe
 size_t spectra_smem_bytes(int s) {
     return (static_cast<size_t>(spec_f2(s)) + kCarrierTable) * sizeof(float2);
 }
-size_t correlate_smem_bytes(int np) {
-    return (4 * static_cast<size_t>(kFft) + 2 * np * kTileF2) * sizeof(float2) + 2 * np * sizeof(PairPartial) + 16;
+size_t correlate_smem_bytes() {
+    return (4 * static_cast<size_t>(kFft) + 2 * kPairs * kTileF2) * sizeof(float2) + 2 * kPairs * sizeof(PairPartial) + 16;
 }
 
 size_t correlate_w2048_smem_bytes(int nw) {
@@ -820,26 +818,15 @@ static cudaError_t spectra_attr() {
     return cudaFuncSetAttribute(k_doppler_spectra<S>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(spectra_smem_bytes(S)));
 }
-template <int NP>
-static cudaError_t correlate_attr() {
-    const int sm = static_cast<int>(correlate_smem_bytes(NP));
-    cudaError_t e;
-    if ((e = cudaFuncSetAttribute(k_correlate_cells<NP, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm))) return e;
-    if ((e = cudaFuncSetAttribute(k_correlate_cells<NP, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm))) return e;
-    if ((e = cudaFuncSetAttribute(k_correlate_cells<NP, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm))) return e;
-    return cudaFuncSetAttribute(k_correlate_cells<NP, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm);
-}
-
 cudaError_t configure_kernels() {
     cudaError_t e;
 #define GB_ATTR(S) if ((e = spectra_attr<S>()) != cudaSuccess) return e;
     GB_ATTR(1) GB_ATTR(2) GB_ATTR(3) GB_ATTR(4) GB_ATTR(5) GB_ATTR(6) GB_ATTR(8) GB_ATTR(10) GB_ATTR(12) GB_ATTR(16)
 #undef GB_ATTR
-    if ((e = correlate_attr<8>()) != cudaSuccess) return e;
-    if ((e = correlate_attr<10>()) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_correlate_w2048<10, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(correlate_w2048_smem_bytes(10)))) != cudaSuccess)
-        return e;
+    const int sm = static_cast<int>(correlate_smem_bytes());
+    if ((e = cudaFuncSetAttribute(k_correlate_cells<kKindCoherent, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm))) return e;
+    if ((e = cudaFuncSetAttribute(k_correlate_cells<kKindCoherent, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm))) return e;
+    if ((e = cudaFuncSetAttribute(k_correlate_cells<kKindNonCoherent, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm))) return e;
     if ((e = cudaFuncSetAttribute(k_correlate_w2048<12, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(correlate_w2048_smem_bytes(12)))) != cudaSuccess)
         return e;
@@ -867,8 +854,21 @@ cudaError_t launch_doppler_spectra(const SpectraArgs& a, cudaStream_t st) {
     return cudaGetLastError();
 }
 
+// Start stagger of the one-warp kernel's warps after each replica re-stage, in ns: (warp / 4) * row + (warp % 4) * column.
+constexpr int kW2048StaggerRowNs = 600, kW2048StaggerColNs = 150;
+
+// Coherent launches, coherent probes and full profiles need the pair kernel; every other launch takes the one-warp kernel,
+// which is faster on every record-only shape measured on the H100 (DESIGN.md §4).
+static bool pair_kernel(int kind, bool profile) { return kind == kKindCoherent || profile; }
+
+int correlate_slots(int kind, int M, bool profile) {
+    if (pair_kernel(kind, profile)) return kPairs;
+    return M == 1 ? 12 : 8;  // 8 warps when the 32 accumulators live across the milliseconds
+}
+
 // Launch as a programmatic dependent of the previous kernel in the stream (doppler_spectra): the grid may start its
-// prologue while the producer drains; it blocks at griddepcontrol.wait until the producer's writes are visible.
+// prologue while the producer drains; it blocks at griddepcontrol.wait until the producer's writes are visible.  Only
+// k_correlate_w2048 executes that wait, so only it may be launched this way.
 template <class K>
 static void launch_dependent(K kernel, const CorrelateArgs& a, int grid, int block, size_t sm, cudaStream_t st) {
     cudaLaunchConfig_t cfg{};
@@ -880,39 +880,23 @@ static void launch_dependent(K kernel, const CorrelateArgs& a, int grid, int blo
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    static const bool pdl = !(getenv("GB200_PDL") && atoi(getenv("GB200_PDL")) == 0);
-    cfg.numAttrs = pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     cudaLaunchKernelEx(&cfg, kernel, a);
 }
 
-template <int NP>
-static void correlate_dispatch(const CorrelateArgs& a, int grid, cudaStream_t st) {
-    const size_t sm = correlate_smem_bytes(NP);
-    const bool prof = a.profile != nullptr;
-    if (a.kind == kKindCoherent) {
-        if (prof) launch_dependent(k_correlate_cells<NP, 1, true>, a, grid, NP * 64, sm, st);
-        else launch_dependent(k_correlate_cells<NP, 1, false>, a, grid, NP * 64, sm, st);
-    } else {
-        if (prof) launch_dependent(k_correlate_cells<NP, 2, true>, a, grid, NP * 64, sm, st);
-        else launch_dependent(k_correlate_cells<NP, 2, false>, a, grid, NP * 64, sm, st);
+cudaError_t launch_correlate(const CorrelateArgs& a0, int grid, cudaStream_t st) {
+    if (pair_kernel(a0.kind, a0.profile != nullptr)) {
+        const size_t sm = correlate_smem_bytes();
+        if (a0.kind != kKindCoherent) k_correlate_cells<kKindNonCoherent, true><<<grid, kPairs * 64, sm, st>>>(a0);
+        else if (a0.profile) k_correlate_cells<kKindCoherent, true><<<grid, kPairs * 64, sm, st>>>(a0);
+        else k_correlate_cells<kKindCoherent, false><<<grid, kPairs * 64, sm, st>>>(a0);
+        return cudaGetLastError();
     }
-}
-// One-warp-per-transform build: nw = 10 warps needs M == 1 (the caller guarantees it), nw = 8 takes any M.
-cudaError_t launch_correlate_w2048(const CorrelateArgs& a0, int nw, int grid, cudaStream_t st) {
-    static const int stag_a = [] { const char* v = getenv("GB200_STAGGER_A"); return v ? atoi(v) : 600; }();
-    static const int stag_b = [] { const char* v = getenv("GB200_STAGGER_B"); return v ? atoi(v) : 150; }();
     CorrelateArgs a = a0;
-    a.stag_a = stag_a;
-    a.stag_b = stag_b;
-    if (nw == 12) launch_dependent(k_correlate_w2048<12, true>, a, grid, 384, correlate_w2048_smem_bytes(12), st);
-    else if (nw == 10) launch_dependent(k_correlate_w2048<10, true>, a, grid, 320, correlate_w2048_smem_bytes(10), st);
-    else launch_dependent(k_correlate_w2048<8, false>, a, grid, 256, correlate_w2048_smem_bytes(8), st);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_correlate_cells(const CorrelateArgs& a, int np, int grid, cudaStream_t st) {
-    if (np == 10) correlate_dispatch<10>(a, grid, st);
-    else correlate_dispatch<8>(a, grid, st);
+    a.stag_a = kW2048StaggerRowNs;
+    a.stag_b = kW2048StaggerColNs;
+    if (a.M == 1) launch_dependent(k_correlate_w2048<12, true>, a, grid, 12 * 32, correlate_w2048_smem_bytes(12), st);
+    else launch_dependent(k_correlate_w2048<8, false>, a, grid, 8 * 32, correlate_w2048_smem_bytes(8), st);
     return cudaGetLastError();
 }
 

@@ -20,7 +20,8 @@ struct SpectraArgs {
     int N, s, M, n_doppler, n_units;  // n_units = n_blocks * n_doppler
 };
 
-// correlate_cells: one warp pair per (cell, r-range); NP pairs per CTA all on the same PRN.
+// correlate_cells: one warp (k_correlate_w2048) or warp pair (k_correlate_cells) per (cell, r-range); every slot of a CTA
+// works on the same PRN.
 struct CorrelateArgs {
     const float2* spec;
     const float2* crep;  // [n_prn][2][1024]  conj(FFT2048(c'))/2048, even / odd bins
@@ -29,7 +30,7 @@ struct CorrelateArgs {
     CellRecord* records;
     float* profile;      // optional: full profile of the single cell (N floats, or 2N when coherent)
     int N, s, M, kind;
-    int rsplit;          // pairs cooperating on one cell (divides s and NP)
+    int rsplit;          // slots cooperating on one cell (divides s and correlate_slots)
     int n_groups;
     // grid mode (cells = blocks x prn list x doppler list)
     int grid_mode, P, D, n_blocks, chunks;  // chunks = ceil(n_blocks * D / cells_per_group): groups per PRN
@@ -42,7 +43,7 @@ struct CorrelateArgs {
     const int* cell_u;      // spectrum unit of each sorted cell
     const int* cell_out;    // where its record goes
     const int* cell_probe;  // coherent probe index or -1 (both modes, indexed by output slot; may be null)
-    int stag_a, stag_b;       // k_correlate_w2048 start stagger in ns: (warp / 4) * stag_a + (warp % 4) * stag_b
+    int stag_a, stag_b;       // k_correlate_w2048 start stagger in ns: (warp / 4) * stag_a + (warp % 4) * stag_b (set by launch_correlate)
     const double* cell_gate;  // optional, indexed by output slot: NaN = this cell is switched off (device-planned lists)
 };
 
@@ -131,12 +132,14 @@ cudaError_t launch_track_channels(const TrackArgs& a, cudaStream_t st);
 cudaError_t launch_integrate_bits(const BitArgs& a, cudaStream_t st);
 size_t spectra_smem_bytes(int s);
 bool spectra_supports(int s);
-size_t correlate_smem_bytes(int np);
 cudaError_t launch_init_tables(float2* tw1, float2* tw2, cudaStream_t st);
 cudaError_t launch_replica_spectra(const uint8_t* chips_dev, int n_prn, float2* crep, cudaStream_t st);
 cudaError_t launch_doppler_spectra(const SpectraArgs& a, cudaStream_t st);
-cudaError_t launch_correlate_cells(const CorrelateArgs& a, int np, int grid, cudaStream_t st);
-cudaError_t launch_correlate_w2048(const CorrelateArgs& a, int nw, int grid, cudaStream_t st);
+// Slots per CTA of the correlate kernel that runs a launch of this kind, M milliseconds and profile output: warps of the
+// one-warp-per-transform kernel, or warp pairs of the pair kernel.  rsplit must divide it.
+int correlate_slots(int kind, int M, bool profile);
+// Runs the kernel correlate_slots(a.kind, a.M, a.profile != nullptr) describes.
+cudaError_t launch_correlate(const CorrelateArgs& a, int grid, cudaStream_t st);
 cudaError_t launch_correlate_generic(const float2* iq, const float2* replica, int N, int n_ms, double doppler, double inv_fs,
                                      int kind, float* out, cudaStream_t st);
 cudaError_t configure_kernels();

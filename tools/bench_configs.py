@@ -129,7 +129,8 @@ def detector_case():
         found = det.detect_satellites_in_antenna_data(ids, x, A)
         ts.append(time.perf_counter() - t0)
     print(json.dumps({"workload": "real detector: 32 SV x 10 passes (222 bins) + coherent, 10 ms @ 2.046 Msps",
-                      "detect_kernel": os.environ.get("GB200_DETECT_FUSED", "1") != "0" and "fused" or "split",
+                      # gb200_detect takes the fused kernel at 2.046 and 4.092 Msps, the split kernels at other rates
+                      "detect_kernel": "fused" if A.samples_per_prn_transmission in (2046, 4092) else "split",
                       "seconds_per_scan": float(np.median(ts)), "cell_ms_per_scan": 32 * 223 * 10,
                       "found": [[r.satellite_id.id, r.doppler_shift, r.prn_phase_shift] for r in found]}), flush=True)
 

@@ -1,4 +1,4 @@
-"""Single-block host-to-host latency of the config-2 grid, by entry point (A/B aid: GB200_GRAPH=0/1)."""
+"""Single-block host-to-host latency of the config-2 grid, by entry point."""
 import os
 import sys
 import time
@@ -46,7 +46,7 @@ def two_calls(k):
     eng.acquire_grid(1, 1, prn, dop, 2, out=out)
 
 
-print("graph env", os.environ.get("GB200_GRAPH", "1"), "acquire_grid_host us", med(host_call), "with a pinned record buffer us", med(host_call_pinned),
+print("acquire_grid_host us", med(host_call), "with a pinned record buffer us", med(host_call_pinned),
       "upload+acquire_grid us", med(two_calls))
 host_call(0)
 assert out_pinned.tobytes() != out.tobytes() or True

@@ -1,5 +1,5 @@
 """One line for config 3 (32x41x10 ms @ 4.092 Msps, one window per call) and the config-5 shape: device ms and per-kernel ms.
-A/B aid: GB200_W2048=8 python tools/quick_cfg3.py"""
+A/B aid: GB200_LIB=... python tools/quick_cfg3.py"""
 import sys
 
 sys.argv = ["x"]

@@ -1,5 +1,5 @@
-"""One line for the headline grid (config 2 x 32 blocks): device ms and per-kernel ms.  Used for A/B runs of env knobs /
-experiment builds: GB200_LIB=... GB200_STAGGER_A=... python tools/quick_grid.py"""
+"""One line for the headline grid (config 2 x 32 blocks): device ms and per-kernel ms.  Used for A/B runs of experiment
+builds: GB200_LIB=... python tools/quick_grid.py"""
 import sys
 
 sys.argv = ["x"]

@@ -25,7 +25,7 @@ for n, m in ((2046, 2), (4092, 1)):
     p = eng.correlation_profile(24, 1500.0, m, _native.NON_COHERENT)
     assert int(p.argmax()) == 777 % n == int(g["argmax"][0, 0, 7])
     if n == 2046:
-        big = eng.acquire_grid(2, 1, np.arange(32), np.linspace(-10000, 10000, 161))  # whole-cell-per-pair path, 10-pair build
+        big = eng.acquire_grid(2, 1, np.arange(32), np.linspace(-10000, 10000, 161))  # full 32-PRN grid, 12-warp one-warp build
         r = eng.detect([24, 2], m)
         assert int(big["argmax"][0, 24, int(np.argmax(big["peak"][0, 24]))]) == 777 and int(r["code_phase"][0]) == 777
         xs = to.synth_tracking_iq(3, n, 12, fs, [(25, 1500.3, 0.0, 777, 0.3, 0.004)])
