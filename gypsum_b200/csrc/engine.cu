@@ -1262,7 +1262,6 @@ int gb200_tracker_create(gb200_engine* e, int n_channels, const int32_t* prn_idx
     if (!out) GB_FAIL(e, GB200_EINVAL, "null output");
     *out = nullptr;
     if (n_channels < 1 || !prn_idx || !doppler_hz || !carrier_phase || !code_phase) GB_FAIL(e, GB200_EINVAL, "no channels");
-    if (e->s != 2 && e->s != 4) GB_FAIL(e, GB200_EINVAL, "tracking needs 2046 or 4092 samples per ms (reference tracker.py:301 hard-wires 2046)");
     if (e->n_prn == 0) GB_FAIL(e, GB200_ESTATE, "no PRN replicas loaded (gb200_set_replicas)");
     for (int c = 0; c < n_channels; ++c)
         if (prn_idx[c] < 0 || prn_idx[c] >= e->n_prn) GB_FAIL(e, GB200_EINVAL, "prn index %d out of range", prn_idx[c]);
@@ -1447,7 +1446,6 @@ int gb200_tracker_create_pool(gb200_engine* e, int capacity, gb200_tracker** out
     if (!out) GB_FAIL(e, GB200_EINVAL, "null output");
     *out = nullptr;
     if (capacity < 1) GB_FAIL(e, GB200_EINVAL, "no channels");
-    if (e->s != 2 && e->s != 4) GB_FAIL(e, GB200_EINVAL, "tracking needs 2046 or 4092 samples per ms (reference tracker.py:301 hard-wires 2046)");
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_CUDA(e, configure_track_kernel());
     gb200_tracker* t = new gb200_tracker;

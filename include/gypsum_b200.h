@@ -177,7 +177,9 @@ typedef struct gb200_track_record {
 } gb200_track_record;
 
 /* satellite_signal_processing_pipeline.py:56-63: one channel per (replica row, Doppler, carrier phase, code
- * phase).  Needs samples_per_ms == 2046 or 4092 (the reference hard-wires 2046, tracker.py:301-303,319).     */
+ * phase).  Works at every rate gb200_create accepts (samples_per_ms / 1023 in {1, 2, 3, 4, 5, 6, 8, 10, 12,
+ * 16}).  Like the reference, the code-phase accumulator wraps at 2046 and the pseudosymbol delay is code phase /
+ * 2046 ms at every rate (tracker.py:301-303,319): above 2.046 Msps only code phases below 2046 can be kept.     */
 int gb200_tracker_create(gb200_engine* e, int n_channels, const int32_t* prn_idx, const double* doppler_hz,
                          const double* carrier_phase, const int32_t* code_phase, gb200_tracker** out);
 int gb200_tracker_destroy(gb200_tracker* t);

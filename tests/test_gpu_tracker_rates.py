@@ -1,0 +1,265 @@
+"""GPU tracking at every rate the engine acquires at other than 2.046 / 4.092 Msps: k_track_channels at S = 1, 3 and
+k_track_channels_wide at S = 5 .. 16 (tracker.cu), against the tracker oracle and the live reference's trajectories
+(tests/golden/tracker_fs1/fs8/fs16/fs16_long.npz).  Same tolerances as tests/test_gpu_tracker.py."""
+import os
+import subprocess
+import sys
+
+import numpy as np
+import pytest
+
+from oracle import gypsum_oracle as o
+from oracle import tracker_oracle as t
+
+pytestmark = pytest.mark.gpu
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+GOLDEN = os.path.join(ROOT, "tests", "golden")
+RATES = [1, 3, 5, 6, 8, 10, 12, 16]
+N16, FS16 = 16368, 16368000
+
+_FIRST_RUN_SCRIPT = r"""
+import sys
+import numpy as np
+sys.path.insert(0, sys.argv[1])
+from gypsum_b200 import _native
+from oracle import gypsum_oracle as o
+from oracle import tracker_oracle as t
+
+for s in (1, 3, 5, 16):
+    n, fs = 1023 * s, 1023000 * s
+    x = t.synth_tracking_iq(7, n, 20, fs, [(12, 640.4, 0.0, 1501, 0.7, 0.004)])
+    eng = _native.Engine(fs, n)
+    eng.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
+    eng.upload_iq(x)
+    trk = _native.Tracker(eng, [11], [640.0], [0.0], [1501])
+    rec = trk.process(20, np.array([t.chunk_times(k, fs, n)[0] for k in range(20)]))[0]
+    tr = t.TrackerOracle(12, 640.0, 0.0, 1501, fs, n)
+    want = [tr.step(x[k * n:(k + 1) * n], *t.chunk_times(k, fs, n))["symbol"] for k in range(20)]
+    assert not rec["lost"].any() and list(rec["symbol"]) == want, s
+    trk.close()
+    eng.close()
+print("rates ok")
+"""
+
+
+def test_first_run_of_the_new_instantiations_in_a_child_process(native_lib):
+    """Runs first, in its own process, so that a fault in a never-exercised kernel cannot disturb the CUDA context of
+    the tests below."""
+    proc = subprocess.run([sys.executable, "-c", _FIRST_RUN_SCRIPT, ROOT], capture_output=True, text=True, timeout=600)
+    assert proc.returncode == 0 and "rates ok" in proc.stdout, proc.stderr[-2000:]
+
+
+_ENGINES = {}
+
+
+def engine_for(s):
+    from gypsum_b200 import _native
+
+    if s not in _ENGINES:
+        e = _native.Engine(1023000 * s, 1023 * s)
+        e.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
+        _ENGINES[s] = e
+    return _ENGINES[s]
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _close_engines():
+    yield
+    for e in _ENGINES.values():
+        e.close()
+    _ENGINES.clear()
+
+
+def times(n_ms, fs, n):
+    return np.array([t.chunk_times(k, fs, n)[0] for k in range(n_ms)])
+
+
+@pytest.mark.parametrize("s", RATES)
+def test_teacher_forced_correlators_at_every_rate(native_lib, s):
+    """Each millisecond starts from the oracle's loop state: early / late / prompt outputs and the updated state."""
+    from gypsum_b200 import _native
+
+    n, fs = 1023 * s, 1023000 * s
+    amp = 0.004 if s < 8 else 0.002
+    x = t.synth_tracking_iq(100 + s, n, 60, fs, [(25, 1500.3, 0.0, 777, 0.3, amp)])
+    tr = t.TrackerOracle(25, 1500.0, 0.0, 777, fs, n)
+    eng = engine_for(s)
+    trk = _native.Tracker(eng, [24], [1500.0], [0.0], [777])
+    for k in range(60):
+        a, b = t.chunk_times(k, fs, n)
+        trk.set_state(0, tr.doppler, tr.carrier_phase, float(tr.phase), tr.code_phase)
+        eng.upload_iq(x[k * n:(k + 1) * n])
+        rec = trk.process(1, [a])[0, 0]
+        r = tr.step(x[k * n:(k + 1) * n], a, b)
+        scale = abs(r["peak"])
+        assert abs(complex(rec["peak_re"], rec["peak_im"]) - r["peak"]) <= 1e-5 * scale, k
+        assert abs(complex(rec["early_re"], rec["early_im"]) - r["early"]) <= 1e-5 * scale, k
+        assert abs(complex(rec["late_re"], rec["late_im"]) - r["late"]) <= 1e-5 * scale, k
+        assert abs(rec["strength"] - r["strength"]) <= 1e-4 * r["strength"], k
+        assert rec["peak_offset"] == r["peak_offset"] and rec["symbol"] == r["symbol"], k
+        assert rec["code_phase"] == r["code_phase"], k
+        assert abs(rec["disc"] - r["disc"]) <= 1e-4 * max(1.0, abs(r["disc"])), k
+        assert abs(rec["error"] - r["error"]) <= 1e-4 * max(1.0, abs(r["error"])), k
+    trk.close()
+
+
+def load_case(name):
+    z = np.load(os.path.join(GOLDEN, f"tracker_{name}.npz"))
+    ch = z["channel"]
+    ch = (int(ch[0]), ch[1], ch[2], int(ch[3]), ch[4], ch[5])
+    n, fs = int(z["n"]), int(z["fs"])
+    x = t.synth_tracking_iq(int(z["seed"]), n, int(z["n_ms"]), fs, [ch], float(z["sigma"]))
+    return z, ch, x, n, fs
+
+
+@pytest.mark.parametrize("name", ["fs1", "fs8", "fs16", "fs16_long"])
+def test_free_running_matches_reference_at_other_rates(native_lib, name):
+    from gypsum_b200 import _native
+    from test_gpu_tracker import assert_symbols_and_code_phase_follow_reference
+
+    z, ch, x, n, fs = load_case(name)
+    init, rows = z["init"], z["rows"]
+    n_ms = len(rows)
+    eng = engine_for(n // 1023)
+    trk = _native.Tracker(eng, [ch[0] - 1], [init[0]], [init[1]], [int(init[2])])
+    eng.upload_iq(x)
+    rec = trk.process(n_ms, times(n_ms, fs, n))[0]
+    trk.close()
+    assert not rec["lost"].any()
+    assert_symbols_and_code_phase_follow_reference(rec, rows)
+    assert np.abs(rec["doppler"] - rows[:, 6]).max() <= 5e-3
+    d = np.abs(rec["carrier_phase"] - rows[:, 7])
+    assert np.minimum(d, 2 * np.pi - d).max() <= 2e-3
+    assert np.abs(rec["doppler_hist"] - rows[:, 12]).max() <= 5e-3
+    assert np.array_equal(rec["doppler"] != rec["doppler_hist"], rows[:, 6] != rows[:, 12])
+    if name == "fs16":  # sigma 0.01: the reference reaches is_locked(); the device decides the same milliseconds
+        tr = t.TrackerOracle(ch[0], init[0], init[1], int(init[2]), fs, n)
+        want = np.array([tr.step(x[k * n:(k + 1) * n], *t.chunk_times(k, fs, n))["locked"] for k in range(n_ms)])
+        assert want.sum() > 0 and rec["locked"].sum() > 0
+        assert np.count_nonzero(rec["locked"].astype(bool) != want) <= n_ms // 200
+    if name == "fs16_long":  # sigma 0.02: never locked (I-pole variance ~ sigma^2 N / 2 > 2); the 6-s check passes
+        assert n_ms > 6000 and rec["locked"].sum() == 0
+
+
+def test_bank_and_profile_at_16368_ksps(native_lib):
+    """Several channels over one stream == each channel alone; |prompt profile| matches the oracle."""
+    from gypsum_b200 import _native
+
+    chans = [(25, 1500.3, 0.0, 777, 0.3, 0.002), (7, -2212.7, 0.0, 100, 1.0, 0.002), (31, 3000.2, 0.0, 2045, 2.0, 0.002)]
+    init = [(24, 1500.0, 0.0, 777), (6, -2210.0, 0.5, 100), (30, 3000.0, 0.0, 2045)]
+    x = t.synth_tracking_iq(21, N16, 40, FS16, chans)
+    eng = engine_for(16)
+    eng.upload_iq(x)
+    bank = _native.Tracker(eng, *[list(v) for v in zip(*init)])
+    rec, prof = bank.process(40, times(40, FS16, N16), want_profiles=True)
+    bank.close()
+    for c in range(3):
+        one = _native.Tracker(eng, *[[v] for v in init[c]])
+        r1 = one.process(40, times(40, FS16, N16))[0]
+        one.close()
+        for k in ("doppler", "carrier_phase", "peak_re", "code_phase", "symbol"):
+            assert np.array_equal(rec[c][k], r1[k]), (c, k)
+        assert (prof[c].argmax(axis=1) == rec[c]["peak_offset"]).all()
+    tr = t.TrackerOracle(25, 1500.0, 0.0, 777, FS16, N16)
+    y = x[:N16] * np.exp(-1j * (2 * np.pi * 1500.0 * (np.arange(N16) / FS16)))
+    ref = np.abs(o.correlate_1ms(y, np.roll(tr.prn, 777)))
+    assert np.abs(prof[0][0] - ref).max() <= 1e-5 * ref.max()
+
+
+def test_drop_in_pool_with_undo_equals_bank_and_bits_at_16368_ksps(native_lib):
+    """GpsSatelliteTracker, one call per millisecond through the channel pool: the second tracker is asked about a copy
+    of the chunk the first one advanced it through, so the pool takes the step back (undo) and recomputes.  Same
+    symbols as TrackerBank; integrate_bits gives the host NavigationBitIntegrator's events."""
+    from gypsum_b200.antenna_sample_provider import AntennaSampleChunk, SampleProviderAttributes
+    from gypsum_b200.gps_ca_prn_codes import GpsSatelliteId, generate_replica_prn_signals
+    from gypsum_b200.navigation_bit_integrator import NavigationBitIntegrator
+    from gypsum_b200.satellite import GpsSatellite
+    from gypsum_b200.tracker import BitValue, GpsSatelliteTracker, GpsSatelliteTrackingParameters, TrackerBank
+
+    n_ms = 400
+    attrs = SampleProviderAttributes(FS16, N16)
+    chans = [(25, 1500.3, 0.0, 777, 0.3, 0.002), (7, -2212.7, 0.0, 100, 1.0, 0.002)]
+    seeds = [(25, 1500.0, 0.0, 777), (7, -2210.0, 0.5, 100)]
+    x = t.synth_tracking_iq(33, N16, n_ms, FS16, chans)
+    tt = np.array([t.chunk_times(k, FS16, N16) for k in range(n_ms)])
+    codes = generate_replica_prn_signals()
+    sats = {sv: GpsSatellite(GpsSatelliteId(sv), codes[GpsSatelliteId(sv)], 16) for sv in (25, 7)}
+    bank = TrackerBank([(sats[sv], f, p, cp) for sv, f, p, cp in seeds], attrs)
+    rec = bank.process(x, tt[:, 0])
+    events = bank.integrate_bits(tt[:, 0], tt[:, 1])
+    trks = [GpsSatelliteTracker(GpsSatelliteTrackingParameters(satellite=sats[sv], current_doppler_shift=f,
+                                                               current_carrier_wave_phase_shift=p,
+                                                               current_prn_code_phase_shift=cp, doppler_shifts=[]),
+                                attrs, keep_correlation_profiles=False) for sv, f, p, cp in seeds]
+    code = {BitValue.ONE: 1, BitValue.ZERO: 0, BitValue.UNKNOWN: -1}
+    kept, got = [], [[], []]
+    integ = [NavigationBitIntegrator(GpsSatelliteId(sv)) for sv, *_ in seeds]
+    host_bits = [[], []]
+    for k in range(n_ms):
+        first = AntennaSampleChunk(tt[k, 0], tt[k, 1], x[k * N16:(k + 1) * N16])
+        second = AntennaSampleChunk(tt[k, 0], tt[k, 1], x[k * N16:(k + 1) * N16].copy())
+        kept += [first, second]  # keeps the two chunk keys distinct
+        for c, chunk in enumerate((first, second)):
+            ps = trks[c].process_samples(chunk)
+            got[c].append(ps.pseudosymbol.as_val())
+            host_bits[c] += [(k, e.receiver_timestamp, e.trailing_edge_receiver_timestamp, code[e.bit_value])
+                             for e in integ[c].process_pseudosymbol(chunk.start_time, ps)]
+    for c in range(2):
+        assert got[c] == list(rec[c]["symbol"]), c
+        assert trks[c].tracking_params.current_doppler_shift == rec[c, -1]["doppler"]
+        dev = [(int(e["ms_index"]), float(e["receiver_timestamp"]), float(e["trailing_edge_receiver_timestamp"]),
+                int(e["bit_value"])) for e in events[c]]
+        assert dev == host_bits[c] and len(dev) >= 10, c
+        trks[c].close()
+
+
+def test_receiver_flow_at_16368_ksps(tmp_path, native_lib):
+    """file provider -> DeviceSampleRing -> detector -> trackers -> pseudosymbols, step for step against the oracle
+    flow (acquisition and tracking).  Planted code phases stay below 2046, the only ones the reference can keep."""
+    from gypsum_b200.acquisition import GpsSatelliteDetector
+    from gypsum_b200.antenna_sample_provider import (AntennaSampleProviderBackedByFile, DeviceSampleRing, InputFileInfo,
+                                                     NoMoreSamplesError)
+    from gypsum_b200.gps_ca_prn_codes import GpsSatelliteId, generate_replica_prn_signals
+    from gypsum_b200.satellite import GpsSatellite
+    from gypsum_b200.tracker import GpsSatelliteTracker, GpsSatelliteTrackingParameters
+
+    n_ms = 60
+    planted = [(25, 1500.3, 0.0, 777, 0.3, 0.004), (7, -2212.7, 0.0, 1900, 1.0, 0.004)]
+    x = t.synth_tracking_iq(44, N16, n_ms + 1, FS16, planted)
+    path = tmp_path / "recording"
+    x.view(np.float32).tofile(path)
+    provider = AntennaSampleProviderBackedByFile(InputFileInfo(path, FS16))
+    attrs = provider.get_attributes()
+    codes = generate_replica_prn_signals()
+    satellites = {sid: GpsSatellite(sid, code, attrs.samples_per_prn_transmission // 1023) for sid, code in codes.items()}
+    detector = GpsSatelliteDetector(satellites)
+    ring = DeviceSampleRing(attrs, 10)
+    search_for = [GpsSatelliteId(i) for i in (3, 7, 25)]
+    trackers, symbols, acq = {}, {}, {}
+    k = 0
+    while True:
+        try:
+            chunk = ring.append(provider.get_samples(attrs.samples_per_prn_transmission))
+        except NoMoreSamplesError:
+            break
+        if ring.is_full() and not trackers:
+            for r in detector.detect_satellites_in_antenna_data(search_for, ring.window(), attrs):
+                params = GpsSatelliteTrackingParameters(
+                    satellite=satellites[r.satellite_id], current_doppler_shift=r.doppler_shift,
+                    current_carrier_wave_phase_shift=r.carrier_wave_phase_shift,
+                    current_prn_code_phase_shift=r.prn_phase_shift, doppler_shifts=[])
+                trackers[r.satellite_id.id] = GpsSatelliteTracker(params, attrs, keep_correlation_profiles=False)
+                symbols[r.satellite_id.id], acq[r.satellite_id.id] = [], r
+        for sv, trk in trackers.items():
+            symbols[sv].append(trk.process_samples(chunk).pseudosymbol.as_val())
+        k += 1
+    assert k == n_ms and sorted(trackers) == [7, 25]  # detector first (acquisition), then the trackers
+    first = x[: 10 * N16]
+    for sv, trk in trackers.items():
+        ref = o.acquire_sv(sv, first, FS16, N16)
+        assert (ref.doppler, ref.code_phase) == (acq[sv].doppler_shift, acq[sv].prn_phase_shift), sv
+        tr = t.TrackerOracle(sv, ref.doppler, ref.carrier_phase, ref.code_phase, FS16, N16)
+        want = [tr.step(x[ms * N16:(ms + 1) * N16], *t.chunk_times(ms, FS16, N16))["symbol"] for ms in range(9, n_ms)]
+        assert symbols[sv] == want, sv
+        trk.close()
+    ring.native.close()

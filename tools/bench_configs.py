@@ -1,5 +1,5 @@
 """Secondary measurements on one H100 (not the driver's bench line): BASELINE configs 2 (single block), 3, 5,
-the real 10-pass detector, and config 4 (tracking).  Prints one JSON line per workload.
+the real 10-pass detector, and config 4 (tracking, at 2.046 and at 16.368 Msps).  Prints one JSON line per workload.
 usage: python tools/bench_configs.py [--quick]"""
 import json
 import os
@@ -172,6 +172,54 @@ def tracker_case(n_ch, n_ms):
     eng.close()
 
 
+def tracker_case_16368(n_ch, n_ms):
+    """Config 4 at 16.368 Msps (k_track_channels_wide<16>): device-resident IQ, a 1-s synthetic base repeated.  Planted code
+    phases stay below 2046, the only ones the reference's tracker keeps at this rate.  The symbols of 3 channels over the
+    first second are checked against the tracker oracle."""
+    from oracle import tracker_oracle as t
+
+    n, fs, base_ms = 16368, 16368000, 1000
+    eng = _native.Engine(fs, n)
+    eng.set_replicas(CHIPS)
+    st = torch.cuda.Stream()  # the engine launches on this stream; the events are recorded on it
+    eng.set_stream(st.cuda_stream)
+    chans = [(sv, 1000.0 + 37.3 * sv, 0.0, (53 * sv) % 2046, 0.1 * sv, 0.002) for sv in range(1, n_ch + 1)]
+    base = to.synth_tracking_iq(5, n, base_ms, fs, chans)
+    xd = torch.from_numpy(base.view(np.float32)).cuda().repeat(-(-n_ms // base_ms))[: n_ms * n * 2]
+    eng.bind_iq_device(xd.data_ptr(), n_ms * n)
+    seeds = ([c[0] - 1 for c in chans], [c[1] for c in chans], [0.0] * n_ch, [c[3] for c in chans])
+    times = np.array([round(k * n / fs, 6) for k in range(n_ms)])
+    out = torch.empty(n_ch * n_ms * _native.TRACK_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()  # the stream and its buffers are ready before the engine's stream reads them
+    trk = _native.Tracker(eng, *seeds)
+    trk.process_device(200, times[:200], out.data_ptr())  # warm-up
+    trk.close()
+    trk = _native.Tracker(eng, *seeds)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    e0.record(st)
+    trk.process_device(n_ms, times, out.data_ptr())
+    e1.record(st)
+    torch.cuda.synchronize()
+    dt = e0.elapsed_time(e1) * 1e-3
+    rec = out.cpu().numpy().view(_native.TRACK_DTYPE).reshape(n_ch, n_ms)
+    trk.close()
+    check_ms, mism = min(n_ms, base_ms), {}
+    for i in (0, 13, 31):
+        sv, f, _, cp = chans[i][:4]
+        tr = t.TrackerOracle(sv, f, 0.0, cp, fs, n)
+        want = [tr.step(base[k * n:(k + 1) * n], *t.chunk_times(k, fs, n))["symbol"] for k in range(check_ms)]
+        mism[sv] = int(np.count_nonzero(rec["symbol"][i, :check_ms] != np.array(want)))
+    print(json.dumps({"workload": f"config 4 @ 16.368 Msps: {n_ch}-channel tracking, {n_ms / 1000:.0f} s of device-resident IQ",
+                      "kernel": "k_track_channels_wide<16>", "device_seconds": dt, "us_per_stream_ms": dt / n_ms * 1e6,
+                      "realtime_factor": (n_ms / 1000) / dt, "channel_ms_per_s": n_ch * n_ms / dt,
+                      "lost_channels": int((rec["lost"] > 0).any(axis=1).sum()),
+                      "oracle_symbol_mismatches": {"ms": check_ms, "by_sv": mism},
+                      "gpu": torch.cuda.get_device_name()}), flush=True)
+    eng.set_stream(0)
+    eng.close()
+
+
 if __name__ == "__main__":
     grid_case("config 2, one block", 2046, 1, 41, 1, 200)
     grid_case("config 2 x 32 blocks", 2046, 1, 41, 32, 50)
@@ -181,3 +229,4 @@ if __name__ == "__main__":
     fused_case(2046, 10, 24, 10)
     detector_case()
     tracker_case(32, 5000 if quick else 60000)
+    tracker_case_16368(32, 2000 if quick else 10000)

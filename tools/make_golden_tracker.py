@@ -1,5 +1,6 @@
 """Generate tests/golden/tracker_*.npz by running the LIVE reference tracker (/root/reference/gypsum/tracker.py).
-Run:  python tools/make_golden_tracker.py     (takes ~10 s)"""
+Run:  python tools/make_golden_tracker.py [name ...]     (all cases: ~1 min; np.savez_compressed stamps the time, so
+regenerate only the cases you add)"""
 import os
 import sys
 import warnings
@@ -26,6 +27,8 @@ def run(name, seed, n_ms, channel, init, sigma=0.02, N=N, FS=FS):
     codes = generate_replica_prn_signals()
     sv = channel[0]
     x = t.synth_tracking_iq(seed, N, n_ms, FS, [channel], sigma)
+    # prn_as_complex is lru-cached per satellite id (satellite.py:20-21): a cached replica of another rate would collide
+    GpsSatellite.prn_as_complex.fget.cache_clear()
     sat = GpsSatellite(GpsSatelliteId(sv), codes[GpsSatelliteId(sv)], N // 1023)
     params = GpsSatelliteTrackingParameters(satellite=sat, current_doppler_shift=init[0],
                                             current_carrier_wave_phase_shift=init[1],
@@ -55,13 +58,28 @@ def run(name, seed, n_ms, channel, init, sigma=0.02, N=N, FS=FS):
     print(name, "ms", len(rows), "lost_at", lost_at, "final doppler", r[-1, 6], "symbols +/-", (r[:, 3] > 0).sum(), (r[:, 3] < 0).sum())
 
 
-if __name__ == "__main__":
+CASES = {
     # (sv, doppler, doppler rate, code phase, carrier phase, amplitude); init = (doppler, carrier phase, code phase)
-    run("short", 11, 700, (25, 1500.3, 0.0, 777, 0.3, 0.004), (1500.0, 0.0, 777))
-    run("long", 12, 6300, (7, -2212.7, 0.5, 100, 1.0, 0.005), (-2210.0, 0.5, 100))   # crosses the 6 s circularity check
-    run("noise", 13, 6100, (3, 800.0, 0.0, 5, 0.0, 0.0), (800.0, 0.0, 5))            # no signal: loses lock at the check
+    "short": lambda: run("short", 11, 700, (25, 1500.3, 0.0, 777, 0.3, 0.004), (1500.0, 0.0, 777)),
+    "long": lambda: run("long", 12, 6300, (7, -2212.7, 0.5, 100, 1.0, 0.005), (-2210.0, 0.5, 100)),  # crosses the 6 s circularity check
+    "noise": lambda: run("noise", 13, 6100, (3, 800.0, 0.0, 5, 0.0, 0.0), (800.0, 0.0, 5)),  # no signal: loses lock at the check
     # 4.092 Msps: the reference keeps its hard-wired 2046 (tracker.py:301-303, :319) -- SURVEY F12 -- so the code-phase
     # accumulator wraps at 2046 although a millisecond is 4092 samples; the planted phase stays below 2046
     # weak signal: circularity 0.89 at the 6-second check -> the -+5 Hz / +-pi/2 nudge of tracker.py:380-387 fires
-    run("adjust", 21, 6100, (9, 432.1, 0.0, 300, 0.4, 0.0016), (430.0, 0.0, 300))
-    run("fs4", 14, 500, (12, 640.4, 0.0, 1501, 0.7, 0.004), (640.0, 0.0, 1501), N=4092, FS=4092000)
+    "adjust": lambda: run("adjust", 21, 6100, (9, 432.1, 0.0, 300, 0.4, 0.0016), (430.0, 0.0, 300)),
+    "fs4": lambda: run("fs4", 14, 500, (12, 640.4, 0.0, 1501, 0.7, 0.004), (640.0, 0.0, 1501), N=4092, FS=4092000),
+    # the other rates (same 2046 wrap).  1.023 Msps: the accumulator exceeds N = 1023 and np.roll is modular.
+    "fs1": lambda: run("fs1", 31, 2000, (12, 640.4, 0.0, 1501, 0.7, 0.004), (640.0, 0.0, 1501), N=1023, FS=1023000),
+    "fs8": lambda: run("fs8", 32, 2000, (12, 640.4, 0.0, 1501, 0.7, 0.002), (640.0, 0.0, 1501), N=8184, FS=8184000),
+    # 16.368 Msps: the I-pole variance of is_locked() (tracker.py:184-192) sees the noise variance sigma^2 N / 2, so the
+    # reference reports lock only at low sigma ...
+    "fs16": lambda: run("fs16", 33, 1500, (12, 640.4, 0.0, 1501, 0.7, 0.001), (640.0, 0.0, 1501), sigma=0.01, N=16368,
+                        FS=16368000),
+    # ... and never at sigma = 0.02; this one crosses the 6-second constellation check
+    "fs16_long": lambda: run("fs16_long", 34, 6100, (12, 640.4, 0.0, 1501, 0.7, 0.001), (640.0, 0.0, 1501), N=16368,
+                             FS=16368000),
+}
+
+if __name__ == "__main__":
+    for name in sys.argv[1:] or CASES:
+        CASES[name]()

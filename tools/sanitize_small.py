@@ -82,4 +82,23 @@ for n, m in ((2046, 2), (4092, 1)):
         pr = eng.correlation_profile_replica(odd, 250.0, 2, _native.NON_COHERENT)
         assert pr.shape == (n,)
     eng.close()
+# 16.368 Msps tracking (k_track_channels_wide<16>): a channel bank with profiles, then a pool step with undo
+n = 16368
+fs = n * 1000
+eng = _native.Engine(fs, n)
+eng.set_replicas(chips)
+xs = to.synth_tracking_iq(4, n, 3, fs, [(25, 1500.3, 0.0, 777, 0.3, 0.002)])
+eng.upload_iq(xs)
+t = _native.Tracker(eng, [24, 6], [1500.0, -100.0], [0.0, 0.0], [777, 5])
+rec, prof = t.process(3, [round(k * n / fs, 6) for k in range(3)], want_profiles=True)
+assert rec["symbol"].shape == (2, 3) and prof.shape == (2, 3, n)
+t.close()
+pool = _native.Tracker.pool(eng, 2)
+pool.reset_channel(1, 24, 1500.0, 0.0, 777)
+r1 = pool.process_channels([1], 1, [0.0], keep_undo=True)
+pool.undo_channel(1)
+r2 = pool.process_channels([1], 1, [0.0])
+assert r1["symbol"][0, 0] == r2["symbol"][0, 0]
+pool.close()
+eng.close()
 print("sanitize_small ok")
