@@ -9,6 +9,8 @@
 #include <map>
 #include <numeric>
 #include <string>
+#include <tuple>
+#include <utility>
 #include <vector>
 
 #include "../../include/gypsum_b200.h"
@@ -23,46 +25,44 @@ namespace {
 
 thread_local std::string g_create_error;
 
-template <class T>
-struct DevBuf {
+struct DeviceMemory {
+    static cudaError_t alloc(void** p, size_t bytes) { return cudaMalloc(p, bytes); }
+    static void free(void* p) { cudaFree(p); }
+};
+struct PinnedMemory {
+    static cudaError_t alloc(void** p, size_t bytes) { return cudaMallocHost(p, bytes); }
+    static void free(void* p) { cudaFreeHost(p); }
+};
+
+// A growable array of device (DeviceMemory) or page-locked host (PinnedMemory) memory that frees itself.  ensure() keeps
+// the contents only while the array does not have to grow.
+template <class T, class Memory>
+struct Buf {
     T* p = nullptr;
     size_t cap = 0;
+    Buf() = default;
+    Buf(const Buf&) = delete;
+    Buf& operator=(const Buf&) = delete;
+    Buf(Buf&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+    ~Buf() { release(); }
     cudaError_t ensure(size_t n) {
         if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
+        release();
         size_t want = std::max(n, static_cast<size_t>(16));
-        cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&p), want * sizeof(T));
+        cudaError_t e = Memory::alloc(reinterpret_cast<void**>(&p), want * sizeof(T));
         if (e == cudaSuccess) cap = want;
         return e;
     }
     void release() {
-        if (p) cudaFree(p);
+        if (p) Memory::free(p);
         p = nullptr;
         cap = 0;
     }
 };
 template <class T>
-struct PinnedBuf {
-    T* p = nullptr;
-    size_t cap = 0;
-    cudaError_t ensure(size_t n) {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-        size_t want = std::max(n, static_cast<size_t>(16));
-        cudaError_t e = cudaMallocHost(reinterpret_cast<void**>(&p), want * sizeof(T));
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-    void release() {
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-    }
-};
+using DevBuf = Buf<T, DeviceMemory>;
+template <class T>
+using PinnedBuf = Buf<T, PinnedMemory>;
 
 // L2 window of the one-warp correlate kernel: the fastest size for the benchmark's config-2 call and for config 3 on the
 // H100's 50 MB L2 (DESIGN.md §4, L2 windows).
@@ -94,7 +94,7 @@ struct gb200_engine {
     PinnedBuf<int> rh_cell_prn;
     PinnedBuf<int> rh_ints;
     PinnedBuf<RefineResult> rh_results;
-    PinnedBuf<float2> h_iq;
+    PinnedBuf<float2> h_iq, h_replica;
     PinnedBuf<CellRecord> h_records;
     PinnedBuf<int> h_ints;
     PinnedBuf<double> h_doubles;
@@ -114,48 +114,34 @@ struct gb200_engine {
     PinnedBuf<BestRecord> h_best;
     // gb200_acquire_grid_host: one CUDA graph (copy-in, doppler_spectra, correlate_cells, copy-out) per grid shape
     struct HostGraph {
+        // Everything a captured graph bakes in: the grid's shape and axes, and every buffer it reads or writes.
+        struct Key {
+            int n_blocks = 0, M = 0, P = 0, D = 0, kind = 0;
+            std::vector<double> dop;
+            std::vector<int> prn;
+            const void *iq_dev = nullptr, *rec_dev = nullptr, *iq_stage = nullptr, *rec_stage = nullptr, *spec = nullptr;
+            const void *d_dop = nullptr, *d_prn = nullptr, *crep = nullptr;  // what the captured kernels dereference besides the above
+            const void* rec_target = nullptr;  // where the captured correlate kernel stores its records
+            cudaStream_t stream = nullptr;
+            auto ids() const {
+                return std::tie(n_blocks, M, P, D, kind, iq_dev, rec_dev, iq_stage, rec_stage, spec, d_dop, d_prn, crep, rec_target,
+                                stream);
+            }
+            // the axes compare bit for bit, as the device copies of them do (upload_grid_axes)
+            bool operator==(const Key& o) const {
+                return ids() == o.ids() && dop.size() == o.dop.size() && prn == o.prn &&
+                       memcmp(dop.data(), o.dop.data(), sizeof(double) * dop.size()) == 0;
+            }
+        } key;
         cudaGraphExec_t exec = nullptr;
-        int n_blocks = 0, M = 0, P = 0, D = 0, kind = 0, seen = 0;
-        std::vector<double> dop;
-        std::vector<int> prn;
-        const void *iq_dev = nullptr, *rec_dev = nullptr, *iq_stage = nullptr, *rec_stage = nullptr, *spec = nullptr;
-        const void *d_dop = nullptr, *d_prn = nullptr, *crep = nullptr;  // what the captured kernels dereference besides the above
-        const void* rec_target = nullptr;  // where the captured correlate kernel stores its records
-        cudaStream_t stream = nullptr;
+        int seen = 0;
     } hg;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev[2];
     size_t ev_used[2] = {0, 0};
     std::string err;
 
-    ~gb200_engine() {
+    ~gb200_engine() {  // the buffers free themselves
         if (hg.exec) cudaGraphExecDestroy(hg.exec);
-        d_best.release();
-        h_best.release();
-        tw1.release();
-        tw2.release();
-        crep.release();
-        d_replica.release();
-        iq_own.release();
-        spec.release();
-        chips.release();
-        d_doppler.release();
-        d_ints.release();
-        d_records.release();
-        d_profile.release();
-        r_state.release();
-        r_doppler.release();
-        r_records.release();
-        r_ints.release();
-        r_results.release();
-        r_cell_prn.release();
-        rh_cell_prn.release();
-        rh_ints.release();
-        rh_results.release();
-        h_iq.release();
-        h_records.release();
-        h_ints.release();
-        h_doubles.release();
-        h_profile.release();
         for (auto& pool : ev)
             for (auto& pr : pool) {
                 cudaEventDestroy(pr.first);
@@ -240,6 +226,23 @@ static_assert(sizeof(gb200_bit_event) == sizeof(BitEvent), "ABI bit event and de
         }                                                                                                  \
     } while (0)
 
+#define GB_TRY(expr)                       \
+    do {                                   \
+        const int rc_ = (expr);            \
+        if (rc_ != GB200_OK) return rc_;   \
+    } while (0)
+
+// One kernel launch: the optional timing bracket of kernel class `which` (0 doppler_spectra, 1 correlate, -1 untimed),
+// the error check and the launch count (gb200_launch_count).
+#define GB_LAUNCH(e, which, expr)              \
+    do {                                       \
+        {                                      \
+            TimedLaunch tl_((e), (which));     \
+            GB_CUDA((e), expr);                \
+        }                                      \
+        (e)->launches++;                       \
+    } while (0)
+
 namespace {
 
 // optional event bracket around one kernel launch (measurement aid, off by default)
@@ -248,7 +251,7 @@ struct TimedLaunch {
     int which;
     cudaEvent_t stop = nullptr;
     TimedLaunch(gb200_engine* e_, int which_) : e(e_), which(which_) {
-        if (!e->timing) return;
+        if (!e->timing || which < 0) return;
         auto& pool = e->ev[which];
         if (e->ev_used[which] == pool.size()) {
             cudaEvent_t a, b;
@@ -264,14 +267,12 @@ struct TimedLaunch {
     }
 };
 
-int gcd_int(int a, int b) { return b ? gcd_int(b, a % b) : a; }
-
 // How many of a CTA's slots (correlate_slots: warps or warp pairs) share one cell.  With plenty of cells per slot each
 // slot keeps a whole cell (no cross-slot merge, no CTA-wide barrier); small launches split a cell's polyphase branches
 // over slots to fill the machine.
 int pick_rsplit(const gb200_engine* e, int slots, long long n_cells) {
     if (n_cells >= 8LL * e->num_sms * slots) return 1;
-    return gcd_int(e->s, slots);
+    return std::gcd(e->s, slots);
 }
 
 size_t unit_floats2(const gb200_engine* e, int M) { return static_cast<size_t>(M) * e->s * 2 * kFft; }
@@ -291,11 +292,7 @@ int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int
     sa.M = M;
     sa.n_doppler = n_doppler;
     sa.n_units = n_units;
-    {
-        TimedLaunch tl(e, 0);
-        GB_CUDA(e, launch_doppler_spectra(sa, e->stream));
-    }
-    e->launches++;
+    GB_LAUNCH(e, 0, launch_doppler_spectra(sa, e->stream));
     return GB200_OK;
 }
 
@@ -316,13 +313,140 @@ CorrelateArgs correlate_args(const gb200_engine* e, int M, int kind, int rsplit,
     return ca;
 }
 
-int check_common(gb200_engine* e, int n_ms, int kind) {
-    if (!e) return GB200_EINVAL;
+// The fused-kernel arguments every launch sets (the kernel is configured on first use); the caller adds its cells.
+int fused_args(gb200_engine* e, int M, FusedArgs* fa) {
+    if (!e->fused_configured) {
+        GB_CUDA(e, configure_fused_kernel());
+        e->fused_configured = true;
+    }
+    *fa = FusedArgs{};
+    fa->iq = e->iq;
+    fa->crep = e->crep.p;
+    fa->tw1 = e->tw1.p;
+    fa->tw2 = e->tw2.p;
+    fa->inv_fs = 1.0 / static_cast<double>(e->fs);
+    fa->N = e->N;
+    fa->M = M;
+    return GB200_OK;
+}
+
+// A list-mode correlate plan: cells sorted by PRN (cell_u: spectrum unit, cell_out: record slot) and groups of consecutive
+// cells of one PRN.  It lives in an int buffer as [cell_u][cell_out][grp_first][grp_count][grp_prn].
+struct ListPlan {
+    std::vector<int> cell_u, cell_out, grp_first, grp_count, grp_prn;
+    size_t size() const { return 2 * cell_u.size() + 3 * grp_prn.size(); }
+    void write(int* host) const {
+        for (const auto* v : {&cell_u, &cell_out, &grp_first, &grp_count, &grp_prn}) host = std::copy(v->begin(), v->end(), host);
+    }
+    // Points ca at n_groups groups from group g0 on of the plan written at dev.
+    void bind(CorrelateArgs& ca, const int* dev, int g0, int n_groups) const {
+        const size_t nc = cell_u.size(), ng = grp_prn.size();
+        ca.n_groups = n_groups;
+        ca.cell_u = dev;
+        ca.cell_out = dev + nc;
+        ca.grp_first = dev + 2 * nc + g0;
+        ca.grp_count = dev + 2 * nc + ng + g0;
+        ca.grp_prn = dev + 2 * nc + 2 * ng + g0;
+    }
+};
+
+// Argument rules shared by the entry points, one function each.
+int check_kind(gb200_engine* e, int kind) {
     if (kind != GB200_COHERENT && kind != GB200_NON_COHERENT) GB_FAIL(e, GB200_EINVAL, "Unexpected integration type");
+    return GB200_OK;
+}
+
+int check_replicas(gb200_engine* e) {
     if (e->n_prn == 0) GB_FAIL(e, GB200_ESTATE, "no PRN replicas loaded (gb200_set_replicas)");
+    return GB200_OK;
+}
+
+int check_prns(gb200_engine* e, const int32_t* prn_idx, int n) {
+    for (int i = 0; i < n; ++i)
+        if (prn_idx[i] < 0 || prn_idx[i] >= e->n_prn) GB_FAIL(e, GB200_EINVAL, "prn index %d out of range", prn_idx[i]);
+    return GB200_OK;
+}
+
+int check_iq(gb200_engine* e, int n_ms) {
     if (!e->iq) GB_FAIL(e, GB200_ESTATE, "no IQ loaded (gb200_upload_iq / gb200_bind_iq_device)");
     if (n_ms < 1) GB_FAIL(e, GB200_EINVAL, "need at least one whole millisecond of samples");
     return GB200_OK;
+}
+
+int check_samples(gb200_engine* e, int n_ms) {
+    if (static_cast<int64_t>(n_ms) * e->N > e->iq_samples)
+        GB_FAIL(e, GB200_EINVAL, "need %lld samples, %lld loaded", static_cast<long long>(n_ms) * e->N,
+                static_cast<long long>(e->iq_samples));
+    return GB200_OK;
+}
+
+int check_grid(gb200_engine* e, int n_blocks, int P, int D, const int32_t* prn_idx, const double* dop) {
+    if (n_blocks < 1 || P < 1 || D < 1 || !prn_idx || !dop) GB_FAIL(e, GB200_EINVAL, "empty grid");
+    return GB200_OK;
+}
+
+int check_channel(gb200_tracker* t, int channel) {
+    if (channel < 0 || channel >= t->n_channels) GB_FAIL(t->e, GB200_EINVAL, "channel %d out of range", channel);
+    return GB200_OK;
+}
+
+// What every acquisition needs before its own arguments are looked at.
+int check_common(gb200_engine* e, int n_ms, int kind) {
+    GB_TRY(check_kind(e, kind));
+    GB_TRY(check_replicas(e));
+    return check_iq(e, n_ms);
+}
+
+// Whether p is page-locked host memory, which the DMA engine reads and writes directly; *alias (optional) receives its
+// device address.
+bool is_pinned(const void* p, void** alias = nullptr) {
+    cudaPointerAttributes attr{};
+    const bool pinned = cudaPointerGetAttributes(&attr, p) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+    cudaGetLastError();
+    if (alias) *alias = pinned ? attr.devicePointer : nullptr;
+    return pinned;
+}
+
+// Copies n host elements into the pinned buffer stage (grown to fit) and points src at the copy.  No copy in flight may
+// still read stage: the caller synchronises first, or owns the buffer.
+template <class T>
+cudaError_t stage_in(PinnedBuf<T>& stage, const T*& src, size_t n) {
+    cudaError_t ce = stage.ensure(std::max<size_t>(n, 1));
+    if (ce != cudaSuccess) return ce;
+    memcpy(stage.p, src, n * sizeof(T));
+    src = stage.p;
+    return cudaSuccess;
+}
+
+// Puts n host elements on the device at dst through the pinned buffer stage (see stage_in).
+template <class T>
+int upload(gb200_engine* e, T* dst, const T* src, size_t n, PinnedBuf<T>& stage) {
+    GB_CUDA(e, stage_in(stage, src, n));
+    GB_CUDA(e, cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyHostToDevice, e->stream));
+    return GB200_OK;
+}
+
+// Brings n device elements to dst and waits for them (and for everything enqueued before): straight DMA when dst is
+// pinned, else through the pinned buffer stage.
+template <class T>
+int download(gb200_engine* e, T* dst, const T* src, size_t n, PinnedBuf<T>& stage) {
+    T* to = dst;
+    if (!is_pinned(dst)) {
+        GB_CUDA(e, stage.ensure(n));
+        to = stage.p;
+    }
+    GB_CUDA(e, cudaMemcpyAsync(to, src, n * sizeof(T), cudaMemcpyDeviceToHost, e->stream));
+    GB_CUDA(e, cudaStreamSynchronize(e->stream));
+    if (to != dst) memcpy(dst, to, n * sizeof(T));
+    return GB200_OK;
+}
+
+// Forgets the engine's IQ binding when it points into the n samples at buf, which are about to be freed.
+void unbind_iq(gb200_engine* e, const float2* buf, size_t n) {
+    if (e->iq >= buf && e->iq < buf + n) {
+        e->iq = nullptr;
+        e->iq_samples = 0;
+    }
 }
 
 // The grid's axes (PRN rows in d_ints, Doppler bins in d_doppler) are uploaded only when they changed -- or when a list-mode
@@ -336,12 +460,8 @@ int upload_grid_axes(gb200_engine* e, const int32_t* prn_idx, int P, const doubl
     GB_CUDA(e, cudaStreamSynchronize(e->stream));  // staging buffers may still be in flight
     GB_CUDA(e, e->d_doppler.ensure(D));
     GB_CUDA(e, e->d_ints.ensure(P));
-    GB_CUDA(e, e->h_doubles.ensure(D));
-    GB_CUDA(e, e->h_ints.ensure(P));
-    memcpy(e->h_doubles.p, dop, sizeof(double) * D);
-    memcpy(e->h_ints.p, prn_idx, sizeof(int) * P);
-    GB_CUDA(e, cudaMemcpyAsync(e->d_doppler.p, e->h_doubles.p, sizeof(double) * D, cudaMemcpyHostToDevice, e->stream));
-    GB_CUDA(e, cudaMemcpyAsync(e->d_ints.p, e->h_ints.p, sizeof(int) * P, cudaMemcpyHostToDevice, e->stream));
+    GB_TRY(upload(e, e->d_doppler.p, dop, D, e->h_doubles));
+    GB_TRY(upload(e, e->d_ints.p, prn_idx, P, e->h_ints));
     e->doppler_cache.assign(dop, dop + D);
     e->prn_cache.assign(prn_idx, prn_idx + P);
     e->grid_cache_valid = true;
@@ -351,17 +471,13 @@ int upload_grid_axes(gb200_engine* e, const int32_t* prn_idx, int P, const doubl
 // grid mode: all cells of n_blocks x prn list x doppler list; records written to rec_dev (device)
 int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D, int kind,
              CellRecord* rec_dev) {
-    int rc = check_common(e, M, kind);
-    if (rc) return rc;
-    if (n_blocks < 1 || P < 1 || D < 1 || !prn_idx || !dop) GB_FAIL(e, GB200_EINVAL, "empty grid");
+    GB_TRY(check_common(e, M, kind));
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     if (static_cast<int64_t>(n_blocks) * M * e->N > e->iq_samples)
         GB_FAIL(e, GB200_EINVAL, "grid needs %lld samples, %lld loaded", static_cast<long long>(n_blocks) * M * e->N,
                 static_cast<long long>(e->iq_samples));
-    for (int i = 0; i < P; ++i)
-        if (prn_idx[i] < 0 || prn_idx[i] >= e->n_prn) GB_FAIL(e, GB200_EINVAL, "prn index %d out of range", prn_idx[i]);
-
-    rc = upload_grid_axes(e, prn_idx, P, dop, D);
-    if (rc) return rc;
+    GB_TRY(check_prns(e, prn_idx, P));
+    GB_TRY(upload_grid_axes(e, prn_idx, P, dop, D));
 
     const size_t unit = unit_floats2(e, M);
     const size_t per_block = unit * D;
@@ -375,8 +491,7 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
     for (int b0 = 0; b0 < n_blocks; b0 += nb) {
         const int nbb = std::min(nb, n_blocks - b0);
         const int chunks = (nbb * D + cpg - 1) / cpg;  // groups per PRN: its nbb*D cells in chunks of cpg
-        rc = run_spectra(e, e->iq + static_cast<size_t>(b0) * M * e->N, M, e->d_doppler.p, D, nbb * D);
-        if (rc) return rc;
+        GB_TRY(run_spectra(e, e->iq + static_cast<size_t>(b0) * M * e->N, M, e->d_doppler.p, D, nbb * D));
 
         CorrelateArgs ca = correlate_args(e, M, kind, rsplit, rec_dev + static_cast<size_t>(b0) * P * D, nullptr);
         ca.n_groups = P * chunks;
@@ -397,23 +512,13 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
             const long long n_win = static_cast<long long>((batch_bytes + win_bytes - 1) / win_bytes);
             long long wc = (chunks + n_win - 1) / n_win;
             // a window whose P * wc groups divide evenly among the CTAs, when one exists within a quarter of the target size
-            long long q = grid, gcd_a = P, gcd_b = grid;
-            while (gcd_b) {
-                const long long t = gcd_a % gcd_b;
-                gcd_a = gcd_b;
-                gcd_b = t;
-            }
-            q = grid / gcd_a;
+            const long long q = grid / std::gcd(P, grid);
             const long long even = ((wc + q / 2) / q) * q;
             if (even > 0 && even * 4 >= wc * 3 && even * 4 <= wc * 5) wc = even;
             static const int min_groups = env_int("GB200_L2_WINDOW_MIN_GROUPS", 2);
             if (wc * P >= static_cast<long long>(min_groups) * grid && wc < chunks) ca.win_chunks = static_cast<int>(wc);
         }
-        {
-            TimedLaunch tl(e, 1);
-            GB_CUDA(e, launch_correlate(ca, grid, e->stream));
-        }
-        e->launches++;
+        GB_LAUNCH(e, 1, launch_correlate(ca, grid, e->stream));
     }
     return GB200_OK;
 }
@@ -421,14 +526,10 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
 // list mode.  Cells are sorted by PRN and cut into chunks whose spectra fit the scratch budget.
 int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double* dop, const int32_t* probe, int M,
               int kind, CellRecord* rec_dev, float* profile_dev) {
-    int rc = check_common(e, M, kind);
-    if (rc) return rc;
+    GB_TRY(check_common(e, M, kind));
     if (n_cells < 1 || !prn_idx || !dop) GB_FAIL(e, GB200_EINVAL, "empty cell list");
-    if (static_cast<int64_t>(M) * e->N > e->iq_samples)
-        GB_FAIL(e, GB200_EINVAL, "need %lld samples, %lld loaded", static_cast<long long>(M) * e->N,
-                static_cast<long long>(e->iq_samples));
-    for (int i = 0; i < n_cells; ++i)
-        if (prn_idx[i] < 0 || prn_idx[i] >= e->n_prn) GB_FAIL(e, GB200_EINVAL, "prn index %d out of range", prn_idx[i]);
+    GB_TRY(check_samples(e, M));
+    GB_TRY(check_prns(e, prn_idx, n_cells));
     e->grid_cache_valid = false;  // d_ints / d_doppler are about to be overwritten
 
     bool use_fused = e->fused == 1;
@@ -442,41 +543,25 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
         use_fused = n_unique * 4 > n_cells || static_cast<long long>(n_cells) * M <= 8192;
     }
     if (use_fused && fused_supports(e->s) && !profile_dev) {
-        if (!e->fused_configured) {
-            GB_CUDA(e, configure_fused_kernel());
-            e->fused_configured = true;
-        }
         // one CTA per cell, whole pipeline in one kernel
+        FusedArgs fa;
+        GB_TRY(fused_args(e, M, &fa));
         GB_CUDA(e, cudaStreamSynchronize(e->stream));
         GB_CUDA(e, e->d_ints.ensure(static_cast<size_t>(n_cells) * 2));
         GB_CUDA(e, e->h_ints.ensure(static_cast<size_t>(n_cells) * 2));
         GB_CUDA(e, e->d_doppler.ensure(n_cells));
-        GB_CUDA(e, e->h_doubles.ensure(n_cells));
         for (int i = 0; i < n_cells; ++i) {
             e->h_ints.p[i] = prn_idx[i];
             e->h_ints.p[n_cells + i] = probe ? probe[i] : -1;
-            e->h_doubles.p[i] = dop[i];
         }
         GB_CUDA(e, cudaMemcpyAsync(e->d_ints.p, e->h_ints.p, sizeof(int) * 2 * n_cells, cudaMemcpyHostToDevice, e->stream));
-        GB_CUDA(e, cudaMemcpyAsync(e->d_doppler.p, e->h_doubles.p, sizeof(double) * n_cells, cudaMemcpyHostToDevice, e->stream));
-        FusedArgs fa{};
-        fa.iq = e->iq;
+        GB_TRY(upload(e, e->d_doppler.p, dop, n_cells, e->h_doubles));
         fa.doppler = e->d_doppler.p;
         fa.prn = e->d_ints.p;
         fa.probe = e->d_ints.p + n_cells;
         fa.records = rec_dev;
-        fa.crep = e->crep.p;
-        fa.tw1 = e->tw1.p;
-        fa.tw2 = e->tw2.p;
-        fa.inv_fs = 1.0 / static_cast<double>(e->fs);
-        fa.N = e->N;
-        fa.M = M;
         fa.n_cells = n_cells;
-        {
-            TimedLaunch tl(e, 1);
-            GB_CUDA(e, launch_acquire_fused(fa, e->s, kind, e->stream));
-        }
-        e->launches++;
+        GB_LAUNCH(e, 1, launch_acquire_fused(fa, e->s, kind, e->stream));
         return GB200_OK;
     }
 
@@ -491,12 +576,11 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
     const int max_cells = static_cast<int>(std::max<size_t>(cpg, e->spec_budget_bytes / (unit * sizeof(float2)) / cpg * cpg));
 
     GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    // probe indices live at the front of the int buffer for the whole call
+    // probe indices live at the front of the int buffer for the whole call, each chunk's plan behind them
     const size_t ints_needed = static_cast<size_t>(n_cells) * 3 + 3 * (static_cast<size_t>(n_cells) + 1);
     GB_CUDA(e, e->d_ints.ensure(ints_needed));
     GB_CUDA(e, e->h_ints.ensure(ints_needed));
     GB_CUDA(e, e->d_doppler.ensure(n_cells));
-    GB_CUDA(e, e->h_doubles.ensure(n_cells));
     for (int i = 0; i < n_cells; ++i) e->h_ints.p[i] = probe ? probe[i] : -1;
     GB_CUDA(e, cudaMemcpyAsync(e->d_ints.p, e->h_ints.p, sizeof(int) * n_cells, cudaMemcpyHostToDevice, e->stream));
     GB_CUDA(e, e->spec.ensure(unit * std::min(max_cells, n_cells)));
@@ -508,7 +592,7 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
         // plan arrays for this chunk (indices into the chunk)
         std::map<double, int> uniq;
         std::vector<double> udop;
-        std::vector<int> cell_u, cell_out, g_first, g_count, g_prn;
+        ListPlan plan;
         for (int c = c0; c < c1; ++c) {
             const int orig = order[c];
             auto it = uniq.find(dop[orig]);
@@ -520,71 +604,38 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
             } else {
                 u = it->second;
             }
-            cell_u.push_back(u);
-            cell_out.push_back(orig);
-            if (g_prn.empty() || g_prn.back() != prn_idx[orig] || g_count.back() == cpg) {
-                g_first.push_back(c - c0);
-                g_count.push_back(1);
-                g_prn.push_back(prn_idx[orig]);
+            plan.cell_u.push_back(u);
+            plan.cell_out.push_back(orig);
+            if (plan.grp_prn.empty() || plan.grp_prn.back() != prn_idx[orig] || plan.grp_count.back() == cpg) {
+                plan.grp_first.push_back(c - c0);
+                plan.grp_count.push_back(1);
+                plan.grp_prn.push_back(prn_idx[orig]);
             } else {
-                g_count.back()++;
+                plan.grp_count.back()++;
             }
         }
-        const int nc = c1 - c0, ng = static_cast<int>(g_prn.size()), nu = static_cast<int>(udop.size());
         // the staging buffers are reused per chunk: wait for the previous chunk's copies
         if (c0 > 0) GB_CUDA(e, cudaStreamSynchronize(e->stream));
-        int* hi = e->h_ints.p + n_cells;
         int* di = e->d_ints.p + n_cells;
-        memcpy(hi, cell_u.data(), sizeof(int) * nc);
-        memcpy(hi + nc, cell_out.data(), sizeof(int) * nc);
-        memcpy(hi + 2 * nc, g_first.data(), sizeof(int) * ng);
-        memcpy(hi + 2 * nc + ng, g_count.data(), sizeof(int) * ng);
-        memcpy(hi + 2 * nc + 2 * ng, g_prn.data(), sizeof(int) * ng);
-        memcpy(e->h_doubles.p, udop.data(), sizeof(double) * nu);
-        GB_CUDA(e, cudaMemcpyAsync(di, hi, sizeof(int) * (2 * nc + 3 * ng), cudaMemcpyHostToDevice, e->stream));
-        GB_CUDA(e, cudaMemcpyAsync(e->d_doppler.p, e->h_doubles.p, sizeof(double) * nu, cudaMemcpyHostToDevice, e->stream));
+        plan.write(e->h_ints.p + n_cells);
+        GB_CUDA(e, cudaMemcpyAsync(di, e->h_ints.p + n_cells, sizeof(int) * plan.size(), cudaMemcpyHostToDevice, e->stream));
+        GB_TRY(upload(e, e->d_doppler.p, udop.data(), udop.size(), e->h_doubles));
 
-        rc = run_spectra(e, e->iq, M, e->d_doppler.p, nu, nu);
-        if (rc) return rc;
+        const int nu = static_cast<int>(udop.size()), ng = static_cast<int>(plan.grp_prn.size());
+        GB_TRY(run_spectra(e, e->iq, M, e->d_doppler.p, nu, nu));
 
         CorrelateArgs ca = correlate_args(e, M, kind, rsplit, rec_dev, profile_dev);
-        ca.n_groups = ng;
-        ca.cell_u = di;
-        ca.cell_out = di + nc;
-        ca.grp_first = di + 2 * nc;
-        ca.grp_count = di + 2 * nc + ng;
-        ca.grp_prn = di + 2 * nc + 2 * ng;
+        plan.bind(ca, di, 0, ng);
         ca.cell_probe = e->d_ints.p;
-        const int grid = std::min(ng, e->num_sms);
-        {
-            TimedLaunch tl(e, 1);
-            GB_CUDA(e, launch_correlate(ca, grid, e->stream));
-        }
-        e->launches++;
+        GB_LAUNCH(e, 1, launch_correlate(ca, std::min(ng, e->num_sms), e->stream));
         c0 = c1;
     }
     return GB200_OK;
 }
 
-bool is_pinned_host(const void* p) {
-    cudaPointerAttributes attr;
-    const bool pinned = cudaPointerGetAttributes(&attr, p) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-    cudaGetLastError();
-    return pinned;
-}
-
-// Records to the caller: straight DMA when the caller's buffer is pinned, else through the engine's pinned staging.
+// Records to the caller (see download).
 int fetch_records(gb200_engine* e, size_t n, gb200_cell_record* out_host) {
-    if (is_pinned_host(out_host)) {
-        GB_CUDA(e, cudaMemcpyAsync(out_host, e->d_records.p, n * sizeof(CellRecord), cudaMemcpyDeviceToHost, e->stream));
-        GB_CUDA(e, cudaStreamSynchronize(e->stream));
-        return GB200_OK;
-    }
-    GB_CUDA(e, e->h_records.ensure(n));
-    GB_CUDA(e, cudaMemcpyAsync(e->h_records.p, e->d_records.p, n * sizeof(CellRecord), cudaMemcpyDeviceToHost, e->stream));
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    memcpy(out_host, e->h_records.p, n * sizeof(CellRecord));
-    return GB200_OK;
+    return download(e, reinterpret_cast<CellRecord*>(out_host), e->d_records.p, n, e->h_records);
 }
 
 }  // namespace
@@ -676,8 +727,7 @@ int gb200_set_replicas(gb200_engine* e, const uint8_t* chips, int n_prn) {
     GB_CUDA(e, e->chips.ensure(static_cast<size_t>(n_prn) * kChips));
     GB_CUDA(e, e->crep.ensure(static_cast<size_t>(n_prn) * 2 * kFft));
     GB_CUDA(e, cudaMemcpyAsync(e->chips.p, chips, static_cast<size_t>(n_prn) * kChips, cudaMemcpyHostToDevice, e->stream));
-    GB_CUDA(e, launch_replica_spectra(e->chips.p, n_prn, e->crep.p, e->stream));
-    e->launches++;
+    GB_LAUNCH(e, -1, launch_replica_spectra(e->chips.p, n_prn, e->crep.p, e->stream));
     GB_CUDA(e, cudaStreamSynchronize(e->stream));
     e->n_prn = n_prn;
     return GB200_OK;
@@ -688,13 +738,10 @@ int gb200_upload_iq(gb200_engine* e, const float* iq_host, int64_t n_samples) {
     if (!iq_host || n_samples < 0) GB_FAIL(e, GB200_EINVAL, "bad IQ buffer");
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_CUDA(e, e->iq_own.ensure(static_cast<size_t>(std::max<int64_t>(n_samples, 1))));
-    const void* src = iq_host;
-    const bool pinned = is_pinned_host(iq_host);
-    if (!pinned) {
+    const float2* src = reinterpret_cast<const float2*>(iq_host);
+    if (!is_pinned(iq_host)) {
         GB_CUDA(e, cudaStreamSynchronize(e->stream));  // staging buffer may still be in flight
-        GB_CUDA(e, e->h_iq.ensure(static_cast<size_t>(std::max<int64_t>(n_samples, 1))));
-        memcpy(e->h_iq.p, iq_host, static_cast<size_t>(n_samples) * sizeof(float2));
-        src = e->h_iq.p;
+        GB_CUDA(e, stage_in(e->h_iq, src, static_cast<size_t>(n_samples)));
     }
     GB_CUDA(e, cudaMemcpyAsync(e->iq_own.p, src, static_cast<size_t>(n_samples) * sizeof(float2), cudaMemcpyHostToDevice,
                                e->stream));
@@ -726,11 +773,10 @@ int gb200_acquire_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_
     if (!e) return GB200_EINVAL;
     if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
     GB_CUDA(e, cudaSetDevice(e->device));
-    if (n_blocks < 1 || P < 1 || D < 1) GB_FAIL(e, GB200_EINVAL, "empty grid");
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     const size_t n = static_cast<size_t>(n_blocks) * P * D;
     GB_CUDA(e, e->d_records.ensure(n));
-    int rc = run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p);
-    if (rc) return rc;
+    GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p));
     return fetch_records(e, n, out_host);
 }
 
@@ -740,14 +786,12 @@ int gb200_acquire_grid_best_device(gb200_engine* e, int n_blocks, int M, const i
     if (!e) return GB200_EINVAL;
     if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
     GB_CUDA(e, cudaSetDevice(e->device));
-    if (n_blocks < 1 || P < 1 || D < 1) GB_FAIL(e, GB200_EINVAL, "empty grid");
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     const size_t n = static_cast<size_t>(n_blocks) * P * D;
     GB_CUDA(e, e->d_records.ensure(n));
-    int rc = run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p);
-    if (rc) return rc;
-    GB_CUDA(e, launch_best_bins(n_blocks * P, D, e->N, e->d_records.p, e->d_doppler.p, static_cast<BestRecord*>(out_device),
-                                e->stream));
-    e->launches++;
+    GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p));
+    GB_LAUNCH(e, -1, launch_best_bins(n_blocks * P, D, e->N, e->d_records.p, e->d_doppler.p, static_cast<BestRecord*>(out_device),
+                                      e->stream));
     return GB200_OK;
 }
 
@@ -756,17 +800,11 @@ int gb200_acquire_grid_best(gb200_engine* e, int n_blocks, int M, const int32_t*
     if (!e) return GB200_EINVAL;
     if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
     GB_CUDA(e, cudaSetDevice(e->device));
-    if (n_blocks < 1 || P < 1 || D < 1) GB_FAIL(e, GB200_EINVAL, "empty grid");
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     const size_t n = static_cast<size_t>(n_blocks) * P;
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));  // h_best may still be in flight
     GB_CUDA(e, e->d_best.ensure(n));
-    GB_CUDA(e, e->h_best.ensure(n));
-    int rc = gb200_acquire_grid_best_device(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_best.p);
-    if (rc) return rc;
-    GB_CUDA(e, cudaMemcpyAsync(e->h_best.p, e->d_best.p, n * sizeof(BestRecord), cudaMemcpyDeviceToHost, e->stream));
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    memcpy(out_host, e->h_best.p, n * sizeof(BestRecord));
-    return GB200_OK;
+    GB_TRY(gb200_acquire_grid_best_device(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_best.p));
+    return download(e, reinterpret_cast<BestRecord*>(out_host), e->d_best.p, n, e->h_best);
 }
 
 // Host to host in one call.  The first call of a shape runs eagerly (it may have to upload the axes and grow buffers,
@@ -776,13 +814,12 @@ int gb200_acquire_grid_host(gb200_engine* e, const float* iq_host, int n_blocks,
                             const double* dop, int D, int kind, gb200_cell_record* out_host) {
     if (!e) return GB200_EINVAL;
     if (!iq_host || !out_host) GB_FAIL(e, GB200_EINVAL, "null buffer");
-    if (n_blocks < 1 || M < 1 || P < 1 || D < 1 || !prn_idx || !dop) GB_FAIL(e, GB200_EINVAL, "empty grid");
+    GB_TRY(check_grid(e, std::min(n_blocks, M), P, D, prn_idx, dop));  // blocks of no milliseconds make an empty grid too
     GB_CUDA(e, cudaSetDevice(e->device));
     const size_t n_iq = static_cast<size_t>(n_blocks) * M * e->N, n_rec = static_cast<size_t>(n_blocks) * P * D;
     const size_t spec_bytes = unit_floats2(e, M) * D * sizeof(float2) * n_blocks;
     if (e->timing || spec_bytes > e->spec_budget_bytes) {  // several scratch batches / per-kernel events: plain path
-        int rc = gb200_upload_iq(e, iq_host, static_cast<int64_t>(n_iq));
-        if (rc) return rc;
+        GB_TRY(gb200_upload_iq(e, iq_host, static_cast<int64_t>(n_iq)));
         return gb200_acquire_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, out_host);
     }
     GB_CUDA(e, cudaStreamSynchronize(e->stream));  // the pinned staging buffers may still be in flight
@@ -793,64 +830,41 @@ int gb200_acquire_grid_host(gb200_engine* e, const float* iq_host, int n_blocks,
     // Large pinned inputs (a 10-ms window is 327 KB) are copied by the DMA engine straight from the caller's buffer: staging them
     // would cost a host memcpy.  The copy node of the graph has its source baked in, so those calls launch eagerly (a few us
     // more than a replay).  Small inputs are staged and replayed.
-    const float2* h2d_src = e->h_iq.p;
-    bool eager_src = false;
-    if (n_iq * sizeof(float2) > (64u << 10)) {
-        cudaPointerAttributes pa{};
-        if (cudaPointerGetAttributes(&pa, iq_host) == cudaSuccess && pa.type == cudaMemoryTypeHost) {
-            h2d_src = reinterpret_cast<const float2*>(iq_host);
-            eager_src = true;
-        } else {
-            cudaGetLastError();
-        }
-    }
-    if (!eager_src) memcpy(e->h_iq.p, iq_host, n_iq * sizeof(float2));
+    const float2* h2d_src = reinterpret_cast<const float2*>(iq_host);
+    const bool eager_src = n_iq * sizeof(float2) > (64u << 10) && is_pinned(iq_host);
+    if (!eager_src) GB_CUDA(e, stage_in(e->h_iq, h2d_src, n_iq));
     e->iq = e->iq_own.p;
     e->iq_samples = static_cast<int64_t>(n_iq);
 
     // The captured kernels read the axes from d_doppler / d_ints and the replica spectra from crep: make sure those hold THIS
     // grid's axes now (a list-mode call may have reused them since the last replay; cheap when nothing changed), and treat a
     // moved buffer (gb200_set_replicas with a larger table, a larger list-mode call) as a new shape.
-    {
-        if (e->n_prn == 0) GB_FAIL(e, GB200_ESTATE, "no PRN replicas loaded (gb200_set_replicas)");
-        for (int i = 0; i < P; ++i)
-            if (prn_idx[i] < 0 || prn_idx[i] >= e->n_prn) GB_FAIL(e, GB200_EINVAL, "prn index %d out of range", prn_idx[i]);
-        int rc = upload_grid_axes(e, prn_idx, P, dop, D);
-        if (rc) return rc;
-    }
+    GB_TRY(check_replicas(e));
+    GB_TRY(check_prns(e, prn_idx, P));
+    GB_TRY(upload_grid_axes(e, prn_idx, P, dop, D));
     // Small grids: the correlate kernel stores its 32-byte records straight into pinned (device-mapped under UVA) memory --
     // posted PCIe writes at the kernel's tail instead of a separate copy node behind it -- and into the CALLER's buffer when that
     // is itself pinned, which also saves the host copy out of the staging buffer.
     const bool direct = n_rec * sizeof(CellRecord) <= (256u << 10);
-    CellRecord* rec_target = direct ? e->h_records.p : e->d_records.p;
-    bool to_caller = false;
-    if (direct) {
-        cudaPointerAttributes pa{};
-        if (cudaPointerGetAttributes(&pa, out_host) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer) {
-            rec_target = static_cast<CellRecord*>(pa.devicePointer);
-            to_caller = true;
-        } else {
-            cudaGetLastError();
-        }
-    }
+    void* caller_alias = nullptr;
+    const bool to_caller = direct && is_pinned(out_host, &caller_alias) && caller_alias;
+    CellRecord* rec_target = to_caller ? static_cast<CellRecord*>(caller_alias) : direct ? e->h_records.p : e->d_records.p;
     auto& g = e->hg;
-    const bool same = g.seen && g.n_blocks == n_blocks && g.M == M && g.P == P && g.D == D && g.kind == kind &&
-                      g.iq_dev == e->iq_own.p && g.rec_dev == e->d_records.p && g.iq_stage == e->h_iq.p &&
-                      g.rec_stage == e->h_records.p && g.spec == e->spec.p && g.stream == e->stream &&
-                      g.d_dop == e->d_doppler.p && g.d_prn == e->d_ints.p && g.crep == e->crep.p &&
-                      g.rec_target == rec_target &&
-                      memcmp(g.dop.data(), dop, sizeof(double) * D) == 0 && memcmp(g.prn.data(), prn_idx, sizeof(int) * P) == 0;
+    auto key = [&] {
+        return gb200_engine::HostGraph::Key{n_blocks, M, P, D, kind, {dop, dop + D}, {prn_idx, prn_idx + P},
+                                            e->iq_own.p, e->d_records.p, e->h_iq.p, e->h_records.p, e->spec.p,
+                                            e->d_doppler.p, e->d_ints.p, e->crep.p, rec_target, e->stream};
+    };
+    const bool same = g.seen && g.key == key();
     auto enqueue = [&]() -> int {
         GB_CUDA(e, cudaMemcpyAsync(e->iq_own.p, h2d_src, n_iq * sizeof(float2), cudaMemcpyHostToDevice, e->stream));
-        int rc = run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, rec_target);
-        if (rc) return rc;
+        GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, rec_target));
         if (!direct)
             GB_CUDA(e, cudaMemcpyAsync(e->h_records.p, e->d_records.p, n_rec * sizeof(CellRecord), cudaMemcpyDeviceToHost, e->stream));
         return GB200_OK;
     };
     if (eager_src) {
-        int rc = enqueue();
-        if (rc) return rc;
+        GB_TRY(enqueue());
     } else if (same && g.exec) {
         GB_CUDA(e, cudaGraphLaunch(g.exec, e->stream));
         e->launches += 2;
@@ -866,8 +880,7 @@ int gb200_acquire_grid_host(gb200_engine* e, const float* iq_host, int n_blocks,
         if (rc != GB200_OK || ce != cudaSuccess || !g.exec) {
             cudaGetLastError();
             g.exec = nullptr;
-            rc = enqueue();  // capture unavailable: stay on the eager path for this shape
-            if (rc) return rc;
+            GB_TRY(enqueue());  // capture unavailable: stay on the eager path for this shape
         } else {
             GB_CUDA(e, cudaGraphLaunch(g.exec, e->stream));
         }
@@ -876,26 +889,9 @@ int gb200_acquire_grid_host(gb200_engine* e, const float* iq_host, int n_blocks,
             if (g.exec) cudaGraphExecDestroy(g.exec);
             g.exec = nullptr;
         }
-        int rc = enqueue();
-        if (rc) return rc;
+        GB_TRY(enqueue());
         if (!same) {
-            g.n_blocks = n_blocks;
-            g.M = M;
-            g.P = P;
-            g.D = D;
-            g.kind = kind;
-            g.dop.assign(dop, dop + D);
-            g.prn.assign(prn_idx, prn_idx + P);
-            g.iq_dev = e->iq_own.p;
-            g.rec_dev = e->d_records.p;
-            g.iq_stage = e->h_iq.p;
-            g.rec_stage = e->h_records.p;
-            g.spec = e->spec.p;
-            g.d_dop = e->d_doppler.p;
-            g.d_prn = e->d_ints.p;
-            g.crep = e->crep.p;
-            g.rec_target = rec_target;
-            g.stream = e->stream;
+            g.key = key();  // after the run, which may have grown the spectra scratch
             g.seen = 1;
         }
     }
@@ -931,12 +927,7 @@ int gb200_ring_destroy(gb200_ring* r) {
     gb200_engine* e = r->e;
     cudaSetDevice(e->device);
     cudaStreamSynchronize(e->stream);
-    if (e->iq >= r->buf.p && e->iq < r->buf.p + r->buf.cap) {  // the engine was reading the ring: unbind
-        e->iq = nullptr;
-        e->iq_samples = 0;
-    }
-    r->buf.release();
-    r->h_stage.release();
+    unbind_iq(e, r->buf.p, r->buf.cap);
     delete r;
     return GB200_OK;
 }
@@ -949,11 +940,9 @@ int gb200_ring_append(gb200_ring* r, const float* iq_host, int n_ms) {
     GB_CUDA(e, cudaSetDevice(e->device));
     const size_t N = static_cast<size_t>(e->N);
     const float2* src = reinterpret_cast<const float2*>(iq_host);
-    if (!is_pinned_host(iq_host)) {
+    if (!is_pinned(iq_host)) {
         GB_CUDA(e, cudaStreamSynchronize(e->stream));  // staging buffer may still be in flight
-        GB_CUDA(e, r->h_stage.ensure(N * n_ms));
-        memcpy(r->h_stage.p, iq_host, N * n_ms * sizeof(float2));
-        src = r->h_stage.p;
+        GB_CUDA(e, stage_in(r->h_stage, src, N * n_ms));
     }
     int done = 0;
     while (done < n_ms) {
@@ -995,8 +984,7 @@ int gb200_acquire_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, co
     GB_CUDA(e, cudaSetDevice(e->device));
     if (n_cells < 1) GB_FAIL(e, GB200_EINVAL, "empty cell list");
     GB_CUDA(e, e->d_records.ensure(n_cells));
-    int rc = run_cells(e, n_cells, prn_idx, dop, probe, n_ms, kind, e->d_records.p, nullptr);
-    if (rc) return rc;
+    GB_TRY(run_cells(e, n_cells, prn_idx, dop, probe, n_ms, kind, e->d_records.p, nullptr));
     return fetch_records(e, n_cells, out_host);
 }
 
@@ -1006,42 +994,28 @@ int gb200_correlation_profile(gb200_engine* e, int prn, double dop, int n_ms, in
     GB_CUDA(e, cudaSetDevice(e->device));
     const size_t nf = static_cast<size_t>(e->N) * (kind == GB200_COHERENT ? 2 : 1);
     GB_CUDA(e, e->d_profile.ensure(nf));
-    GB_CUDA(e, e->h_profile.ensure(nf));
     GB_CUDA(e, e->d_records.ensure(1));
     const int32_t p = prn;
-    int rc = run_cells(e, 1, &p, &dop, nullptr, n_ms, kind, e->d_records.p, e->d_profile.p);
-    if (rc) return rc;
-    GB_CUDA(e, cudaMemcpyAsync(e->h_profile.p, e->d_profile.p, nf * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    memcpy(out_host, e->h_profile.p, nf * sizeof(float));
-    return GB200_OK;
+    GB_TRY(run_cells(e, 1, &p, &dop, nullptr, n_ms, kind, e->d_records.p, e->d_profile.p));
+    return download(e, out_host, e->d_profile.p, nf, e->h_profile);
 }
 
 int gb200_correlation_profile_replica(gb200_engine* e, const float* replica_host, double dop, int n_ms, int kind,
                                       float* out_host) {
     if (!e) return GB200_EINVAL;
     if (!replica_host || !out_host) GB_FAIL(e, GB200_EINVAL, "null buffer");
-    if (kind != GB200_COHERENT && kind != GB200_NON_COHERENT) GB_FAIL(e, GB200_EINVAL, "Unexpected integration type");
-    if (!e->iq) GB_FAIL(e, GB200_ESTATE, "no IQ loaded (gb200_upload_iq / gb200_bind_iq_device)");
-    if (n_ms < 1) GB_FAIL(e, GB200_EINVAL, "need at least one whole millisecond of samples");
-    if (static_cast<int64_t>(n_ms) * e->N > e->iq_samples)
-        GB_FAIL(e, GB200_EINVAL, "need %lld samples, %lld loaded", static_cast<long long>(n_ms) * e->N,
-                static_cast<long long>(e->iq_samples));
+    GB_TRY(check_kind(e, kind));
+    GB_TRY(check_iq(e, n_ms));
+    GB_TRY(check_samples(e, n_ms));
     GB_CUDA(e, cudaSetDevice(e->device));
     const size_t nf = static_cast<size_t>(e->N) * (kind == GB200_COHERENT ? 2 : 1);
     GB_CUDA(e, cudaStreamSynchronize(e->stream));  // staging buffers may still be in flight
     GB_CUDA(e, e->d_profile.ensure(nf));
-    GB_CUDA(e, e->h_profile.ensure(std::max(nf, static_cast<size_t>(2) * e->N)));
     GB_CUDA(e, e->d_replica.ensure(e->N));
-    memcpy(e->h_profile.p, replica_host, sizeof(float2) * e->N);  // the pinned profile buffer doubles as replica staging
-    GB_CUDA(e, cudaMemcpyAsync(e->d_replica.p, e->h_profile.p, sizeof(float2) * e->N, cudaMemcpyHostToDevice, e->stream));
-    GB_CUDA(e, launch_correlate_generic(e->iq, e->d_replica.p, e->N, n_ms, dop, 1.0 / static_cast<double>(e->fs), kind,
-                                        e->d_profile.p, e->stream));
-    e->launches++;
-    GB_CUDA(e, cudaMemcpyAsync(e->h_profile.p, e->d_profile.p, nf * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    memcpy(out_host, e->h_profile.p, nf * sizeof(float));
-    return GB200_OK;
+    GB_TRY(upload(e, e->d_replica.p, reinterpret_cast<const float2*>(replica_host), e->N, e->h_replica));
+    GB_LAUNCH(e, -1, launch_correlate_generic(e->iq, e->d_replica.p, e->N, n_ms, dop, 1.0 / static_cast<double>(e->fs), kind,
+                                              e->d_profile.p, e->stream));
+    return download(e, out_host, e->d_profile.p, nf, e->h_profile);
 }
 
 int gb200_enable_kernel_timing(gb200_engine* e, int on) {
@@ -1077,14 +1051,10 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
     if (!e) return GB200_EINVAL;
     if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
     GB_CUDA(e, cudaSetDevice(e->device));
-    int rc = check_common(e, n_ms, GB200_NON_COHERENT);
-    if (rc) return rc;
+    GB_TRY(check_common(e, n_ms, GB200_NON_COHERENT));
     if (n_sv < 1 || !prn_idx) GB_FAIL(e, GB200_EINVAL, "no satellites to search for");
-    if (static_cast<int64_t>(n_ms) * e->N > e->iq_samples)
-        GB_FAIL(e, GB200_EINVAL, "need %lld samples, %lld loaded", static_cast<long long>(n_ms) * e->N,
-                static_cast<long long>(e->iq_samples));
-    for (int i = 0; i < n_sv; ++i)
-        if (prn_idx[i] < 0 || prn_idx[i] >= e->n_prn) GB_FAIL(e, GB200_EINVAL, "prn index %d out of range", prn_idx[i]);
+    GB_TRY(check_samples(e, n_ms));
+    GB_TRY(check_prns(e, prn_idx, n_sv));
 
     const int MAXB = kRefineMaxBins;
     const int n_cells = n_sv * MAXB;
@@ -1096,50 +1066,39 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
     int sv_per_chunk = static_cast<int>(std::max<size_t>(1, e->spec_budget_bytes / (unit * sizeof(float2) * MAXB)));
     sv_per_chunk = std::min(sv_per_chunk, n_sv);
 
-    // ---- static plan: cell c = sv*MAXB + b ----
-    // ints: [cell_u n_cells][cell_out n_cells][grp_first][grp_count][grp_prn] (n_sv*gps each)
-    //       then the coherent pass: [ccell_u n_sv][ccell_out n_sv][cgrp_first][cgrp_count][cgrp_prn] (n_sv each), [probe n_sv]
-    const int ng = n_sv * gps;
-    const size_t n_ints = static_cast<size_t>(2) * n_cells + 3 * ng + 6 * n_sv;
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    GB_CUDA(e, e->r_ints.ensure(n_ints));
-    GB_CUDA(e, e->rh_ints.ensure(n_ints));
-    int* hi = e->rh_ints.p;
-    int* cell_u = hi;
-    int* cell_out = cell_u + n_cells;
-    int* g_first = cell_out + n_cells;
-    int* g_count = g_first + ng;
-    int* g_prn = g_count + ng;
-    int* cc_u = g_prn + ng;
-    int* cc_out = cc_u + n_sv;
-    int* cg_first = cc_out + n_sv;
-    int* cg_count = cg_first + n_sv;
-    int* cg_prn = cg_count + n_sv;
+    // Static plans: the refinement passes (cell c = sv*MAXB + b; a chunk's spectra units restart at 0) and the coherent pass
+    // (one cell per satellite), then room for the probe indices the device plans.
+    ListPlan plan, coh;
     for (int sv = 0; sv < n_sv; ++sv) {
         for (int b = 0; b < MAXB; ++b) {
-            cell_u[sv * MAXB + b] = (sv % sv_per_chunk) * MAXB + b;
-            cell_out[sv * MAXB + b] = sv * MAXB + b;
+            plan.cell_u.push_back((sv % sv_per_chunk) * MAXB + b);
+            plan.cell_out.push_back(sv * MAXB + b);
         }
         for (int g = 0; g < gps; ++g) {
-            g_first[sv * gps + g] = sv * MAXB + g * cpg;
-            g_count[sv * gps + g] = std::min(cpg, MAXB - g * cpg);
-            g_prn[sv * gps + g] = prn_idx[sv];
+            plan.grp_first.push_back(sv * MAXB + g * cpg);
+            plan.grp_count.push_back(std::min(cpg, MAXB - g * cpg));
+            plan.grp_prn.push_back(prn_idx[sv]);
         }
-        cc_u[sv] = sv;
-        cc_out[sv] = sv;
-        cg_first[sv] = sv;
-        cg_count[sv] = 1;
-        cg_prn[sv] = prn_idx[sv];
+        coh.cell_u.push_back(sv);
+        coh.cell_out.push_back(sv);
+        coh.grp_first.push_back(sv);
+        coh.grp_count.push_back(1);
+        coh.grp_prn.push_back(prn_idx[sv]);
     }
+    const size_t n_plans = plan.size() + coh.size();
+    GB_CUDA(e, cudaStreamSynchronize(e->stream));
+    GB_CUDA(e, e->r_ints.ensure(n_plans + n_sv));
+    GB_CUDA(e, e->rh_ints.ensure(n_plans + n_sv));
+    plan.write(e->rh_ints.p);
+    coh.write(e->rh_ints.p + plan.size());
     int* di = e->r_ints.p;
-    GB_CUDA(e, cudaMemcpyAsync(di, hi, sizeof(int) * (n_ints - n_sv), cudaMemcpyHostToDevice, e->stream));
-    int* d_probe = di + (n_ints - n_sv);
+    GB_CUDA(e, cudaMemcpyAsync(di, e->rh_ints.p, sizeof(int) * n_plans, cudaMemcpyHostToDevice, e->stream));
+    int* d_probe = di + n_plans;
 
     GB_CUDA(e, e->r_state.ensure(n_sv));
     GB_CUDA(e, e->r_doppler.ensure(static_cast<size_t>(n_cells) + n_sv));
     GB_CUDA(e, e->r_records.ensure(static_cast<size_t>(n_cells) + n_sv));
     GB_CUDA(e, e->r_results.ensure(n_sv));
-    GB_CUDA(e, e->rh_results.ensure(n_sv));
     GB_CUDA(e, e->spec.ensure(unit * std::max(sv_per_chunk * MAXB, n_sv)));
     double* d_coh_doppler = e->r_doppler.p + n_cells;
     CellRecord* d_coh_records = e->r_records.p + n_cells;
@@ -1150,10 +1109,7 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
     FusedArgs fbase{};
     const int* d_cell_prn = nullptr;
     if (use_fused) {
-        if (!e->fused_configured) {
-            GB_CUDA(e, configure_fused_kernel());
-            e->fused_configured = true;
-        }
+        GB_TRY(fused_args(e, n_ms, &fbase));
         // [n_cells] replica row of every (satellite, bin) slot, then [n_sv] one per satellite for the coherent pass
         GB_CUDA(e, e->r_cell_prn.ensure(static_cast<size_t>(n_cells) + n_sv));
         GB_CUDA(e, e->rh_cell_prn.ensure(static_cast<size_t>(n_cells) + n_sv));
@@ -1162,20 +1118,11 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
         GB_CUDA(e, cudaMemcpyAsync(e->r_cell_prn.p, e->rh_cell_prn.p, sizeof(int) * (n_cells + n_sv), cudaMemcpyHostToDevice,
                                    e->stream));
         d_cell_prn = e->r_cell_prn.p;
-        fbase.iq = e->iq;
-        fbase.crep = e->crep.p;
-        fbase.tw1 = e->tw1.p;
-        fbase.tw2 = e->tw2.p;
-        fbase.inv_fs = 1.0 / static_cast<double>(e->fs);
-        fbase.N = e->N;
-        fbase.M = n_ms;
     }
 
-    GB_CUDA(e, launch_refine_init(n_sv, e->r_state.p, e->stream));
-    e->launches++;
+    GB_LAUNCH(e, -1, launch_refine_init(n_sv, e->r_state.p, e->stream));
     for (double spread = 7000.0; spread >= 10.0; spread /= 2.0) {  // acquisition.py:78-89
-        GB_CUDA(e, launch_refine_plan(n_sv, spread, e->r_state.p, e->r_doppler.p, e->stream));
-        e->launches++;
+        GB_LAUNCH(e, -1, launch_refine_plan(n_sv, spread, e->r_state.p, e->r_doppler.p, e->stream));
         if (use_fused) {
             // one launch per pass: a CTA per (satellite, bin) slot, no spectra scratch
             FusedArgs fa = fbase;
@@ -1184,36 +1131,20 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
             fa.probe = nullptr;
             fa.records = e->r_records.p;
             fa.n_cells = n_cells;
-            {
-                TimedLaunch tl(e, 1);
-                GB_CUDA(e, launch_acquire_fused(fa, e->s, GB200_NON_COHERENT, e->stream));
-            }
-            e->launches++;
+            GB_LAUNCH(e, 1, launch_acquire_fused(fa, e->s, GB200_NON_COHERENT, e->stream));
         }
         for (int sv0 = 0; !use_fused && sv0 < n_sv; sv0 += sv_per_chunk) {
             const int nsv = std::min(sv_per_chunk, n_sv - sv0);
-            rc = run_spectra(e, e->iq, n_ms, e->r_doppler.p + static_cast<size_t>(sv0) * MAXB, nsv * MAXB, nsv * MAXB);
-            if (rc) return rc;
+            GB_TRY(run_spectra(e, e->iq, n_ms, e->r_doppler.p + static_cast<size_t>(sv0) * MAXB, nsv * MAXB, nsv * MAXB));
             CorrelateArgs ca = correlate_args(e, n_ms, GB200_NON_COHERENT, rsplit, e->r_records.p, nullptr);
-            ca.n_groups = nsv * gps;
-            ca.cell_u = di;
-            ca.cell_out = di + n_cells;
-            ca.grp_first = di + 2 * n_cells + sv0 * gps;
-            ca.grp_count = di + 2 * n_cells + ng + sv0 * gps;
-            ca.grp_prn = di + 2 * n_cells + 2 * ng + sv0 * gps;
+            plan.bind(ca, di, sv0 * gps, nsv * gps);
             ca.cell_gate = e->r_doppler.p;
-            {
-                TimedLaunch tl(e, 1);
-                GB_CUDA(e, launch_correlate(ca, std::min(ca.n_groups, e->num_sms), e->stream));
-            }
-            e->launches++;
+            GB_LAUNCH(e, 1, launch_correlate(ca, std::min(ca.n_groups, e->num_sms), e->stream));
         }
-        GB_CUDA(e, launch_refine_select(n_sv, e->N, e->r_records.p, e->r_doppler.p, e->r_state.p, e->stream));
-        e->launches++;
+        GB_LAUNCH(e, -1, launch_refine_select(n_sv, e->N, e->r_records.p, e->r_doppler.p, e->r_state.p, e->stream));
     }
     // coherent integration at the kept Doppler (acquisition.py:120-136)
-    GB_CUDA(e, launch_refine_coherent_plan(n_sv, e->r_state.p, d_coh_doppler, d_probe, e->stream));
-    e->launches++;
+    GB_LAUNCH(e, -1, launch_refine_coherent_plan(n_sv, e->r_state.p, d_coh_doppler, d_probe, e->stream));
     if (use_fused) {
         FusedArgs fa = fbase;
         fa.doppler = d_coh_doppler;
@@ -1221,36 +1152,17 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
         fa.probe = d_probe;
         fa.records = d_coh_records;
         fa.n_cells = n_sv;
-        {
-            TimedLaunch tl(e, 1);
-            GB_CUDA(e, launch_acquire_fused(fa, e->s, GB200_COHERENT, e->stream));
-        }
-        e->launches++;
+        GB_LAUNCH(e, 1, launch_acquire_fused(fa, e->s, GB200_COHERENT, e->stream));
     } else {
-        rc = run_spectra(e, e->iq, n_ms, d_coh_doppler, n_sv, n_sv);
-        if (rc) return rc;
-        const int* cbase = di + 2 * n_cells + 3 * ng;
+        GB_TRY(run_spectra(e, e->iq, n_ms, d_coh_doppler, n_sv, n_sv));
         const int crsplit = pick_rsplit(e, correlate_slots(GB200_COHERENT, n_ms, false), n_sv);
         CorrelateArgs ca = correlate_args(e, n_ms, GB200_COHERENT, crsplit, d_coh_records, nullptr);
-        ca.n_groups = n_sv;
-        ca.cell_u = cbase;
-        ca.cell_out = cbase + n_sv;
-        ca.grp_first = cbase + 2 * n_sv;
-        ca.grp_count = cbase + 3 * n_sv;
-        ca.grp_prn = cbase + 4 * n_sv;
+        coh.bind(ca, di + plan.size(), 0, n_sv);
         ca.cell_probe = d_probe;
-        {
-            TimedLaunch tl(e, 1);
-            GB_CUDA(e, launch_correlate(ca, std::min(n_sv, e->num_sms), e->stream));
-        }
-        e->launches++;
+        GB_LAUNCH(e, 1, launch_correlate(ca, std::min(n_sv, e->num_sms), e->stream));
     }
-    GB_CUDA(e, launch_refine_finalize(n_sv, e->r_state.p, d_coh_records, e->r_results.p, e->stream));
-    e->launches++;
-    GB_CUDA(e, cudaMemcpyAsync(e->rh_results.p, e->r_results.p, sizeof(RefineResult) * n_sv, cudaMemcpyDeviceToHost, e->stream));
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    memcpy(out_host, e->rh_results.p, sizeof(RefineResult) * n_sv);
-    return GB200_OK;
+    GB_LAUNCH(e, -1, launch_refine_finalize(n_sv, e->r_state.p, d_coh_records, e->r_results.p, e->stream));
+    return download(e, reinterpret_cast<RefineResult*>(out_host), e->r_results.p, n_sv, e->rh_results);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1262,9 +1174,8 @@ int gb200_tracker_create(gb200_engine* e, int n_channels, const int32_t* prn_idx
     if (!out) GB_FAIL(e, GB200_EINVAL, "null output");
     *out = nullptr;
     if (n_channels < 1 || !prn_idx || !doppler_hz || !carrier_phase || !code_phase) GB_FAIL(e, GB200_EINVAL, "no channels");
-    if (e->n_prn == 0) GB_FAIL(e, GB200_ESTATE, "no PRN replicas loaded (gb200_set_replicas)");
-    for (int c = 0; c < n_channels; ++c)
-        if (prn_idx[c] < 0 || prn_idx[c] >= e->n_prn) GB_FAIL(e, GB200_EINVAL, "prn index %d out of range", prn_idx[c]);
+    GB_TRY(check_replicas(e));
+    GB_TRY(check_prns(e, prn_idx, n_channels));
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_CUDA(e, configure_track_kernel());
     gb200_tracker* t = new gb200_tracker;
@@ -1292,23 +1203,6 @@ int gb200_tracker_destroy(gb200_tracker* t) {
     if (!t) return GB200_OK;
     cudaSetDevice(t->e->device);
     cudaStreamSynchronize(t->e->stream);
-    t->states.release();
-    t->shadow.release();
-    t->d_sel.release();
-    t->h_sel.release();
-    t->d_out.release();
-    t->d_times.release();
-    t->d_prof.release();
-    t->h_out.release();
-    t->h_times.release();
-    t->h_prof.release();
-    t->bit_states.release();
-    t->d_events.release();
-    t->d_counts.release();
-    t->d_bit_times.release();
-    t->h_events.release();
-    t->h_counts.release();
-    t->h_bit_times.release();
     delete t;
     return GB200_OK;
 }
@@ -1319,14 +1213,12 @@ static int tracker_launch(gb200_tracker* t, int n_sel, const int32_t* sel, int n
                           TrackMsRecord* out_dev, float* prof_dev, bool keep_undo) {
     gb200_engine* e = t->e;
     if (n_ms < 1 || !start_times) GB_FAIL(e, GB200_EINVAL, "need at least one whole millisecond of samples");
-    if (!e->iq) GB_FAIL(e, GB200_ESTATE, "no IQ loaded (gb200_upload_iq / gb200_bind_iq_device)");
-    if (static_cast<int64_t>(n_ms) * e->N > e->iq_samples)
-        GB_FAIL(e, GB200_EINVAL, "need %lld samples, %lld loaded", static_cast<long long>(n_ms) * e->N,
-                static_cast<long long>(e->iq_samples));
+    GB_TRY(check_iq(e, n_ms));
+    GB_TRY(check_samples(e, n_ms));
     if (reinterpret_cast<uintptr_t>(e->iq) % 16 != 0) GB_FAIL(e, GB200_EINVAL, "IQ buffer must be 16-byte aligned for tracking");
     if (sel) {
         for (int i = 0; i < n_sel; ++i) {
-            if (sel[i] < 0 || sel[i] >= t->n_channels) GB_FAIL(e, GB200_EINVAL, "channel %d out of range", sel[i]);
+            GB_TRY(check_channel(t, sel[i]));
             if (!t->seeded[sel[i]]) GB_FAIL(e, GB200_ESTATE, "channel %d was never seeded (gb200_tracker_reset_channel)", sel[i]);
             for (int j = 0; j < i; ++j)
                 if (sel[j] == sel[i]) GB_FAIL(e, GB200_EINVAL, "channel %d listed twice", sel[i]);
@@ -1342,9 +1234,7 @@ static int tracker_launch(gb200_tracker* t, int n_sel, const int32_t* sel, int n
     } else {
         GB_CUDA(e, cudaStreamSynchronize(e->stream));  // h_times may still be in flight
         GB_CUDA(e, t->d_times.ensure(n_ms));
-        GB_CUDA(e, t->h_times.ensure(n_ms));
-        memcpy(t->h_times.p, start_times, sizeof(double) * n_ms);
-        GB_CUDA(e, cudaMemcpyAsync(t->d_times.p, t->h_times.p, sizeof(double) * n_ms, cudaMemcpyHostToDevice, e->stream));
+        GB_TRY(upload(e, t->d_times.p, start_times, n_ms, t->h_times));
         a.start_times = t->d_times.p;
     }
     if (sel) {
@@ -1352,9 +1242,7 @@ static int tracker_launch(gb200_tracker* t, int n_sel, const int32_t* sel, int n
         if (!cached) {  // the subset rarely changes between calls: upload it only when it did
             GB_CUDA(e, cudaStreamSynchronize(e->stream));
             GB_CUDA(e, t->d_sel.ensure(n_sel));
-            GB_CUDA(e, t->h_sel.ensure(n_sel));
-            memcpy(t->h_sel.p, sel, sizeof(int) * n_sel);
-            GB_CUDA(e, cudaMemcpyAsync(t->d_sel.p, t->h_sel.p, sizeof(int) * n_sel, cudaMemcpyHostToDevice, e->stream));
+            GB_TRY(upload(e, t->d_sel.p, sel, n_sel, t->h_sel));
             t->sel_cache.assign(sel, sel + n_sel);
         }
         a.channel_idx = t->d_sel.p;
@@ -1376,8 +1264,7 @@ static int tracker_launch(gb200_tracker* t, int n_sel, const int32_t* sel, int n
     a.s = e->s;
     a.n_ms = n_ms;
     a.n_channels = sel ? n_sel : t->n_channels;
-    GB_CUDA(e, launch_track_channels(a, e->stream));
-    e->launches++;
+    GB_LAUNCH(e, -1, launch_track_channels(a, e->stream));
     for (int i = 0; i < a.n_channels; ++i) t->undo_ok[sel ? sel[i] : i] = keep_undo ? 1 : 0;
     return GB200_OK;
 }
@@ -1399,20 +1286,17 @@ static int tracker_process_host(gb200_tracker* t, int n_sel, const int32_t* sel,
     if (n_sel < 1) GB_FAIL(e, GB200_EINVAL, "no channels");
     const size_t n = static_cast<size_t>(n_sel) * n_ms;
     GB_CUDA(e, t->d_out.ensure(n));
-    GB_CUDA(e, t->h_out.ensure(n));
     const size_t np = profiles_host ? n * e->N : 0;
     if (np) {
         GB_CUDA(e, t->d_prof.ensure(np));
         GB_CUDA(e, t->h_prof.ensure(np));
     }
     t->last_n_ms = 0;
-    int rc = tracker_launch(t, n_sel, sel, n_ms, start_times, t->d_out.p, np ? t->d_prof.p : nullptr, keep_undo);
-    if (rc) return rc;
+    GB_TRY(tracker_launch(t, n_sel, sel, n_ms, start_times, t->d_out.p, np ? t->d_prof.p : nullptr, keep_undo));
     if (!sel) t->last_n_ms = n_ms;  // gb200_tracker_integrate_bits reads [channel][n_ms] of the whole bank
-    GB_CUDA(e, cudaMemcpyAsync(t->h_out.p, t->d_out.p, n * sizeof(TrackMsRecord), cudaMemcpyDeviceToHost, e->stream));
+    // the profiles' copy is enqueued first, so the records' download waits for both
     if (np) GB_CUDA(e, cudaMemcpyAsync(t->h_prof.p, t->d_prof.p, np * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    memcpy(out_host, t->h_out.p, n * sizeof(TrackMsRecord));
+    GB_TRY(download(e, reinterpret_cast<TrackMsRecord*>(out_host), t->d_out.p, n, t->h_out));
     if (np) memcpy(profiles_host, t->h_prof.p, np * sizeof(float));
     return GB200_OK;
 }
@@ -1433,7 +1317,7 @@ int gb200_tracker_process_channels(gb200_tracker* t, int n_sel, const int32_t* c
 int gb200_tracker_undo_channel(gb200_tracker* t, int channel) {
     if (!t) return GB200_EINVAL;
     gb200_engine* e = t->e;
-    if (channel < 0 || channel >= t->n_channels) GB_FAIL(e, GB200_EINVAL, "channel %d out of range", channel);
+    GB_TRY(check_channel(t, channel));
     if (!t->undo_ok[channel]) GB_FAIL(e, GB200_ESTATE, "channel %d has no kept state to go back to", channel);
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_CUDA(e, cudaMemcpyAsync(t->states.p + channel, t->shadow.p + channel, sizeof(TrackState), cudaMemcpyDeviceToDevice, e->stream));
@@ -1468,8 +1352,8 @@ int gb200_tracker_reset_channel(gb200_tracker* t, int channel, int32_t prn_idx, 
                                 int32_t code_phase) {
     if (!t) return GB200_EINVAL;
     gb200_engine* e = t->e;
-    if (channel < 0 || channel >= t->n_channels) GB_FAIL(e, GB200_EINVAL, "channel %d out of range", channel);
-    if (prn_idx < 0 || prn_idx >= e->n_prn) GB_FAIL(e, GB200_EINVAL, "prn index %d out of range", prn_idx);
+    GB_TRY(check_channel(t, channel));
+    GB_TRY(check_prns(e, &prn_idx, 1));
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_CUDA(e, cudaStreamSynchronize(e->stream));
     std::vector<TrackState> init(1);
@@ -1485,7 +1369,7 @@ int gb200_tracker_get_state(gb200_tracker* t, int channel, double* doppler_hz, d
                             int32_t* code_phase, int32_t* lost) {
     if (!t) return GB200_EINVAL;
     gb200_engine* e = t->e;
-    if (channel < 0 || channel >= t->n_channels) GB_FAIL(e, GB200_EINVAL, "channel %d out of range", channel);
+    GB_TRY(check_channel(t, channel));
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_CUDA(e, cudaStreamSynchronize(e->stream));
     TrackState st;
@@ -1502,7 +1386,7 @@ int gb200_tracker_set_state(gb200_tracker* t, int channel, double doppler_hz, do
                             int32_t code_phase) {
     if (!t) return GB200_EINVAL;
     gb200_engine* e = t->e;
-    if (channel < 0 || channel >= t->n_channels) GB_FAIL(e, GB200_EINVAL, "channel %d out of range", channel);
+    GB_TRY(check_channel(t, channel));
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_CUDA(e, cudaStreamSynchronize(e->stream));
     TrackState st;
@@ -1541,7 +1425,6 @@ int gb200_tracker_integrate_bits(gb200_tracker* t, int n_ms, const double* start
     }
     const size_t ne = static_cast<size_t>(nc) * max_events;
     GB_CUDA(e, t->d_events.ensure(ne));
-    GB_CUDA(e, t->h_events.ensure(ne));
     GB_CUDA(e, t->d_counts.ensure(nc));
     GB_CUDA(e, t->h_counts.ensure(nc));
     GB_CUDA(e, t->d_bit_times.ensure(2 * static_cast<size_t>(n_ms)));
@@ -1559,12 +1442,10 @@ int gb200_tracker_integrate_bits(gb200_tracker* t, int n_ms, const double* start
     a.n_ms = n_ms;
     a.n_channels = nc;
     a.max_events = max_events;
-    GB_CUDA(e, launch_integrate_bits(a, e->stream));
-    e->launches++;
-    GB_CUDA(e, cudaMemcpyAsync(t->h_events.p, t->d_events.p, ne * sizeof(BitEvent), cudaMemcpyDeviceToHost, e->stream));
+    GB_LAUNCH(e, -1, launch_integrate_bits(a, e->stream));
+    // the counts' copy is enqueued first, so the events' download waits for both
     GB_CUDA(e, cudaMemcpyAsync(t->h_counts.p, t->d_counts.p, nc * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    memcpy(events_host, t->h_events.p, ne * sizeof(BitEvent));
+    GB_TRY(download(e, reinterpret_cast<BitEvent*>(events_host), t->d_events.p, ne, t->h_events));
     memcpy(counts_host, t->h_counts.p, nc * sizeof(int));
     return GB200_OK;
 }
@@ -1572,7 +1453,8 @@ int gb200_tracker_integrate_bits(gb200_tracker* t, int n_ms, const double* start
 int gb200_tracker_bit_state(gb200_tracker* t, int channel, int64_t out[8]) {
     if (!t) return GB200_EINVAL;
     gb200_engine* e = t->e;
-    if (channel < 0 || channel >= t->n_channels || !out) GB_FAIL(e, GB200_EINVAL, "channel %d out of range", channel);
+    GB_TRY(check_channel(t, channel));
+    if (!out) GB_FAIL(e, GB200_EINVAL, "channel %d out of range", channel);
     BitState st;
     memset(&st, 0, sizeof(st));
     bit_state_init(st);
@@ -1602,10 +1484,7 @@ int gb200_grid_stream_destroy(gb200_grid_stream* g) {
     if (g->s_in) cudaStreamSynchronize(g->s_in);
     if (g->s_out) cudaStreamSynchronize(g->s_out);
     for (auto& sl : g->slots) {
-        sl.iq.release();
-        sl.rec.release();
-        sl.h_iq.release();
-        sl.h_rec.release();
+        unbind_iq(g->e, sl.iq.p, sl.iq.cap);  // gb200_grid_stream_submit binds the slot's IQ
         if (sl.h2d) cudaEventDestroy(sl.h2d);
         if (sl.done) cudaEventDestroy(sl.done);
         if (sl.d2h) cudaEventDestroy(sl.d2h);
@@ -1621,12 +1500,10 @@ int gb200_grid_stream_create(gb200_engine* e, int n_blocks, int M, const int32_t
     if (!e) return GB200_EINVAL;
     if (!out) GB_FAIL(e, GB200_EINVAL, "null output");
     *out = nullptr;
-    if (n_blocks < 1 || P < 1 || D < 1 || !prn_idx || !dop) GB_FAIL(e, GB200_EINVAL, "empty grid");
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     if (depth < 1 || depth > 8) GB_FAIL(e, GB200_EINVAL, "depth must be 1..8");
-    int rc = check_common(e, M, kind);
-    if (rc) return rc;
-    for (int i = 0; i < P; ++i)
-        if (prn_idx[i] < 0 || prn_idx[i] >= e->n_prn) GB_FAIL(e, GB200_EINVAL, "prn index %d out of range", prn_idx[i]);
+    GB_TRY(check_common(e, M, kind));
+    GB_TRY(check_prns(e, prn_idx, P));
     GB_CUDA(e, cudaSetDevice(e->device));
     gb200_grid_stream* g = new gb200_grid_stream;
     g->e = e;
@@ -1667,22 +1544,17 @@ int gb200_grid_stream_submit(gb200_grid_stream* g, const float* iq_host, gb200_c
     auto& sl = g->slots[g->head % g->depth];
     const size_t n_iq = static_cast<size_t>(g->n_blocks) * g->M * e->N, n_rec = static_cast<size_t>(g->n_blocks) * g->P * g->D;
     // the slot's previous batch was collected, so its device buffers and staging are free
-    const void* src = iq_host;
-    if (!is_pinned_host(iq_host)) {
-        GB_CUDA(e, sl.h_iq.ensure(n_iq));
-        memcpy(sl.h_iq.p, iq_host, n_iq * sizeof(float2));
-        src = sl.h_iq.p;
-    }
+    const float2* src = reinterpret_cast<const float2*>(iq_host);
+    if (!is_pinned(iq_host)) GB_CUDA(e, stage_in(sl.h_iq, src, n_iq));
     sl.out = out_host;
-    sl.staged_out = !is_pinned_host(out_host);
+    sl.staged_out = !is_pinned(out_host);
     if (sl.staged_out) GB_CUDA(e, sl.h_rec.ensure(n_rec));
     GB_CUDA(e, cudaMemcpyAsync(sl.iq.p, src, n_iq * sizeof(float2), cudaMemcpyHostToDevice, g->s_in));
     GB_CUDA(e, cudaEventRecord(sl.h2d, g->s_in));
     GB_CUDA(e, cudaStreamWaitEvent(e->stream, sl.h2d, 0));
     e->iq = sl.iq.p;
     e->iq_samples = static_cast<int64_t>(n_iq);
-    int rc = run_grid(e, g->n_blocks, g->M, g->prn.data(), g->P, g->dop.data(), g->D, g->kind, sl.rec.p);
-    if (rc) return rc;
+    GB_TRY(run_grid(e, g->n_blocks, g->M, g->prn.data(), g->P, g->dop.data(), g->D, g->kind, sl.rec.p));
     GB_CUDA(e, cudaEventRecord(sl.done, e->stream));
     GB_CUDA(e, cudaStreamWaitEvent(g->s_out, sl.done, 0));
     GB_CUDA(e, cudaMemcpyAsync(sl.staged_out ? reinterpret_cast<gb200_cell_record*>(sl.h_rec.p) : out_host, sl.rec.p,
