@@ -75,6 +75,8 @@ SYMBOLS = {
     "gb200_grid_stream_destroy": (C.c_int, [_P]),
     "gb200_tracker_integrate_bits": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int32, _P]),
     "gb200_tracker_bit_state": (C.c_int, [_P, C.c_int, _P]),
+    "gb200_tracker_decode_subframes": (C.c_int, [_P, _P, _P, C.c_int32, _P, C.c_int32, _P]),
+    "gb200_tracker_subframe_state": (C.c_int, [_P, C.c_int, _P]),
     "gb200_set_fused": (C.c_int, [_P, C.c_int]),
     "gb200_launch_count": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "gb200_enable_kernel_timing": (C.c_int, [_P, C.c_int]),
@@ -471,6 +473,8 @@ class Tracker:
     def undo_channel(self, channel: int) -> None:
         self._engine._check(self._lib.gb200_tracker_undo_channel(self._h, int(channel)), "gb200_tracker_undo_channel")
 
+    _last_bit_stride = 0  # events per channel the last integrate_bits call could hold
+
     def __init__(self, engine: Engine, prn_idx, doppler_hz, carrier_phase, code_phase):
         self._engine = engine
         self._lib = engine._lib
@@ -529,6 +533,7 @@ class Tracker:
                                                    _ptr(ev), cap, _ptr(cnt)), "gb200_tracker_integrate_bits")
         if (cnt > cap).any():
             raise RuntimeError("bit event buffer too small")  # cannot happen: see `cap`
+        self._last_bit_stride = cap
         return [ev[c, : cnt[c]].copy() for c in range(self.n_channels)]
 
     def bit_state(self, channel: int) -> dict:
@@ -539,6 +544,42 @@ class Tracker:
         d = dict(zip(keys, (int(v) for v in out)))
         for k in ("determined_bit_phase", "previous_bit_phase_decision"):
             d[k] = None if d[k] < 0 else d[k]
+        return d
+
+    def decode_subframes(self, bits_device_ptr: int | None = None, counts=None, stride: int | None = None) -> list:
+        """navigation_message_decoder.py:173-196 for every channel over bit events in device memory: by default the
+        ones the last `integrate_bits` call left there; else a device array [n_channels][stride] of BIT_DTYPE with
+        counts[c] events in row c.  Returns one SUBFRAME_DTYPE array per channel (kinds: 0 subframe, 1 determined
+        phase, 2 cannot determine phase, 3 the reference raises; see include/gypsum_b200.h)."""
+        if bits_device_ptr is None:
+            if counts is not None or stride is not None:
+                raise ValueError("counts / stride describe a caller's device array only")
+            n_bits = self._last_bit_stride
+            cnt_in = None
+        else:
+            cnt_in = np.ascontiguousarray(counts, dtype=np.int32)
+            if cnt_in.shape != (self.n_channels,) or stride is None:
+                raise ValueError("a device bit array needs one count per channel and its stride")
+            n_bits = int(cnt_in.max(initial=0))
+        cap = subframe_event_capacity(n_bits)
+        ev = np.empty((self.n_channels, cap), dtype=SUBFRAME_DTYPE)
+        cnt = np.empty(self.n_channels, dtype=np.int32)
+        self._engine._check(
+            self._lib.gb200_tracker_decode_subframes(self._h, None if bits_device_ptr is None else _P(bits_device_ptr),
+                                                     None if cnt_in is None else _ptr(cnt_in), int(stride or 0), _ptr(ev),
+                                                     cap, _ptr(cnt)), "gb200_tracker_decode_subframes")
+        if (cnt > cap).any():
+            raise RuntimeError("subframe event buffer too small")  # cannot happen: see subframe_event_capacity
+        return [ev[c, : cnt[c]].copy() for c in range(self.n_channels)]
+
+    def subframe_state(self, channel: int) -> dict:
+        out = np.zeros(6, dtype=np.int64)
+        self._engine._check(self._lib.gb200_tracker_subframe_state(self._h, channel, _ptr(out)), "gb200_tracker_subframe_state")
+        keys = ("determined_subframe_phase", "emitted_subframe_count", "polarity", "queued_bit_count", "stopped",
+                "processed_bit_count")
+        d = dict(zip(keys, (int(v) for v in out)))
+        if d["determined_subframe_phase"] < 0:
+            d["determined_subframe_phase"] = None
         return d
 
     def get_state(self, channel: int) -> dict:
@@ -557,6 +598,29 @@ BIT_DTYPE = np.dtype([  # gb200_bit_event
     ("receiver_timestamp", "<f8"), ("trailing_edge_receiver_timestamp", "<f8"), ("ms_index", "<i4"), ("bit_value", "<i4"),
     ("slide", "<i4"), ("pad_", "<i4")])
 assert BIT_DTYPE.itemsize == 32
+
+SUBFRAME_DTYPE = np.dtype([  # gb200_subframe_event
+    ("receiver_timestamp", "<f8"), ("trailing_edge_receiver_timestamp", "<f8"), ("words", "<u4", (10,)), ("kind", "<i4"),
+    ("bit_index", "<i4"), ("subframe_id", "<i4"), ("tow", "<i4"), ("phase", "<i4"), ("polarity", "<i4"),
+    ("parity_ok", "<i4"), ("pad_", "<i4", (3,))])
+assert SUBFRAME_DTYPE.itemsize == 96
+SUBFRAME, DETERMINED_PHASE, CANNOT_DETERMINE_PHASE, RAISED = 0, 1, 2, 3  # SUBFRAME_DTYPE["kind"]
+STOP_RAISED, STOP_OVERFLOW, STOP_LOST_LOCK = 1, 2, 3  # Tracker.subframe_state()["stopped"]
+
+
+def subframe_event_capacity(n_bits: int) -> int:
+    """Most events one channel's decoder can produce from n_bits bit events: one phase event per bit at most, where a
+    run of CannotDetermine events spans at most 497 bits (3600..4096 queued) and runs are >= 3300 bits apart, a
+    determined phase needs >= 300 new bits, and the subframes drained come from the queue (<= 4096 bits) plus the new
+    bits."""
+    n = int(n_bits)
+    return min(n, 497 * (1 + n // 3300)) + (1 + n // 300) + (4096 + n) // 300 + 1
+
+
+def subframe_bits(event) -> list[int]:
+    """The 300 upright bits of a SUBFRAME_DTYPE event, IS-GPS-200 bit 1 of word 1 first: the list the reference's
+    NavigationMessageSubframeParser takes."""
+    return [int(w >> (29 - i)) & 1 for w in event["words"] for i in range(30)]
 
 
 def strength_from_records(rec: np.ndarray, n: int) -> np.ndarray:

@@ -16,6 +16,7 @@
 #include "../../include/gypsum_b200.h"
 #include "bits_core.cuh"
 #include "kernels.cuh"
+#include "nav_core.cuh"
 
 using namespace gb;
 
@@ -174,6 +175,15 @@ struct gb200_tracker {
     PinnedBuf<BitEvent> h_events;
     PinnedBuf<int> h_counts;
     PinnedBuf<double> h_bit_times;
+    // the bit events of the last gb200_tracker_integrate_bits call, still in d_events, until they are decoded
+    std::vector<int> bit_counts;
+    int bit_stride = 0;
+    bool bits_pending = false;
+    DevBuf<NavState> nav_states;
+    DevBuf<SubframeEvent> d_sub;
+    DevBuf<int> d_sub_counts, d_bit_counts;
+    PinnedBuf<SubframeEvent> h_sub;
+    PinnedBuf<int> h_sub_counts, h_bit_counts;
 };
 // A pipelined stream of grid batches: slot k's host->device copy, compute and device->host copy run on three streams.
 struct gb200_grid_stream {
@@ -208,6 +218,12 @@ struct gb200_ring {
 static_assert(sizeof(gb200_track_record) == sizeof(TrackMsRecord), "ABI track record and device record must match");
 static_assert(sizeof(gb200_best_record) == sizeof(BestRecord), "ABI best record and device record must match");
 static_assert(sizeof(gb200_bit_event) == sizeof(BitEvent), "ABI bit event and device event must match");
+static_assert(sizeof(gb200_subframe_event) == sizeof(SubframeEvent) && sizeof(SubframeEvent) == 96,
+              "ABI subframe event and device event must match");
+static_assert(offsetof(gb200_subframe_event, words) == offsetof(SubframeEvent, words) &&
+                  offsetof(gb200_subframe_event, kind) == offsetof(SubframeEvent, kind) &&
+                  offsetof(gb200_subframe_event, parity_ok) == offsetof(SubframeEvent, parity_ok),
+              "ABI subframe event and device event must match");
 
 #define GB_FAIL(e, code, ...)                        \
     do {                                             \
@@ -1447,6 +1463,9 @@ int gb200_tracker_integrate_bits(gb200_tracker* t, int n_ms, const double* start
     GB_CUDA(e, cudaMemcpyAsync(t->h_counts.p, t->d_counts.p, nc * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
     GB_TRY(download(e, reinterpret_cast<BitEvent*>(events_host), t->d_events.p, ne, t->h_events));
     memcpy(counts_host, t->h_counts.p, nc * sizeof(int));
+    t->bit_counts.assign(t->h_counts.p, t->h_counts.p + nc);
+    t->bit_stride = max_events;
+    t->bits_pending = true;
     return GB200_OK;
 }
 
@@ -1471,6 +1490,88 @@ int gb200_tracker_bit_state(gb200_tracker* t, int channel, int64_t out[8]) {
     out[5] = st.h.prev_decision;
     out[6] = st.h.cursor;
     out[7] = st.h.stopped;
+    return GB200_OK;
+}
+
+int gb200_tracker_decode_subframes(gb200_tracker* t, const void* bits_device, const int32_t* bit_counts_host,
+                                   int32_t bits_stride, gb200_subframe_event* events_host, int32_t max_events,
+                                   int32_t* counts_host) {
+    if (!t) return GB200_EINVAL;
+    gb200_engine* e = t->e;
+    const int nc = t->n_channels;
+    if (!events_host || !counts_host || max_events < 1) GB_FAIL(e, GB200_EINVAL, "null / empty event buffer");
+    const int* counts = nullptr;
+    int stride = 0;
+    if (bits_device) {
+        if (!bit_counts_host || bits_stride < 1) GB_FAIL(e, GB200_EINVAL, "bit events need their counts and a stride >= 1");
+        for (int c = 0; c < nc; ++c)
+            if (bit_counts_host[c] < 0 || bit_counts_host[c] > bits_stride)
+                GB_FAIL(e, GB200_EINVAL, "channel %d: %d bit events do not fit a stride of %d", c, bit_counts_host[c], bits_stride);
+        counts = bit_counts_host;
+        stride = bits_stride;
+    } else {
+        if (!t->bits_pending) GB_FAIL(e, GB200_ESTATE, "no undecoded bit events on the device (call gb200_tracker_integrate_bits first)");
+        for (int c = 0; c < nc; ++c)
+            if (t->bit_counts[c] > t->bit_stride)
+                GB_FAIL(e, GB200_EINVAL, "channel %d: the last integrate call produced %d bit events but kept %d", c,
+                        t->bit_counts[c], t->bit_stride);
+        counts = t->bit_counts.data();
+        stride = t->bit_stride;
+    }
+    GB_CUDA(e, cudaSetDevice(e->device));
+    GB_CUDA(e, cudaStreamSynchronize(e->stream));  // pinned staging may still be in flight
+    if (!t->nav_states.p) {
+        std::vector<NavState> init(nc);
+        for (int c = 0; c < nc; ++c) {
+            memset(&init[c], 0, sizeof(NavState));
+            nav_state_init(init[c].h);
+        }
+        GB_CUDA(e, t->nav_states.ensure(nc));
+        GB_CUDA(e, cudaMemcpy(t->nav_states.p, init.data(), sizeof(NavState) * nc, cudaMemcpyHostToDevice));
+    }
+    const size_t ne = static_cast<size_t>(nc) * max_events;
+    GB_CUDA(e, t->d_sub.ensure(ne));
+    GB_CUDA(e, t->d_sub_counts.ensure(nc));
+    GB_CUDA(e, t->h_sub_counts.ensure(nc));
+    GB_CUDA(e, t->d_bit_counts.ensure(nc));
+    GB_TRY(upload(e, t->d_bit_counts.p, counts, nc, t->h_bit_counts));
+    NavArgs a{};
+    a.bits = bits_device ? static_cast<const BitEvent*>(bits_device) : t->d_events.p;
+    a.counts = t->d_bit_counts.p;
+    a.bit_states = bits_device ? nullptr : t->bit_states.p;
+    a.states = t->nav_states.p;
+    a.events = t->d_sub.p;
+    a.event_counts = t->d_sub_counts.p;
+    a.stride = stride;
+    a.n_channels = nc;
+    a.max_events = max_events;
+    GB_LAUNCH(e, -1, launch_decode_subframes(a, e->stream));
+    if (!bits_device) t->bits_pending = false;
+    // the counts' copy is enqueued first, so the events' download waits for both
+    GB_CUDA(e, cudaMemcpyAsync(t->h_sub_counts.p, t->d_sub_counts.p, nc * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+    GB_TRY(download(e, reinterpret_cast<SubframeEvent*>(events_host), t->d_sub.p, ne, t->h_sub));
+    memcpy(counts_host, t->h_sub_counts.p, nc * sizeof(int));
+    return GB200_OK;
+}
+
+int gb200_tracker_subframe_state(gb200_tracker* t, int channel, int64_t out[6]) {
+    if (!t) return GB200_EINVAL;
+    gb200_engine* e = t->e;
+    GB_TRY(check_channel(t, channel));
+    if (!out) GB_FAIL(e, GB200_EINVAL, "null output");
+    NavHead h;
+    nav_state_init(h);
+    if (t->nav_states.p) {
+        GB_CUDA(e, cudaSetDevice(e->device));
+        GB_CUDA(e, cudaStreamSynchronize(e->stream));
+        GB_CUDA(e, cudaMemcpy(&h, &t->nav_states.p[channel].h, sizeof(NavHead), cudaMemcpyDeviceToHost));
+    }
+    out[0] = h.phase;
+    out[1] = h.emitted;
+    out[2] = h.polarity;
+    out[3] = h.qlen;
+    out[4] = h.stopped;
+    out[5] = h.bits;
     return GB200_OK;
 }
 

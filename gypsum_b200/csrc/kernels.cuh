@@ -109,6 +109,19 @@ struct BitArgs {
     int n_ms, n_channels, max_events;
 };
 
+// decode_subframes: one warp per channel over its bit events (nav.cu, nav_core.cuh).
+struct NavState;
+struct SubframeEvent;
+struct NavArgs {
+    const BitEvent* bits;        // [n_channels][stride]
+    const int* counts;           // [n_channels] bit events per channel
+    const BitState* bit_states;  // optional: a channel whose integrator stopped stops after these bits
+    NavState* states;            // [n_channels]
+    SubframeEvent* events;       // [n_channels][max_events]
+    int* event_counts;           // [n_channels] events produced (may exceed max_events: truncated)
+    int stride, n_channels, max_events;
+};
+
 // acquire_fused: one CTA per (PRN, Doppler) cell, the whole pipeline in one kernel (fused.cu).
 struct FusedArgs {
     const float2* iq;       // [M*N] one block
@@ -130,6 +143,7 @@ size_t track_smem_bytes(int N, int s);
 cudaError_t configure_track_kernel();
 cudaError_t launch_track_channels(const TrackArgs& a, cudaStream_t st);
 cudaError_t launch_integrate_bits(const BitArgs& a, cudaStream_t st);
+cudaError_t launch_decode_subframes(const NavArgs& a, cudaStream_t st);
 size_t spectra_smem_bytes(int s);
 bool spectra_supports(int s);
 cudaError_t launch_init_tables(float2* tw1, float2* tw2, cudaStream_t st);

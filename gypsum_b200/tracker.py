@@ -350,3 +350,9 @@ class TrackerBank:
         (navigation_bit_intergrator.py:278-288; one integrator per channel, persistent across calls).  Returns one
         _native.BIT_DTYPE array per channel: timestamps of the bit's edges, value 1 / 0 / -1 (unknown)."""
         return self.native.integrate_bits(len(start_times), start_times, end_times)
+
+    def decode_subframes(self) -> list:
+        """Navigation-message subframes of every channel from the bit events the last `integrate_bits` call left on the
+        device (navigation_message_decoder.py:173-196; one decoder per channel, persistent across calls).  Returns one
+        _native.SUBFRAME_DTYPE array per channel; _native.subframe_bits gives an event's 300 upright bits."""
+        return self.native.decode_subframes()

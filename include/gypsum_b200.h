@@ -252,6 +252,46 @@ int gb200_tracker_integrate_bits(gb200_tracker* t, int n_ms, const double* start
  * stopped. */
 int gb200_tracker_bit_state(gb200_tracker* t, int channel, int64_t out[8]);
 
+/* Navigation-message subframe decoding (gypsum/navigation_message_decoder.py), the consumer of the bit events
+ * (satellite_signal_processing_pipeline.py:121-136).  One event, 96 bytes; `kind`:
+ *   0  EmitSubframeEvent: a subframe with a valid TLM prelude and HOW subframe id (:263-269);
+ *   1  DeterminedSubframePhaseEvent (:141): `phase`, `polarity`;
+ *   2  CannotDetermineSubframePhaseEvent (:170): no preamble pair among >= 3600 queued bits, on every such bit;
+ *   3  the reference raises ValueError here (subframe 5 whose data id is not 01, navigation_message_parser.py:626):
+ *      the channel's decoder stops, and events the same bit produced before are dropped, as the exception drops them.
+ * Field parsing (NavigationMessageSubframe1..5) stays with the caller: `words` holds the 300 bits the reference's
+ * NavigationMessageSubframeParser is given.                                                                     */
+typedef struct gb200_subframe_event {
+    double receiver_timestamp;               /* receiver_timestamp of the subframe's first bit             (:203) */
+    double trailing_edge_receiver_timestamp; /* trailing edge of its last bit                              (:204) */
+    uint32_t words[10];   /* the 300 bits after the polarity flip, 30 per word, IS-GPS-200 bit 1 in bit 29       */
+    int32_t kind;         /* 0..3, see above                                                                    */
+    int32_t bit_index;    /* bit event (within this call) whose arrival produced the event                      */
+    int32_t subframe_id;  /* HOW subframe id 1..5 (kinds 0, 3)                                                   */
+    int32_t tow;          /* HOW time-of-week count, 17 bits (kinds 0, 3)                                        */
+    int32_t phase;        /* determined_subframe_phase, -1 = None                                                */
+    int32_t polarity;     /* +1 POSITIVE, -1 NEGATIVE, 0 None                                                   */
+    int32_t parity_ok;    /* bit k: word k+1 meets the IS-GPS-200 parity equations (reported only, as the
+                             reference only logs parity failures)                                             */
+    int32_t pad_[3];
+} gb200_subframe_event;
+typedef char gb200_subframe_event_is_96_bytes[sizeof(gb200_subframe_event) == 96 ? 1 : -1]; /* C99 static assert */
+
+/* NavigationMessageDecoder.process_bit_from_satellite (:173-196) for every channel.  bits_device: a device array
+ * [channel][bits_stride] of gb200_bit_event with bit_counts_host[channel] events per channel, or NULL for the events
+ * the last gb200_tracker_integrate_bits call left on the device (its counts and stride; GB200_ESTATE if there is no
+ * such call not yet decoded, GB200_EINVAL if that call truncated a channel's events).  Each channel keeps one decoder
+ * across calls; with NULL, a channel whose integrator stopped decodes these bits and then stops.  The queue holds at
+ * most 4096 bits: a bit that arrives while 4096 are queued (the reference's queue is unbounded) stops the channel's
+ * decoder.  events_host: [channel][max_events]; counts_host: [channel] events produced (> max_events: truncated). */
+int gb200_tracker_decode_subframes(gb200_tracker* t, const void* bits_device, const int32_t* bit_counts_host,
+                                   int32_t bits_stride, gb200_subframe_event* events_host, int32_t max_events,
+                                   int32_t* counts_host);
+/* one channel's decoder: out[0..5] = determined_subframe_phase (-1 = None), emitted_subframe_count, polarity
+ * (+1 / -1 / 0 = None), queued bits, stopped (0 running, 1 raised, 2 queue overflow, 3 the integrator stopped),
+ * bit events processed. */
+int gb200_tracker_subframe_state(gb200_tracker* t, int channel, int64_t out[6]);
+
 /* Kernel selection for gb200_acquire_cells.  Two implementations of the same arithmetic exist:
  *   0  doppler_spectra + correlate_cells: the PRN-independent half of the pipeline (wipe-off, forward transform) is
  *      computed once per distinct Doppler bin and shared by every PRN -- the grid shape (gb200_acquire_grid always

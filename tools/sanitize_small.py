@@ -37,7 +37,24 @@ for n, m in ((2046, 2), (4092, 1)):
         for _ in range(9):  # > 80 symbols: bit-phase search and bit emission of the navigation-bit kernel
             t.process(12, ts)
             bits = t.integrate_bits(12, ts, ts + 0.001)
+            sub = t.decode_subframes()  # subframe decoding of the bits just integrated
         assert len(bits) == 2 and t.bit_state(0)["processed_pseudosymbol_count"] == 108
+        # subframe decoding over caller bit events: full warp preamble scan, phase, drain, a reset and a re-sync
+        import torch
+
+        nb = 1400
+        sb = np.zeros((2, nb), dtype=_native.BIT_DTYPE)
+        pre = [1, 0, 0, 0, 1, 0, 1, 1]
+        vals = np.random.default_rng(1).integers(0, 2, nb)
+        for at in range(0, nb - 8, 300):
+            vals[at:at + 8] = pre
+        vals[650] = -1
+        sb["bit_value"] = [vals, np.where(vals < 0, vals, 1 - vals)]
+        sb["receiver_timestamp"] = np.arange(nb) * 0.02
+        sb["trailing_edge_receiver_timestamp"] = np.arange(nb) * 0.02 + 0.02
+        sbd = torch.from_numpy(sb.view(np.uint8).reshape(2, -1)).cuda()
+        sub = t.decode_subframes(sbd.data_ptr(), [nb, nb - 100], nb)
+        assert t.subframe_state(0)["processed_bit_count"] >= 600 and len(sub) == 2
         t.close()
         # pipelined batch stream: three streams, pageable staging
         gs = _native.GridStream(eng, 2, 1, [24, 0, 5], dop, _native.NON_COHERENT, depth=2)
