@@ -701,7 +701,9 @@ int gb200_create(int device, int fs, int n, gb200_engine** out) {
     }
     e->num_sms = prop.multiProcessorCount;
     if (!spectra_supports(e->s)) {
-        g_create_error = "samples_per_ms / 1023 must be one of 1,2,3,4,5,6,8,10,12,16";
+#define GB_RATE_TEXT(S) "," #S
+        g_create_error = std::string("samples_per_ms / 1023 must be one of ") + (GB_FOR_EACH_RATE(GB_RATE_TEXT) + 1);  // "1,2,..."
+#undef GB_RATE_TEXT
         delete e;
         return GB200_EINVAL;
     }

@@ -15,16 +15,6 @@
 
 namespace gb {
 
-struct FusedPartial {
-    float mx;
-    int idx;
-    int cnt;
-    float pr_re;
-    double sum;
-    float pr_im;
-    int pad;
-};
-
 // Shared memory per CTA (2.046 Msps): IQ chunk 16 KB + replica spectrum 16 KB + 4 transpose tiles 34 KB = 67 KB, so
 // three CTAs (12 transform warps) share an SM.  The polyphase rows live inside the tile area (they are dead once the
 // transforms start) and the twiddle tables are read through L1 from global memory (every CTA reads the same 16 KB).
@@ -39,7 +29,7 @@ __global__ void __launch_bounds__(2 * S * 32, (S == 2 ? 3 : 1)) k_acquire_fused(
     float2* ypoly = tiles;                 // [S][1024] aliases the tiles: written by the wipe-off, read by build_z only
     const float2* __restrict__ tw1_s = a.tw1;
     const float2* __restrict__ tw2_s = a.tw2;
-    FusedPartial* partial = reinterpret_cast<FusedPartial*>(tiles + kWarps * kTileF2);  // [2S]
+    PeakPartial* partial = reinterpret_cast<PeakPartial*>(tiles + kWarps * kTileF2);    // [2S]
     float2* coarse = reinterpret_cast<float2*>(partial + kWarps);                      // [32]
     uint64_t* mbar = reinterpret_cast<uint64_t*>(coarse + 32);                          // [2]: tables, IQ chunk
 
@@ -145,62 +135,20 @@ __global__ void __launch_bounds__(2 * S * 32, (S == 2 ? 3 : 1)) k_acquire_fused(
     float fsum;
     thread_peak16(v, lane, h, S, r, pk, fsum);
     pk.sum = static_cast<double>(fsum);
-    {
-        const int bits = __float_as_int(pk.mx);
-        const int mb = __reduce_max_sync(0xffffffffu, bits);
-        const bool is = bits == mb;
-        pk.idx = __reduce_min_sync(0xffffffffu, is ? pk.idx : 0x7fffffff);
-        pk.cnt = __reduce_add_sync(0xffffffffu, is ? pk.cnt : 0);
-        pk.mx = __int_as_float(mb);
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) {
-            pk.sum += __shfl_xor_sync(0xffffffffu, pk.sum, off);
-            pr_re += __shfl_xor_sync(0xffffffffu, pr_re, off);
-            pr_im += __shfl_xor_sync(0xffffffffu, pr_im, off);
-        }
-    }
-    if (lane == 0) {
-        FusedPartial pp;
-        pp.mx = pk.mx;
-        pp.idx = pk.idx;
-        pp.cnt = pk.cnt;
-        pp.sum = pk.sum;
-        pp.pr_re = pr_re;
-        pp.pr_im = pr_im;
-        pp.pad = 0;
-        partial[warp] = pp;
-    }
+    warp_reduce_peak(pk);
+    warp_reduce_probe(pr_re, pr_im);
+    if (lane == 0) store_partial(partial + warp, pk, pr_re, pr_im);
     __syncthreads();
     if (tid == 0) {
-        Peak m;
-        peak_init(m);
-        float pre = 0.f, pim = 0.f;
-        for (int w = 0; w < kWarps; ++w) {
-            const FusedPartial pp = partial[w];
-            Peak o;
-            o.mx = pp.mx;
-            o.idx = pp.idx;
-            o.cnt = pp.cnt;
-            o.sum = pp.sum;
-            peak_merge(m, o);
-            pre += pp.pr_re;
-            pim += pp.pr_im;
-        }
-        CellRecord rec;
-        rec.peak = m.mx;
-        rec.argmax = m.idx;
-        rec.sum = m.sum;
-        rec.count = m.cnt;
-        rec.probe_re = pre;
-        rec.probe_im = pim;
-        rec.pad_ = 0;
-        a.records[cell] = rec;
+        float pre, pim;
+        const Peak m = merge_partials(partial, kWarps, pre, pim);
+        write_record(a.records + cell, m, pre, pim);
     }
 }
 
 size_t fused_smem_bytes(int N, int s) {
     return (static_cast<size_t>(N) + 2 * kFft + 2 * static_cast<size_t>(s) * kTileF2 + 32) * sizeof(float2) +
-           2 * s * sizeof(FusedPartial) + 32;
+           2 * s * sizeof(PeakPartial) + 32;
 }
 
 bool fused_supports(int s) { return s == 2 || s == 4; }

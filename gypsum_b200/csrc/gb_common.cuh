@@ -11,6 +11,10 @@
 #define GB_INLINE inline
 #endif
 
+// The sample rates the engine supports, as samples per millisecond / 1023: X(S) once per rate.  Every rate switch, kernel
+// configuration and the error message for an unsupported rate expand this one list.
+#define GB_FOR_EACH_RATE(X) X(1) X(2) X(3) X(4) X(5) X(6) X(8) X(10) X(12) X(16)
+
 namespace gb {
 
 constexpr int kChips = 1023;   // constants.py:7  PRN_CHIP_COUNT
@@ -66,6 +70,65 @@ GB_HD GB_INLINE void peak_merge(Peak& a, const Peak& b) {
         a.idx = b.idx < a.idx ? b.idx : a.idx;
     }
     a.sum += b.sum;
+}
+
+// One warp's (or warp pair's) peak and probe share, exchanged through shared memory when several work on one cell.
+struct PeakPartial {
+    float mx;
+    int idx;
+    int cnt;
+    float pr_re;
+    double sum;
+    float pr_im;
+    int pad;
+};
+
+GB_HD GB_INLINE void store_partial(PeakPartial* dst, const Peak& p, float pr_re, float pr_im) {
+    PeakPartial pp;
+    pp.mx = p.mx;
+    pp.idx = p.idx;
+    pp.cnt = p.cnt;
+    pp.sum = p.sum;
+    pp.pr_re = pr_re;
+    pp.pr_im = pr_im;
+    pp.pad = 0;
+    *dst = pp;
+}
+
+// Merges n partials in order (first index wins ties, counts and sums add) and sums their probe shares.
+GB_HD GB_INLINE Peak merge_partials(const PeakPartial* part, int n, float& pr_re, float& pr_im) {
+    Peak m;
+    peak_init(m);
+    pr_re = pr_im = 0.f;
+    for (int w = 0; w < n; ++w) {
+        const PeakPartial pp = part[w];
+        Peak o;
+        o.mx = pp.mx;
+        o.idx = pp.idx;
+        o.cnt = pp.cnt;
+        o.sum = pp.sum;
+        peak_merge(m, o);
+        pr_re += pp.pr_re;
+        pr_im += pp.pr_im;
+    }
+    return m;
+}
+
+GB_HD GB_INLINE void write_record(CellRecord* dst, const Peak& p, float probe_re, float probe_im) {
+    CellRecord rec;
+    rec.peak = p.mx;
+    rec.argmax = p.idx;
+    rec.sum = p.sum;
+    rec.count = p.cnt;
+    rec.probe_re = probe_re;
+    rec.probe_im = probe_im;
+    rec.pad_ = 0;
+    *dst = rec;
+}
+
+// Correlation strength of a profile (utils.py:111-116): its peak over the mean of the values not equal to the peak.
+GB_HD GB_INLINE double record_strength(double peak, double sum, int count, int N) {
+    return peak / ((sum - count * peak) / (N - count));
 }
 
 }  // namespace gb

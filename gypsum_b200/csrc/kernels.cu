@@ -155,27 +155,59 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 5 : 1) k_doppler_
 // ---------------------------------------------------------------------------------------------------------
 // correlate_cells
 // ---------------------------------------------------------------------------------------------------------
-struct PairPartial {  // exchanged through shared memory when several pairs share a cell
-    float mx;
-    int idx;
-    int cnt;
-    float pr_re;
-    double sum;
-    float pr_im;
-    int pad;
+// Both correlate kernels walk a contiguous range of groups per CTA; every slot (warp pair or warp) of the CTA takes one
+// cell of a group, all on the group's PRN.
+struct GroupCell {
+    int prn, unit, out;  // PRN, spectrum unit, record slot
+    bool active;         // the slot has a cell and the gate has not switched it off
 };
 
-// Warp-level merge of per-thread peaks: REDUX for (max, first index, count), shuffles for the float64 sum.
-// Profile values are >= 0 (an excluded slot holds -1), so their IEEE bit patterns order like signed ints.
-__device__ __forceinline__ void warp_reduce_peak(Peak& p) {
-    const int bits = __float_as_int(p.mx);
-    const int mb = __reduce_max_sync(0xffffffffu, bits);
-    const bool is = bits == mb;
-    p.idx = __reduce_min_sync(0xffffffffu, is ? p.idx : 0x7fffffff);
-    p.cnt = __reduce_add_sync(0xffffffffu, is ? p.cnt : 0);
-    p.mx = __int_as_float(mb);
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) p.sum += __shfl_xor_sync(0xffffffffu, p.sum, off);
+// Decodes group g for the slot working on cell my_cell of it.  Grid mode: the group is chunk chunk0 + gch of PRN list entry
+// gpl, a chunk being cells_per_group consecutive cells of the PRN's flat (block, Doppler) list; gpl / gch then step to the
+// next group, with n_chunks chunks per PRN.  List mode reads the sorted group and cell tables.
+__device__ __forceinline__ GroupCell decode_group(const CorrelateArgs& a, int g, int cells_per_group, int my_cell, int chunk0,
+                                                  int n_chunks, int& gpl, int& gch) {
+    GroupCell gc;
+    int n_cells;
+    gc.unit = gc.out = 0;
+    if (a.grid_mode) {
+        gc.prn = a.prn_idx[gpl];
+        const int first = (chunk0 + gch) * cells_per_group;
+        n_cells = min(cells_per_group, a.n_blocks * a.D - first);
+        const int c = first + my_cell;
+        const int b = c / a.D, d = c - b * a.D;
+        gc.unit = c;  // = b * D + d
+        gc.out = (b * a.P + gpl) * a.D + d;
+        if (++gch == n_chunks) {
+            gch = 0;
+            ++gpl;
+        }
+    } else {
+        gc.prn = a.grp_prn[g];
+        n_cells = a.grp_count[g];
+        if (my_cell < n_cells) {
+            const int c = a.grp_first[g] + my_cell;
+            gc.unit = a.cell_u[c];
+            gc.out = a.cell_out[c];
+        }
+    }
+    gc.active = my_cell < n_cells;
+    if (gc.active && a.cell_gate) gc.active = !isnan(a.cell_gate[gc.out]);
+    return gc;
+}
+
+// Stages conj(FFT(replica)) of a new PRN into crep_s with a TMA bulk copy once every warp is done with the previous one, then
+// de-phases the warps by stagger_ns: warps that restart in step after the CTA-wide barrier convoy on the shared-memory pipe.
+__device__ __forceinline__ void stage_replica(const CorrelateArgs& a, int prn, float2* crep_s, uint64_t* mbar, uint32_t& parity,
+                                              unsigned stagger_ns) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        mbar_expect_tx(mbar, 2 * kFft * sizeof(float2));
+        bulk_g2s(crep_s, a.crep + static_cast<size_t>(prn) * 2 * kFft, 2 * kFft * sizeof(float2), mbar);
+    }
+    mbar_wait(mbar, parity);
+    parity ^= 1;
+    __nanosleep(stagger_ns);
 }
 
 constexpr int kPairs = 8;  // warp pairs per k_correlate_cells CTA
@@ -187,7 +219,7 @@ __global__ void __launch_bounds__(kPairs * 64, 1) k_correlate_cells(const Correl
     float2* tw1_s = crep_s + 2 * kFft;     // [32][32]
     float2* tw2_s = tw1_s + kFft;          // [1024]
     float2* tiles = tw2_s + kFft;          // [2*kPairs][kTileF2]
-    PairPartial* partial = reinterpret_cast<PairPartial*>(tiles + 2 * kPairs * kTileF2);  // [2*kPairs]
+    PeakPartial* partial = reinterpret_cast<PeakPartial*>(tiles + 2 * kPairs * kTileF2);  // [2*kPairs]
     uint64_t* mbar = reinterpret_cast<uint64_t*>(partial + 2 * kPairs);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -223,47 +255,14 @@ __global__ void __launch_bounds__(kPairs * 64, 1) k_correlate_cells(const Correl
         gpl = g0 / a.chunks;
         gch = g0 - gpl * a.chunks;
     }
-    const int cells_per_prn = a.n_blocks * a.D;
 
     for (int g = g0; g < g1; ++g) {
-        // ---- decode the group (uniform across the CTA) ----
-        int prn, n_cells, unit = 0, out = 0;
-        if (a.grid_mode) {
-            prn = a.prn_idx[gpl];
-            n_cells = min(cells_per_group, cells_per_prn - gch * cells_per_group);
-            const int c = gch * cells_per_group + my_cell;  // flat (block, doppler) index within this PRN
-            const int b = c / a.D, d = c - b * a.D;
-            unit = c;  // = b * D + d
-            out = (b * a.P + gpl) * a.D + d;
-            if (++gch == a.chunks) {
-                gch = 0;
-                ++gpl;
-            }
-        } else {
-            prn = a.grp_prn[g];
-            n_cells = a.grp_count[g];
-            if (my_cell < n_cells) {
-                const int c = a.grp_first[g] + my_cell;
-                unit = a.cell_u[c];
-                out = a.cell_out[c];
-            }
-        }
-        bool active = my_cell < n_cells;
-        if (active && a.cell_gate) active = !isnan(a.cell_gate[out]);
-
-        // ---- stage conj(FFT(replica)) of this PRN: TMA bulk copy into shared memory ----
-        if (prn != cur_prn) {
-            __syncthreads();  // everyone is done with the previous replica
-            if (threadIdx.x == 0) {
-                mbar_expect_tx(mbar, 2 * kFft * sizeof(float2));
-                bulk_g2s(crep_s, a.crep + static_cast<size_t>(prn) * 2 * kFft, 2 * kFft * sizeof(float2), mbar);
-            }
-            mbar_wait(mbar, parity);
-            parity ^= 1;
-            cur_prn = prn;
-            // De-phase the pairs after the CTA-wide barrier: warps that restart in step convoy on the shared-memory
-            // pipe.
-            __nanosleep(pair * 300);
+        const GroupCell gc = decode_group(a, g, cells_per_group, my_cell, 0, a.chunks, gpl, gch);
+        const bool active = gc.active;
+        const int unit = gc.unit, out = gc.out;
+        if (gc.prn != cur_prn) {
+            stage_replica(a, gc.prn, crep_s, mbar, parity, pair * 300);
+            cur_prn = gc.prn;
         }
 
         if (active) {
@@ -347,24 +346,8 @@ __global__ void __launch_bounds__(kPairs * 64, 1) k_correlate_cells(const Correl
                 }
             }
             warp_reduce_peak(pk);
-            if (KIND == kKindCoherent) {
-#pragma unroll
-                for (int off = 16; off > 0; off >>= 1) {
-                    pr_re += __shfl_xor_sync(0xffffffffu, pr_re, off);
-                    pr_im += __shfl_xor_sync(0xffffffffu, pr_im, off);
-                }
-            }
-            if (lane == 0) {
-                PairPartial pp;
-                pp.mx = pk.mx;
-                pp.idx = pk.idx;
-                pp.cnt = pk.cnt;
-                pp.sum = pk.sum;
-                pp.pr_re = pr_re;
-                pp.pr_im = pr_im;
-                pp.pad = 0;
-                partial[warp] = pp;
-            }
+            if (KIND == kKindCoherent) warp_reduce_probe(pr_re, pr_im);
+            if (lane == 0) store_partial(partial + warp, pk, pr_re, pr_im);
         }
         // ---- merge the 2*rsplit warp partials of each cell and write its record ----
         if (a.rsplit == 1) {
@@ -373,29 +356,9 @@ __global__ void __launch_bounds__(kPairs * 64, 1) k_correlate_cells(const Correl
             __syncthreads();
         }
         if (active && (pair % a.rsplit) == 0 && h == 0 && lane == 0) {
-            Peak m;
-            peak_init(m);
-            float pre = 0.f, pim = 0.f;
-            for (int w = 0; w < 2 * a.rsplit; ++w) {
-                const PairPartial pp = partial[warp + w];
-                Peak o;
-                o.mx = pp.mx;
-                o.idx = pp.idx;
-                o.cnt = pp.cnt;
-                o.sum = pp.sum;
-                peak_merge(m, o);
-                pre += pp.pr_re;
-                pim += pp.pr_im;
-            }
-            CellRecord rec;
-            rec.peak = m.mx;
-            rec.argmax = m.idx;
-            rec.sum = m.sum;
-            rec.count = m.cnt;
-            rec.probe_re = pre;
-            rec.probe_im = pim;
-            rec.pad_ = 0;
-            a.records[out] = rec;
+            float pre, pim;
+            const Peak m = merge_partials(partial + warp, 2 * a.rsplit, pre, pim);
+            write_record(a.records + out, m, pre, pim);
         }
         if (a.rsplit != 1) __syncthreads();  // partial[] is free again
         // rsplit == 1: the next write to partial[] comes after at least two more pair barriers
@@ -416,7 +379,7 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
     float2* crep_s = smem;              // [2][1024]
     float2* tw1_s = crep_s + 2 * kFft;  // [32][32]
     float2* tiles = tw1_s + kFft;       // [NW][kTile64F2]
-    PairPartial* partial = reinterpret_cast<PairPartial*>(tiles + NW * kTile64F2);  // [NW]
+    PeakPartial* partial = reinterpret_cast<PeakPartial*>(tiles + NW * kTile64F2);  // [NW]
     uint64_t* mbar = reinterpret_cast<uint64_t*>(partial + NW);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -446,7 +409,6 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
     // unit happen while the CTAs are inside the same window, so the unit is fetched from HBM once instead of ~8 times (a
     // 256-block batch carries 344 MB of spectra).  There is no barrier between windows; the split below keeps every CTA within
     // one group of the others over the whole batch.
-    const int cells_per_prn = a.n_blocks * a.D;
     const int wch = (a.grid_mode && a.win_chunks > 0 && a.win_chunks < a.chunks) ? a.win_chunks : a.chunks;
     const int n_win = a.grid_mode ? (a.chunks + wch - 1) / wch : 1;
     for (int w = 0; w < n_win; ++w) {
@@ -474,42 +436,12 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
     }
 
     for (int g = g0; g < g1; ++g) {
-        int prn, n_cells, unit = 0, out = 0;
-        if (a.grid_mode) {
-            prn = a.prn_idx[gpl];
-            const int first = (w * wch + gch) * cells_per_group;  // first cell of this chunk in the PRN's flat (block, doppler) list
-            n_cells = min(cells_per_group, cells_per_prn - first);
-            const int c = first + my_cell;
-            const int b = c / a.D, d = c - b * a.D;
-            unit = c;  // = b * D + d
-            out = (b * a.P + gpl) * a.D + d;
-            if (++gch == ch_w) {
-                gch = 0;
-                ++gpl;
-            }
-        } else {
-            prn = a.grp_prn[g];
-            n_cells = a.grp_count[g];
-            if (my_cell < n_cells) {
-                const int c = a.grp_first[g] + my_cell;
-                unit = a.cell_u[c];
-                out = a.cell_out[c];
-            }
-        }
-        bool active = my_cell < n_cells;
-        if (active && a.cell_gate) active = !isnan(a.cell_gate[out]);
-
-        if (prn != cur_prn) {
-            __syncthreads();
-            if (threadIdx.x == 0) {
-                mbar_expect_tx(mbar, 2 * kFft * sizeof(float2));
-                bulk_g2s(crep_s, a.crep + static_cast<size_t>(prn) * 2 * kFft, 2 * kFft * sizeof(float2), mbar);
-            }
-            mbar_wait(mbar, parity);
-            parity ^= 1;
-            cur_prn = prn;
-            // de-phase the warps after the CTA-wide barrier (they would otherwise hit their memory phases together)
-            __nanosleep((warp >> 2) * a.stag_a + (warp & 3) * a.stag_b);
+        const GroupCell gc = decode_group(a, g, cells_per_group, my_cell, w * wch, ch_w, gpl, gch);
+        const bool active = gc.active;
+        const int unit = gc.unit, out = gc.out;
+        if (gc.prn != cur_prn) {
+            stage_replica(a, gc.prn, crep_s, mbar, parity, (warp >> 2) * a.stag_a + (warp & 3) * a.stag_b);
+            cur_prn = gc.prn;
         }
 
         if (active) {
@@ -555,49 +487,15 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
             }
             warp_reduce_peak(pk);
             if (lane == 0) {
-                if (a.rsplit == 1) {
-                    CellRecord rec;
-                    rec.peak = pk.mx;
-                    rec.argmax = pk.idx;
-                    rec.sum = pk.sum;
-                    rec.count = pk.cnt;
-                    rec.probe_re = rec.probe_im = 0.f;
-                    rec.pad_ = 0;
-                    a.records[out] = rec;
-                } else {
-                    PairPartial pp;
-                    pp.mx = pk.mx;
-                    pp.idx = pk.idx;
-                    pp.cnt = pk.cnt;
-                    pp.sum = pk.sum;
-                    pp.pr_re = pp.pr_im = 0.f;
-                    pp.pad = 0;
-                    partial[warp] = pp;
-                }
+                if (a.rsplit == 1) write_record(a.records + out, pk, 0.f, 0.f);
+                else store_partial(partial + warp, pk, 0.f, 0.f);
             }
         }
         if (a.rsplit != 1) {
             __syncthreads();
             if (active && (warp % a.rsplit) == 0 && lane == 0) {
-                Peak m;
-                peak_init(m);
-                for (int w = 0; w < a.rsplit; ++w) {
-                    const PairPartial pp = partial[warp + w];
-                    Peak o;
-                    o.mx = pp.mx;
-                    o.idx = pp.idx;
-                    o.cnt = pp.cnt;
-                    o.sum = pp.sum;
-                    peak_merge(m, o);
-                }
-                CellRecord rec;
-                rec.peak = m.mx;
-                rec.argmax = m.idx;
-                rec.sum = m.sum;
-                rec.count = m.cnt;
-                rec.probe_re = rec.probe_im = 0.f;
-                rec.pad_ = 0;
-                a.records[out] = rec;
+                float pre, pim;  // no probes in a non-coherent launch
+                write_record(a.records + out, merge_partials(partial + warp, a.rsplit, pre, pim), 0.f, 0.f);
             }
             __syncthreads();
         }
@@ -703,8 +601,7 @@ __global__ void k_refine_select(int n_sv, int N, const CellRecord* rec, const do
     }
     if (best < 0) return;
     const CellRecord r = rec[sv * kRefineMaxBins + best];
-    const double peak = static_cast<double>(r.peak);
-    const double strength = peak / ((r.sum - r.count * peak) / (N - r.count));  // utils.py:111-116
+    const double strength = record_strength(r.peak, r.sum, r.count, N);
     RefineState s = st[sv];
     s.center = doppler[sv * kRefineMaxBins + best];
     if (!s.have_kept || strength > s.kept_strength) {
@@ -753,10 +650,9 @@ __global__ void k_best_bins(int n_rows, int D, int N, const CellRecord* rec, con
         }
     }
     const CellRecord w = r[best];
-    const double peak = static_cast<double>(w.peak);
     BestRecord o;
     o.doppler = doppler[best];
-    o.strength = peak / ((w.sum - w.count * peak) / (N - w.count));  // utils.py:111-116
+    o.strength = record_strength(w.peak, w.sum, w.count, N);
     o.peak = w.peak;
     o.code_phase = w.argmax;
     o.bin = best;
@@ -798,17 +694,19 @@ size_t spectra_smem_bytes(int s) {
     return (static_cast<size_t>(spec_f2(s)) + kCarrierTable) * sizeof(float2);
 }
 size_t correlate_smem_bytes() {
-    return (4 * static_cast<size_t>(kFft) + 2 * kPairs * kTileF2) * sizeof(float2) + 2 * kPairs * sizeof(PairPartial) + 16;
+    return (4 * static_cast<size_t>(kFft) + 2 * kPairs * kTileF2) * sizeof(float2) + 2 * kPairs * sizeof(PeakPartial) + 16;
 }
 
 size_t correlate_w2048_smem_bytes(int nw) {
     return (3 * static_cast<size_t>(kFft) + static_cast<size_t>(nw) * kTile64F2) * sizeof(float2) +
-           nw * sizeof(PairPartial) + 16;
+           nw * sizeof(PeakPartial) + 16;
 }
 
 bool spectra_supports(int s) {
     switch (s) {
-        case 1: case 2: case 3: case 4: case 5: case 6: case 8: case 10: case 12: case 16: return true;
+#define GB_CASE(S) case S:
+        GB_FOR_EACH_RATE(GB_CASE) return true;
+#undef GB_CASE
         default: return false;
     }
 }
@@ -821,7 +719,7 @@ static cudaError_t spectra_attr() {
 cudaError_t configure_kernels() {
     cudaError_t e;
 #define GB_ATTR(S) if ((e = spectra_attr<S>()) != cudaSuccess) return e;
-    GB_ATTR(1) GB_ATTR(2) GB_ATTR(3) GB_ATTR(4) GB_ATTR(5) GB_ATTR(6) GB_ATTR(8) GB_ATTR(10) GB_ATTR(12) GB_ATTR(16)
+    GB_FOR_EACH_RATE(GB_ATTR)
 #undef GB_ATTR
     const int sm = static_cast<int>(correlate_smem_bytes());
     if ((e = cudaFuncSetAttribute(k_correlate_cells<kKindCoherent, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm))) return e;
@@ -847,7 +745,7 @@ cudaError_t launch_doppler_spectra(const SpectraArgs& a, cudaStream_t st) {
     const size_t sm = spectra_smem_bytes(a.s);
     switch (a.s) {
 #define GB_CASE(S) case S: k_doppler_spectra<S><<<grid, spec_warps(S) * 32, sm, st>>>(a); break;
-        GB_CASE(1) GB_CASE(2) GB_CASE(3) GB_CASE(4) GB_CASE(5) GB_CASE(6) GB_CASE(8) GB_CASE(10) GB_CASE(12) GB_CASE(16)
+        GB_FOR_EACH_RATE(GB_CASE)
 #undef GB_CASE
         default: return cudaErrorInvalidValue;
     }

@@ -1,7 +1,9 @@
-// Inline-PTX helpers shared by the kernels: mbarrier + 1-D TMA bulk copy (global -> shared), named barriers,
-// cp.async.
+// Device-only helpers shared by the kernels: mbarrier + 1-D TMA bulk copy (global -> shared), named barriers,
+// cp.async, warp reductions.
 #pragma once
 #include <stdint.h>
+
+#include "gb_common.cuh"
 
 namespace gb {
 
@@ -49,6 +51,27 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// Warp-level merge of per-thread peaks: REDUX for (max, first index, count), shuffles for the float64 sum.
+// Profile values are >= 0 (an excluded slot holds -1), so their IEEE bit patterns order like signed ints.
+__device__ __forceinline__ void warp_reduce_peak(Peak& p) {
+    const int bits = __float_as_int(p.mx);
+    const int mb = __reduce_max_sync(0xffffffffu, bits);
+    const bool is = bits == mb;
+    p.idx = __reduce_min_sync(0xffffffffu, is ? p.idx : 0x7fffffff);
+    p.cnt = __reduce_add_sync(0xffffffffu, is ? p.cnt : 0);
+    p.mx = __int_as_float(mb);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) p.sum += __shfl_xor_sync(0xffffffffu, p.sum, off);
+}
+// Warp sum of a coherent probe value: only the lane holding the probed lag contributes a non-zero value.
+__device__ __forceinline__ void warp_reduce_probe(float& re, float& im) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        re += __shfl_xor_sync(0xffffffffu, re, off);
+        im += __shfl_xor_sync(0xffffffffu, im, off);
+    }
 }
 
 }  // namespace gb

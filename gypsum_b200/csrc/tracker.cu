@@ -40,8 +40,9 @@ __device__ __noinline__ void track_update_device(TrackState* st, float2 E, float
     *out = rec;
 }
 
-// Loads the channel state into shared memory, keeping a copy for a later rollback when asked to.
-__device__ __forceinline__ void load_state(const TrackArgs& a, int ch, TrackState* st, int tid) {
+// Loads the channel state into shared memory (keeping a copy for a later rollback when asked to), the loop constants and
+// rtab[n] = 1 / n for the lock-window counts.  The caller's barrier publishes them.
+__device__ __forceinline__ void track_prologue(const TrackArgs& a, int ch, TrackState* st, TrackConsts* tc, double* rtab, int tid) {
     const int* src = reinterpret_cast<const int*>(a.states + ch);
     int* dst = reinterpret_cast<int*>(st);
     int* shd = a.shadow ? reinterpret_cast<int*>(a.shadow + ch) : nullptr;
@@ -50,11 +51,66 @@ __device__ __forceinline__ void load_state(const TrackArgs& a, int ch, TrackStat
         dst[i] = v;
         if (shd) shd[i] = v;
     }
+    if (tid == 0) *tc = track_consts(a.fs);
+    rtab[tid] = tid ? 1.0 / static_cast<double>(tid) : 0.0;  // kTrackThreads == 256 entries
 }
 __device__ __forceinline__ void store_state(const TrackState* st, TrackState* gst, int tid) {
     const int* src = reinterpret_cast<const int*>(st);
     int* dst = reinterpret_cast<int*>(gst);
     for (int i = tid; i < static_cast<int>(sizeof(TrackState) / 4); i += kTrackThreads) dst[i] = src[i];
+}
+
+// tracker.py:378: once the channel has stopped, later milliseconds are not processed; each gets this record.
+__device__ __forceinline__ void stopped_record(const TrackState* st, TrackMsRecord* out) {
+    TrackMsRecord rec = {};
+    rec.lost = 2;
+    rec.doppler = rec.doppler_hist = st->doppler;
+    rec.carrier_phase = rec.carrier_phase_hist = st->carrier_phase;
+    rec.code_phase = st->code_phase;
+    *out = rec;
+}
+
+// Millisecond k's loop parameters from the channel state.
+struct MsParams {
+    double t0;       // chunk start time
+    int pm, kE, kL;  // prompt code phase mod N; early and late lags
+    float2 fine;     // this thread's fine carrier factor
+};
+// Also writes the coarse carrier table: the wipe-off (tracker.py:278-281) exp(-j(2 pi f (n/fs + t0) + phi)) of sample n is
+// coarse[n / 256] * fine[n % 256], each factor from a float64-reduced phase.  The caller's barrier publishes the table.
+__device__ __forceinline__ MsParams ms_params(const TrackArgs& a, const TrackState* st, int k, int tid, float2* coarse) {
+    MsParams ms;
+    const double f = st->doppler, phi_cycles = st->carrier_phase * (1.0 / kTau);
+    ms.t0 = a.start_times ? a.start_times[k] : a.t0_single;
+    const int p = st->code_phase;
+    ms.pm = pymod_int(p, a.N);
+    ms.kE = pymod_int(p - 1, a.N);
+    ms.kL = pymod_int(p + 1, a.N);
+    if (tid < (a.N + kTrackThreads - 1) / kTrackThreads)
+        coarse[tid] = wipeoff(make_float2(1.f, 0.f), f * (static_cast<double>(tid * kTrackThreads) * a.inv_fs + ms.t0) + phi_cycles);
+    ms.fine = carrier_at(f, static_cast<double>(tid), a.inv_fs);
+    return ms;
+}
+
+// One (branch, parity h) warp's share of the circular correlation of its polyphase row x: forward transform, product with
+// the replica half-spectrum, inverse transform, exchange with the other warp of pair `pair` through the tiles, and
+// recombination into 16 lags per lane.  tw1, tw2 and crep may be in shared or global memory.
+__device__ __forceinline__ void track_correlate(float2 (&x)[32], int lane, int h, int pair, const float2* tw1, const float2* tw2,
+                                                const float2* crep, float2* tile, const float2* ptile, float2 (&out16)[16]) {
+    if (h) mul_tw2(x, lane, tw2);
+    wfft_phase1<false>(x, lane, tw1, tile);
+    __syncwarp();
+    wfft_phase2<false>(x, lane, tile);
+    __syncwarp();
+    mul_vec(x, lane, crep + h * kFft);
+    wfft_phase1<true>(x, lane, tw1, tile);
+    __syncwarp();
+    wfft_phase2<true>(x, lane, tile);
+    __syncwarp();
+    exchange_store(x, lane, h, tile);
+    pair_barrier(pair);
+    if (h == 0) combine_even(x, lane, tw2, ptile, out16);
+    else combine_odd(x, lane, tw2, ptile, out16);
 }
 
 // One (branch r, parity h) warp's 16 finished lags per lane: prompt profile statistics in rolled order
@@ -131,8 +187,7 @@ __device__ __forceinline__ void finish_ms(const TrackPartial* partial, int n_par
         }
         sum += static_cast<double>(pp.sum);
     }
-    const double m = static_cast<double>(mx);
-    const float strength = static_cast<float>(m / ((sum - cnt * m) / (N - cnt)));  // utils.py:111-116
+    const float strength = static_cast<float>(record_strength(mx, sum, cnt, N));
     track_update_device(st, el[0], el[1], make_float2(pre, pim), strength, key, t0, tc, rtab, out);
 }
 
@@ -159,14 +214,9 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_channels(const Track
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     TrackState* gst = a.states + ch;
 
-    // ---- load the channel state (keeping a copy for a later rollback when asked to), the twiddles and this PRN's
-    //      replica spectrum ----
-    load_state(a, ch, st, tid);
-    if (tid == 0) {
-        mbar_init(mbar, 1);
-        *tc = track_consts(a.fs);
-    }
-    rtab[tid] = tid ? 1.0 / static_cast<double>(tid) : 0.0;  // kTrackThreads == 256 entries
+    // ---- load the channel state, the twiddles and this PRN's replica spectrum ----
+    track_prologue(a, ch, st, tc, rtab, tid);
+    if (tid == 0) mbar_init(mbar, 1);
     __syncthreads();
     if (tid == 0) {
         mbar_expect_tx(mbar, 4 * kFft * sizeof(float2));
@@ -202,59 +252,28 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_channels(const Track
             cp_async_wait<0>();
         }
         __syncthreads();  // chunk k landed; the previous millisecond's loop-filter update is visible
-        if (st->lost) {   // tracker.py:378: the channel stopped; later milliseconds are not processed
-            if (tid == 0) {
-                TrackMsRecord rec = {};
-                rec.lost = 2;
-                rec.doppler = rec.doppler_hist = st->doppler;
-                rec.carrier_phase = rec.carrier_phase_hist = st->carrier_phase;
-                rec.code_phase = st->code_phase;
-                out[k] = rec;
-            }
+        if (st->lost) {
+            if (tid == 0) stopped_record(st, &out[k]);
             continue;
         }
-        const double f = st->doppler, phi_cycles = st->carrier_phase * (1.0 / kTau), t0 = a.start_times ? a.start_times[k] : a.t0_single;
-        const int p = st->code_phase;
-        const int pm = pymod_int(p, a.N);
-        const int kE = pymod_int(p - 1, a.N), kL = pymod_int(p + 1, a.N);
-
-        // ---- carrier wipe-off (tracker.py:278-281): exp(-j(2 pi f (n/fs + t0) + phi)) = coarse[n/256] * fine[n%256],
-        //      each factor from a float64-reduced phase; polyphase de-interleave ----
-        if (tid < (a.N + kTrackThreads - 1) / kTrackThreads)
-            coarse[tid] = wipeoff(make_float2(1.f, 0.f), f * (static_cast<double>(tid * kTrackThreads) * a.inv_fs + t0) + phi_cycles);
-        const float2 fine = carrier_at(f, static_cast<double>(tid), a.inv_fs);
+        const MsParams ms = ms_params(a, st, k, tid, coarse);
         __syncthreads();
+        // ---- carrier wipe-off, polyphase de-interleave ----
         const float2* buf = iqbuf + (k & 1) * a.N;
         for (int kk = 0, n = tid; n < a.N; ++kk, n += kTrackThreads)
-            ypoly[(n % S) * kFft + n / S] = cmul(buf[n], cmul(coarse[kk], fine));
+            ypoly[(n % S) * kFft + n / S] = cmul(buf[n], cmul(coarse[kk], ms.fine));
         __syncthreads();
         if (tid < S) ypoly[tid * kFft + (kFft - 1)] = ypoly[tid * kFft];
         __syncthreads();
 
         if (warp < n_fft_warps) {
-            float2 x[32];
-            // forward transform, spectrum product, inverse transform
+            float2 x[32], out16[16];
             build_z(x, lane, r, S, ypoly);
-            if (h) mul_tw2(x, lane, tw2_s);
-            wfft_phase1<false>(x, lane, tw1_s, tile);
-            __syncwarp();
-            wfft_phase2<false>(x, lane, tile);
-            __syncwarp();
-            mul_vec(x, lane, crep_s + h * kFft);
-            wfft_phase1<true>(x, lane, tw1_s, tile);
-            __syncwarp();
-            wfft_phase2<true>(x, lane, tile);
-            __syncwarp();
-            exchange_store(x, lane, h, tile);
-            pair_barrier(r);
-            float2 out16[16];
-            if (h == 0) combine_even(x, lane, tw2_s, ptile, out16);
-            else combine_odd(x, lane, tw2_s, ptile, out16);
-
-            prompt_stats<S>(out16, lane, h, r, pm, kE, kL, a, slot, k, el, partial + warp);
+            track_correlate(x, lane, h, r, tw1_s, tw2_s, crep_s, tile, ptile, out16);
+            prompt_stats<S>(out16, lane, h, r, ms.pm, ms.kE, ms.kL, a, slot, k, el, partial + warp);
         }
         __syncthreads();
-        if (tid == 0) finish_ms(partial, n_fft_warps, a.N, st, el, t0, tc, rtab, &out[k]);
+        if (tid == 0) finish_ms(partial, n_fft_warps, a.N, st, el, ms.t0, tc, rtab, &out[k]);
         // the __syncthreads at the top of the next millisecond publishes st / frees el, partial
     }
     __syncthreads();
@@ -296,9 +315,7 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_channels_wide(const 
     const int slot = blockIdx.x;
     const int ch = a.channel_idx ? a.channel_idx[slot] : slot;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    load_state(a, ch, st, tid);
-    if (tid == 0) *tc = track_consts(a.fs);
-    rtab[tid] = tid ? 1.0 / static_cast<double>(tid) : 0.0;
+    track_prologue(a, ch, st, tc, rtab, tid);
     __syncthreads();
     const float2* crep = a.crep + static_cast<size_t>(st->prn) * 2 * kFft;
     float2* tile = tiles + warp * kTileF2;
@@ -312,28 +329,14 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_channels_wide(const 
             prefetch_l2_bulk(reinterpret_cast<const void*>(b), static_cast<uint32_t>(e - b));
         }
         __syncthreads();  // the previous millisecond's loop-filter update is visible; rows, tiles, el, partial are free
-        if (st->lost) {   // tracker.py:378: the channel stopped; later milliseconds are not processed
-            if (tid == 0) {
-                TrackMsRecord rec = {};
-                rec.lost = 2;
-                rec.doppler = rec.doppler_hist = st->doppler;
-                rec.carrier_phase = rec.carrier_phase_hist = st->carrier_phase;
-                rec.code_phase = st->code_phase;
-                out[k] = rec;
-            }
+        if (st->lost) {
+            if (tid == 0) stopped_record(st, &out[k]);
             continue;
         }
-        const double f = st->doppler, phi_cycles = st->carrier_phase * (1.0 / kTau), t0 = a.start_times ? a.start_times[k] : a.t0_single;
-        const int p = st->code_phase;
-        const int pm = pymod_int(p, a.N);
-        const int kE = pymod_int(p - 1, a.N), kL = pymod_int(p + 1, a.N);
-
-        // ---- carrier wipe-off (tracker.py:278-281), as above; polyphase de-interleave into zpos() rows ----
-        const float2* src = a.iq + static_cast<size_t>(k) * a.N;
-        if (tid < (a.N + kTrackThreads - 1) / kTrackThreads)
-            coarse[tid] = wipeoff(make_float2(1.f, 0.f), f * (static_cast<double>(tid * kTrackThreads) * a.inv_fs + t0) + phi_cycles);
-        const float2 fine = carrier_at(f, static_cast<double>(tid), a.inv_fs);
+        const MsParams ms = ms_params(a, st, k, tid, coarse);
         __syncthreads();
+        // ---- carrier wipe-off, polyphase de-interleave into zpos() rows ----
+        const float2* src = a.iq + static_cast<size_t>(k) * a.N;
         for (int k0 = 0; k0 * kTrackThreads < a.N; k0 += kWideBatch) {
             float2 v[kWideBatch];
 #pragma unroll
@@ -344,7 +347,7 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_channels_wide(const 
 #pragma unroll
             for (int j = 0; j < kWideBatch; ++j) {
                 const int n = tid + (k0 + j) * kTrackThreads;
-                if (n < a.N) ypoly[(n % S) * kFft + zpos(n / S)] = cmul(v[j], cmul(coarse[k0 + j], fine));
+                if (n < a.N) ypoly[(n % S) * kFft + zpos(n / S)] = cmul(v[j], cmul(coarse[k0 + j], ms.fine));
             }
         }
         __syncthreads();
@@ -369,36 +372,27 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_channels_wide(const 
             const int task = round * kWideWarps + warp;
             if (task < n_tasks) {  // 2S and 8 are even: both warps of a pair are active or neither is
                 const int r = task >> 1, h = task & 1;
-                float2 x[32];
-                // forward transform, spectrum product, inverse transform
+                float2 x[32], out16[16];
                 load_vec(x, lane, ypoly + r * kFft);
-                if (h) mul_tw2(x, lane, a.tw2);
-                wfft_phase1<false>(x, lane, a.tw1, tile);
-                __syncwarp();
-                wfft_phase2<false>(x, lane, tile);
-                __syncwarp();
-                mul_vec(x, lane, crep + h * kFft);
-                wfft_phase1<true>(x, lane, a.tw1, tile);
-                __syncwarp();
-                wfft_phase2<true>(x, lane, tile);
-                __syncwarp();
-                exchange_store(x, lane, h, tile);
-                pair_barrier(warp >> 1);
-                float2 out16[16];
-                if (h == 0) combine_even(x, lane, a.tw2, ptile, out16);
-                else combine_odd(x, lane, a.tw2, ptile, out16);
-                prompt_stats<S>(out16, lane, h, r, pm, kE, kL, a, slot, k, el, partial + task);
+                track_correlate(x, lane, h, warp >> 1, a.tw1, a.tw2, crep, tile, ptile, out16);
+                prompt_stats<S>(out16, lane, h, r, ms.pm, ms.kE, ms.kL, a, slot, k, el, partial + task);
             }
             if (round + 1 < n_rounds) __syncthreads();  // the partner's tile was read: the next round may overwrite it
         }
         __syncthreads();
-        if (tid == 0) finish_ms(partial, n_tasks, a.N, st, el, t0, tc, rtab, &out[k]);
+        if (tid == 0) finish_ms(partial, n_tasks, a.N, st, el, ms.t0, tc, rtab, &out[k]);
     }
     __syncthreads();
     store_state(st, a.states + ch, tid);
 }
 
-static bool track_wide(int s) { return s >= 5; }
+// The kernel follows from S alone: k_track_channels while its whole-chunk layout fits (S <= 4), the wide kernel above.
+constexpr bool track_wide(int s) { return s >= 5; }
+template <int S>
+static auto track_kernel() {
+    if constexpr (track_wide(S)) return k_track_channels_wide<S>;
+    else return k_track_channels<S>;
+}
 
 size_t track_smem_bytes(int N, int s) {
     if (track_wide(s))
@@ -409,31 +403,20 @@ size_t track_smem_bytes(int N, int s) {
            sizeof(TrackState) + 8 * sizeof(TrackPartial) + (2 + 16) * sizeof(float2) + 16 + 256 * sizeof(double) + sizeof(TrackConsts);
 }
 
-template <int S>
-static cudaError_t track_attr() {
-    if constexpr (S >= 5)
-        return cudaFuncSetAttribute(k_track_channels_wide<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    else
-        return cudaFuncSetAttribute(k_track_channels<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-}
-
 cudaError_t configure_track_kernel() {
     cudaError_t e;
-#define GB_ATTR(S) if ((e = track_attr<S>()) != cudaSuccess) return e;
-    GB_ATTR(1) GB_ATTR(2) GB_ATTR(3) GB_ATTR(4) GB_ATTR(5) GB_ATTR(6) GB_ATTR(8) GB_ATTR(10) GB_ATTR(12) GB_ATTR(16)
+#define GB_ATTR(S) \
+    if ((e = cudaFuncSetAttribute(track_kernel<S>(), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    GB_FOR_EACH_RATE(GB_ATTR)
 #undef GB_ATTR
     return cudaSuccess;
 }
 
-// The kernel follows from S alone: k_track_channels while its whole-chunk layout fits (S <= 4), the wide kernel above.
 cudaError_t launch_track_channels(const TrackArgs& a, cudaStream_t st) {
     const size_t sm = track_smem_bytes(a.N, a.s);
     switch (a.s) {
-#define GB_CASE(S) case S: k_track_channels<S><<<a.n_channels, kTrackThreads, sm, st>>>(a); break;
-        GB_CASE(1) GB_CASE(2) GB_CASE(3) GB_CASE(4)
-#undef GB_CASE
-#define GB_CASE(S) case S: k_track_channels_wide<S><<<a.n_channels, kTrackThreads, sm, st>>>(a); break;
-        GB_CASE(5) GB_CASE(6) GB_CASE(8) GB_CASE(10) GB_CASE(12) GB_CASE(16)
+#define GB_CASE(S) case S: track_kernel<S>()<<<a.n_channels, kTrackThreads, sm, st>>>(a); break;
+        GB_FOR_EACH_RATE(GB_CASE)
 #undef GB_CASE
         default: return cudaErrorInvalidValue;
     }

@@ -97,7 +97,7 @@ void emu_cell_profile(const float2* iq, int N, int n_ms, double fs, double doppl
             for (int m = 0; m < kChips; ++m) {
                 switch (s) {
 #define EMU_CASE(S) case S: { float2 z[S]; boxcar_column<S>(ypoly.data(), m, z); for (int r = 0; r < S; ++r) znew[(size_t)r * kFft + zpos(m)] = z[r]; } break;
-                    EMU_CASE(2) EMU_CASE(3) EMU_CASE(4) EMU_CASE(5) EMU_CASE(6) EMU_CASE(8) EMU_CASE(10) EMU_CASE(12) EMU_CASE(16)
+                    GB_FOR_EACH_RATE(EMU_CASE)
 #undef EMU_CASE
                 }
             }
@@ -181,14 +181,7 @@ void emu_cell_profile(const float2* iq, int N, int n_ms, double fs, double doppl
                 peak_merge(cell, t);
             }
     }
-    if (rec_out) {
-        rec_out->peak = cell.mx;
-        rec_out->argmax = cell.idx;
-        rec_out->sum = cell.sum;
-        rec_out->count = cell.cnt;
-        rec_out->probe_re = rec_out->probe_im = 0.f;
-        rec_out->pad_ = 0;
-    }
+    if (rec_out) write_record(rec_out, cell, 0.f, 0.f);
     delete w;
     delete wo;
 }
