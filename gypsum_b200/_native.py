@@ -77,6 +77,11 @@ SYMBOLS = {
     "gb200_tracker_bit_state": (C.c_int, [_P, C.c_int, _P]),
     "gb200_tracker_decode_subframes": (C.c_int, [_P, _P, _P, C.c_int32, _P, C.c_int32, _P]),
     "gb200_tracker_subframe_state": (C.c_int, [_P, C.c_int, _P]),
+    "gb200_tracker_parse_subframes": (C.c_int, [_P, _P, _P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int32, _P]),
+    "gb200_tracker_orbit_state": (C.c_int, [_P, C.c_int, _P, C.POINTER(C.c_uint32), C.POINTER(C.c_int64),
+                                            C.POINTER(C.c_int32)]),
+    "gb200_tracker_observations": (C.c_int, [_P, _P]),
+    "gb200_tracker_observations_device": (C.c_int, [_P, _P]),
     "gb200_set_fused": (C.c_int, [_P, C.c_int]),
     "gb200_launch_count": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "gb200_enable_kernel_timing": (C.c_int, [_P, C.c_int]),
@@ -534,6 +539,7 @@ class Tracker:
         if (cnt > cap).any():
             raise RuntimeError("bit event buffer too small")  # cannot happen: see `cap`
         self._last_bit_stride = cap
+        self._chain_bits_n_ms = n_ms if records_device_ptr is None else 0
         return [ev[c, : cnt[c]].copy() for c in range(self.n_channels)]
 
     def bit_state(self, channel: int) -> dict:
@@ -570,7 +576,64 @@ class Tracker:
                                                      cap, _ptr(cnt)), "gb200_tracker_decode_subframes")
         if (cnt > cap).any():
             raise RuntimeError("subframe event buffer too small")  # cannot happen: see subframe_event_capacity
+        self._chain_sub = (self._chain_bits_n_ms if bits_device_ptr is None else 0, cap)
         return [ev[c, : cnt[c]].copy() for c in range(self.n_channels)]
+
+    _chain_bits_n_ms = 0  # n_ms of the last integrate_bits call over the tracker's own records
+    _chain_sub = (0, 0)  # (n_ms, events per channel) of the last decode_subframes call on that chain
+    _orbit_n_ms = 0  # milliseconds the last parse_subframes call covered
+
+    def parse_subframes(self, events_device_ptr: int | None = None, counts=None, stride: int | None = None,
+                        event_ms=None, drop_ms=None, n_ms: int | None = None) -> list:
+        """Subframe fields and the world model's per-satellite state (gb200_tracker_parse_subframes).  By default over
+        the events the last `decode_subframes` call left on the device (the process -> integrate_bits ->
+        decode_subframes chain); else over a device array [n_channels][stride] of SUBFRAME_DTYPE with counts[c] events
+        in row c, their milliseconds event_ms [n_channels, stride], drop_ms [n_channels] (-1 = none) and n_ms.
+        Returns one FIELDS_DTYPE array per channel."""
+        if events_device_ptr is None:
+            if any(v is not None for v in (counts, stride, event_ms, drop_ms, n_ms)):
+                raise ValueError("counts / stride / event_ms / drop_ms / n_ms describe a caller's device array only")
+            n_ms, cap = self._chain_sub
+            args = (None, None, 0, None, None, 0)
+        else:
+            cnt_in = np.ascontiguousarray(counts, dtype=np.int32)
+            ems = np.ascontiguousarray(event_ms, dtype=np.int32)
+            drop = np.ascontiguousarray(drop_ms, dtype=np.int32)
+            if cnt_in.shape != (self.n_channels,) or drop.shape != (self.n_channels,) or stride is None or n_ms is None:
+                raise ValueError("a device event array needs one count and one drop per channel, its stride and n_ms")
+            if ems.shape != (self.n_channels, int(stride)):
+                raise ValueError("event_ms must be [n_channels, stride]")
+            cap = max(1, int(cnt_in.max(initial=0)))
+            args = (_P(events_device_ptr), _ptr(cnt_in), int(stride), _ptr(ems), _ptr(drop), int(n_ms))
+        cap = max(1, int(cap))
+        out = np.empty((self.n_channels, cap), dtype=FIELDS_DTYPE)
+        cnt = np.empty(self.n_channels, dtype=np.int32)
+        self._engine._check(self._lib.gb200_tracker_parse_subframes(self._h, *args, _ptr(out), cap, _ptr(cnt)),
+                            "gb200_tracker_parse_subframes")
+        self._orbit_n_ms = int(n_ms)
+        if events_device_ptr is None:
+            self._chain_sub = (0, 0)
+        return [out[c, : cnt[c]].copy() for c in range(self.n_channels)]
+
+    def orbit_state(self, channel: int) -> dict:
+        """One channel's world-model entry: params (float64[26], OrbitalParameterType order), set_mask, prn_count,
+        counting."""
+        p = np.zeros(ORBIT_PARAMS, dtype=np.float64)
+        mask, count, counting = C.c_uint32(), C.c_int64(), C.c_int32()
+        self._engine._check(self._lib.gb200_tracker_orbit_state(self._h, channel, _ptr(p), C.byref(mask), C.byref(count),
+                                                                C.byref(counting)), "gb200_tracker_orbit_state")
+        return {"params": p, "set_mask": mask.value, "prn_count": count.value, "counting": bool(counting.value)}
+
+    def observations(self) -> np.ndarray:
+        """OBSERVATION_DTYPE [n_channels, n_ms] over the milliseconds of the last parse_subframes call."""
+        out = np.empty((self.n_channels, self._orbit_n_ms), dtype=OBSERVATION_DTYPE)
+        self._engine._check(self._lib.gb200_tracker_observations(self._h, _ptr(out)), "gb200_tracker_observations")
+        return out
+
+    def observations_device(self, out_device_ptr: int) -> None:
+        """Enqueue only: n_channels * n_ms OBSERVATION_DTYPE records to device memory."""
+        self._engine._check(self._lib.gb200_tracker_observations_device(self._h, _P(out_device_ptr)),
+                            "gb200_tracker_observations_device")
 
     def subframe_state(self, channel: int) -> dict:
         out = np.zeros(6, dtype=np.int64)
@@ -606,6 +669,17 @@ SUBFRAME_DTYPE = np.dtype([  # gb200_subframe_event
 assert SUBFRAME_DTYPE.itemsize == 96
 SUBFRAME, DETERMINED_PHASE, CANNOT_DETERMINE_PHASE, RAISED = 0, 1, 2, 3  # SUBFRAME_DTYPE["kind"]
 STOP_RAISED, STOP_OVERFLOW, STOP_LOST_LOCK = 1, 2, 3  # Tracker.subframe_state()["stopped"]
+
+FIELDS_DTYPE = np.dtype([  # gb200_subframe_fields
+    ("event_index", "<i4"), ("ms", "<i4"), ("subframe_id", "<i4"), ("reserved", "<i4"), ("tow_seconds", "<f8"),
+    ("ints", "<i4", (2,)), ("bits", "<u4", (4,)), ("bit_widths", "<i4", (4,)), ("values", "<f8", (10,))])
+assert FIELDS_DTYPE.itemsize == 144
+OBSERVATION_DTYPE = np.dtype([  # gb200_sv_observation
+    ("tow", "<f8"), ("dsv", "<f8"), ("x", "<f8"), ("y", "<f8"), ("z", "<f8"), ("prn_count", "<i8"), ("flags", "<i4"),
+    ("reserved", "<i4")])
+assert OBSERVATION_DTYPE.itemsize == 56
+ORBIT_PARAMS = 26
+OBS_TIMING, OBS_COMPLETE, OBS_FIX_GATE, OBS_COUNTING, OBS_FROZEN = 1, 2, 4, 8, 16  # OBSERVATION_DTYPE["flags"]
 
 
 def subframe_event_capacity(n_bits: int) -> int:

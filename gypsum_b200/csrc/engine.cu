@@ -17,6 +17,7 @@
 #include "bits_core.cuh"
 #include "kernels.cuh"
 #include "nav_core.cuh"
+#include "orbit_core.cuh"
 
 using namespace gb;
 
@@ -184,6 +185,21 @@ struct gb200_tracker {
     DevBuf<int> d_sub_counts, d_bit_counts;
     PinnedBuf<SubframeEvent> h_sub;
     PinnedBuf<int> h_sub_counts, h_bit_counts;
+    std::vector<int> prn;  // replica row per channel, -1 for a pool slot never seeded
+    // The call chain parse_subframes(NULL) reads: n_ms of the integrate call whose bit events still sit in d_events and
+    // came from the records in d_out (0 = none), and of the decode call whose events in d_sub came from those bits.
+    int chain_bits_n_ms = 0, chain_sub_n_ms = 0;
+    std::vector<int> sub_counts;  // events per channel of the last decode call, `sub_stride` apart in d_sub
+    int sub_stride = 0;
+    DevBuf<OrbitSnap> orbit_states, d_changes;
+    DevBuf<SubframeFields> d_fields;
+    DevBuf<int> d_field_counts, d_change_counts, d_event_ms, d_drop_ms, d_orbit_counts;
+    PinnedBuf<SubframeFields> h_fields;
+    PinnedBuf<int> h_field_counts, h_event_ms, h_drop_ms, h_orbit_counts;
+    int orbit_n_ms = 0;  // milliseconds the change table of the last parse call covers (0 = no call yet)
+    int change_stride = 0;
+    DevBuf<SvObservation> d_obs;
+    PinnedBuf<SvObservation> h_obs;
 };
 // A pipelined stream of grid batches: slot k's host->device copy, compute and device->host copy run on three streams.
 struct gb200_grid_stream {
@@ -220,6 +236,15 @@ static_assert(sizeof(gb200_best_record) == sizeof(BestRecord), "ABI best record 
 static_assert(sizeof(gb200_bit_event) == sizeof(BitEvent), "ABI bit event and device event must match");
 static_assert(sizeof(gb200_subframe_event) == sizeof(SubframeEvent) && sizeof(SubframeEvent) == 96,
               "ABI subframe event and device event must match");
+static_assert(sizeof(gb200_subframe_fields) == sizeof(SubframeFields) &&
+                  offsetof(gb200_subframe_fields, tow_seconds) == offsetof(SubframeFields, tow_seconds) &&
+                  offsetof(gb200_subframe_fields, bit_widths) == offsetof(SubframeFields, widths) &&
+                  offsetof(gb200_subframe_fields, values) == offsetof(SubframeFields, values),
+              "ABI subframe fields and device fields must match");
+static_assert(sizeof(gb200_sv_observation) == sizeof(SvObservation) &&
+                  offsetof(gb200_sv_observation, prn_count) == offsetof(SvObservation, prn_count) &&
+                  offsetof(gb200_sv_observation, flags) == offsetof(SvObservation, flags),
+              "ABI observation and device observation must match");
 static_assert(offsetof(gb200_subframe_event, words) == offsetof(SubframeEvent, words) &&
                   offsetof(gb200_subframe_event, kind) == offsetof(SubframeEvent, kind) &&
                   offsetof(gb200_subframe_event, parity_ok) == offsetof(SubframeEvent, parity_ok),
@@ -1201,6 +1226,7 @@ int gb200_tracker_create(gb200_engine* e, int n_channels, const int32_t* prn_idx
     t->n_channels = n_channels;
     t->seeded.assign(n_channels, 1);
     t->undo_ok.assign(n_channels, 0);
+    t->prn.assign(prn_idx, prn_idx + n_channels);
     std::vector<TrackState> init(n_channels);
     for (int c = 0; c < n_channels; ++c) {
         memset(&init[c], 0, sizeof(TrackState));
@@ -1310,6 +1336,7 @@ static int tracker_process_host(gb200_tracker* t, int n_sel, const int32_t* sel,
         GB_CUDA(e, t->h_prof.ensure(np));
     }
     t->last_n_ms = 0;
+    t->chain_bits_n_ms = t->chain_sub_n_ms = 0;  // d_out is about to be rewritten
     GB_TRY(tracker_launch(t, n_sel, sel, n_ms, start_times, t->d_out.p, np ? t->d_prof.p : nullptr, keep_undo));
     if (!sel) t->last_n_ms = n_ms;  // gb200_tracker_integrate_bits reads [channel][n_ms] of the whole bank
     // the profiles' copy is enqueued first, so the records' download waits for both
@@ -1355,6 +1382,7 @@ int gb200_tracker_create_pool(gb200_engine* e, int capacity, gb200_tracker** out
     t->n_channels = capacity;
     t->seeded.assign(capacity, 0);
     t->undo_ok.assign(capacity, 0);
+    t->prn.assign(capacity, -1);
     cudaError_t ce = t->states.ensure(capacity);
     if (ce == cudaSuccess) ce = cudaMemset(t->states.p, 0, sizeof(TrackState) * capacity);
     if (ce != cudaSuccess) {
@@ -1380,6 +1408,7 @@ int gb200_tracker_reset_channel(gb200_tracker* t, int channel, int32_t prn_idx, 
     GB_CUDA(e, cudaMemcpy(t->states.p + channel, init.data(), sizeof(TrackState), cudaMemcpyHostToDevice));
     t->seeded[channel] = 1;
     t->undo_ok[channel] = 0;
+    t->prn[channel] = prn_idx;
     return GB200_OK;
 }
 
@@ -1468,6 +1497,8 @@ int gb200_tracker_integrate_bits(gb200_tracker* t, int n_ms, const double* start
     t->bit_counts.assign(t->h_counts.p, t->h_counts.p + nc);
     t->bit_stride = max_events;
     t->bits_pending = true;
+    t->chain_bits_n_ms = records_device ? 0 : n_ms;
+    t->chain_sub_n_ms = 0;
     return GB200_OK;
 }
 
@@ -1548,11 +1579,14 @@ int gb200_tracker_decode_subframes(gb200_tracker* t, const void* bits_device, co
     a.n_channels = nc;
     a.max_events = max_events;
     GB_LAUNCH(e, -1, launch_decode_subframes(a, e->stream));
+    t->chain_sub_n_ms = bits_device ? 0 : t->chain_bits_n_ms;
     if (!bits_device) t->bits_pending = false;
     // the counts' copy is enqueued first, so the events' download waits for both
     GB_CUDA(e, cudaMemcpyAsync(t->h_sub_counts.p, t->d_sub_counts.p, nc * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
     GB_TRY(download(e, reinterpret_cast<SubframeEvent*>(events_host), t->d_sub.p, ne, t->h_sub));
     memcpy(counts_host, t->h_sub_counts.p, nc * sizeof(int));
+    t->sub_counts.assign(t->h_sub_counts.p, t->h_sub_counts.p + nc);
+    t->sub_stride = max_events;
     return GB200_OK;
 }
 
@@ -1575,6 +1609,147 @@ int gb200_tracker_subframe_state(gb200_tracker* t, int channel, int64_t out[6]) 
     out[4] = h.stopped;
     out[5] = h.bits;
     return GB200_OK;
+}
+
+int gb200_tracker_parse_subframes(gb200_tracker* t, const void* events_device, const int32_t* counts_host, int32_t stride,
+                                  const int32_t* event_ms_host, const int32_t* drop_ms_host, int32_t n_ms,
+                                  gb200_subframe_fields* fields_host, int32_t max_fields, int32_t* field_counts_host) {
+    if (!t) return GB200_EINVAL;
+    gb200_engine* e = t->e;
+    const int nc = t->n_channels;
+    if (!fields_host || !field_counts_host || max_fields < 1) GB_FAIL(e, GB200_EINVAL, "null / empty field buffer");
+    for (int c = 0; c < nc; ++c)
+        for (int d = 0; d < c; ++d)
+            if (t->prn[c] >= 0 && t->prn[c] == t->prn[d])
+                GB_FAIL(e, GB200_EINVAL, "channels %d and %d track the same replica row %d (the world model is keyed by satellite)",
+                        d, c, t->prn[c]);
+    const int* counts = nullptr;
+    if (events_device) {
+        if (!counts_host || !event_ms_host || !drop_ms_host || stride < 1 || n_ms < 1)
+            GB_FAIL(e, GB200_EINVAL, "subframe events need their counts, milliseconds, drops, a stride >= 1 and n_ms >= 1");
+        for (int c = 0; c < nc; ++c) {
+            if (counts_host[c] < 0 || counts_host[c] > stride)
+                GB_FAIL(e, GB200_EINVAL, "channel %d: %d events do not fit a stride of %d", c, counts_host[c], stride);
+            if (drop_ms_host[c] < -1 || drop_ms_host[c] >= n_ms)
+                GB_FAIL(e, GB200_EINVAL, "channel %d: drop millisecond %d outside [-1, %d)", c, drop_ms_host[c], n_ms);
+            for (int j = 0; j < counts_host[c]; ++j) {
+                const int m = event_ms_host[static_cast<size_t>(c) * stride + j];
+                const int prev = j ? event_ms_host[static_cast<size_t>(c) * stride + j - 1] : 0;
+                if (m < prev || m >= n_ms)
+                    GB_FAIL(e, GB200_EINVAL, "channel %d: event %d's millisecond %d is out of order or outside [0, %d)", c, j, m, n_ms);
+            }
+        }
+        counts = counts_host;
+    } else {
+        if (!t->chain_sub_n_ms)
+            GB_FAIL(e, GB200_ESTATE, "no unparsed subframe events of a process -> integrate_bits -> decode_subframes chain on the device");
+        for (int c = 0; c < nc; ++c)
+            if (t->sub_counts[c] > t->sub_stride)
+                GB_FAIL(e, GB200_EINVAL, "channel %d: the last decode call produced %d events but kept %d", c, t->sub_counts[c],
+                        t->sub_stride);
+        counts = t->sub_counts.data();
+        stride = t->sub_stride;
+        n_ms = t->chain_sub_n_ms;
+    }
+    GB_CUDA(e, cudaSetDevice(e->device));
+    GB_CUDA(e, cudaStreamSynchronize(e->stream));  // pinned staging may still be in flight
+    if (!t->orbit_states.p) {
+        std::vector<OrbitSnap> init(nc);
+        for (int c = 0; c < nc; ++c) orbit_state_init(init[c]);
+        GB_CUDA(e, t->orbit_states.ensure(nc));
+        GB_CUDA(e, cudaMemcpy(t->orbit_states.p, init.data(), sizeof(OrbitSnap) * nc, cudaMemcpyHostToDevice));
+    }
+    const size_t nf = static_cast<size_t>(nc) * stride;
+    GB_CUDA(e, t->d_fields.ensure(nf));
+    GB_CUDA(e, t->d_changes.ensure(static_cast<size_t>(nc) * (stride + 2)));
+    GB_CUDA(e, t->d_field_counts.ensure(nc));
+    GB_CUDA(e, t->d_change_counts.ensure(nc));
+    GB_CUDA(e, t->h_field_counts.ensure(nc));
+    GB_CUDA(e, t->d_orbit_counts.ensure(nc));
+    GB_TRY(upload(e, t->d_orbit_counts.p, counts, nc, t->h_orbit_counts));
+    OrbitArgs a{};
+    if (events_device) {
+        GB_CUDA(e, t->d_event_ms.ensure(nf));
+        GB_CUDA(e, t->d_drop_ms.ensure(nc));
+        GB_TRY(upload(e, t->d_event_ms.p, event_ms_host, nf, t->h_event_ms));
+        GB_TRY(upload(e, t->d_drop_ms.p, drop_ms_host, nc, t->h_drop_ms));
+        a.events = static_cast<const SubframeEvent*>(events_device);
+        a.event_ms = t->d_event_ms.p;
+        a.drop_ms = t->d_drop_ms.p;
+    } else {
+        a.events = t->d_sub.p;
+        a.bits = t->d_events.p;
+        a.bit_stride = t->bit_stride;
+        a.records = t->d_out.p;
+    }
+    a.counts = t->d_orbit_counts.p;
+    a.states = t->orbit_states.p;
+    a.fields = t->d_fields.p;
+    a.field_counts = t->d_field_counts.p;
+    a.changes = t->d_changes.p;
+    a.change_counts = t->d_change_counts.p;
+    a.stride = stride;
+    a.n_ms = n_ms;
+    a.n_channels = nc;
+    GB_LAUNCH(e, -1, launch_parse_subframes(a, e->stream));
+    if (!events_device) t->chain_sub_n_ms = 0;
+    t->orbit_n_ms = n_ms;
+    t->change_stride = stride + 2;
+    // the counts' copy is enqueued first, so the fields' download waits for both
+    GB_CUDA(e, cudaMemcpyAsync(t->h_field_counts.p, t->d_field_counts.p, nc * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+    GB_CUDA(e, cudaStreamSynchronize(e->stream));
+    // the fields are [channel][stride] on the device and [channel][max_fields] for the caller
+    const int keep = std::min<int>(stride, max_fields);
+    GB_CUDA(e, cudaMemcpy2DAsync(fields_host, sizeof(SubframeFields) * max_fields, t->d_fields.p, sizeof(SubframeFields) * stride,
+                                 sizeof(SubframeFields) * keep, nc, cudaMemcpyDeviceToHost, e->stream));
+    GB_CUDA(e, cudaStreamSynchronize(e->stream));
+    memcpy(field_counts_host, t->h_field_counts.p, nc * sizeof(int));
+    return GB200_OK;
+}
+
+int gb200_tracker_orbit_state(gb200_tracker* t, int channel, double params[26], uint32_t* set_mask, int64_t* prn_count,
+                              int32_t* counting) {
+    if (!t) return GB200_EINVAL;
+    gb200_engine* e = t->e;
+    GB_TRY(check_channel(t, channel));
+    OrbitSnap s;
+    orbit_state_init(s);
+    if (t->orbit_states.p) {
+        GB_CUDA(e, cudaSetDevice(e->device));
+        GB_CUDA(e, cudaStreamSynchronize(e->stream));
+        GB_CUDA(e, cudaMemcpy(&s, t->orbit_states.p + channel, sizeof(OrbitSnap), cudaMemcpyDeviceToHost));
+    }
+    if (params) memcpy(params, s.p, sizeof(s.p));
+    if (set_mask) *set_mask = s.set;
+    if (prn_count) *prn_count = s.count;
+    if (counting) *counting = s.counting;
+    return GB200_OK;
+}
+
+static int observations_launch(gb200_tracker* t, SvObservation* out_dev) {
+    gb200_engine* e = t->e;
+    if (!t->orbit_n_ms) GB_FAIL(e, GB200_ESTATE, "no gb200_tracker_parse_subframes call yet");
+    GB_LAUNCH(e, -1, launch_sv_observations(t->d_changes.p, t->d_change_counts.p, t->change_stride, t->n_channels, t->orbit_n_ms,
+                                            out_dev, e->stream));
+    return GB200_OK;
+}
+
+int gb200_tracker_observations_device(gb200_tracker* t, void* out_device) {
+    if (!t) return GB200_EINVAL;
+    if (!out_device) GB_FAIL(t->e, GB200_EINVAL, "null output");
+    GB_CUDA(t->e, cudaSetDevice(t->e->device));
+    return observations_launch(t, static_cast<SvObservation*>(out_device));
+}
+
+int gb200_tracker_observations(gb200_tracker* t, gb200_sv_observation* out_host) {
+    if (!t) return GB200_EINVAL;
+    gb200_engine* e = t->e;
+    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
+    GB_CUDA(e, cudaSetDevice(e->device));
+    const size_t n = static_cast<size_t>(t->n_channels) * t->orbit_n_ms;
+    if (n) GB_CUDA(e, t->d_obs.ensure(n));
+    GB_TRY(observations_launch(t, t->d_obs.p));
+    return download(e, reinterpret_cast<SvObservation*>(out_host), t->d_obs.p, n, t->h_obs);
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -122,6 +122,29 @@ struct NavArgs {
     int stride, n_channels, max_events;
 };
 
+// parse_subframes / sv_observations: subframe fields, the world model's per-satellite state and its per-millisecond
+// satellite time and position (orbit.cu, orbit_core.cuh).
+struct OrbitSnap;
+struct SubframeFields;
+struct SvObservation;
+struct OrbitArgs {
+    const SubframeEvent* events;   // [n_channels][stride]
+    const int* counts;             // [n_channels] events per channel
+    const int* event_ms;           // explicit: [n_channels][stride] millisecond of each event; null = from `bits`
+    const BitEvent* bits;          // chain: the bit events the events' bit_index refers to, [n_channels][bit_stride]
+    const TrackMsRecord* records;  // chain: the tracking records, [n_channels][n_ms]; a `lost` one drops the channel
+    const int* drop_ms;            // explicit: [n_channels] millisecond the channel is dropped at, -1 = none
+    OrbitSnap* states;             // [n_channels] carried from call to call
+    SubframeFields* fields;        // [n_channels][stride] parsed kind-0 events
+    int* field_counts;             // [n_channels]
+    OrbitSnap* changes;            // [n_channels][stride + 2] the state after each change, by millisecond
+    int* change_counts;            // [n_channels]
+    int stride, bit_stride, n_ms, n_channels;
+};
+cudaError_t launch_parse_subframes(const OrbitArgs& a, cudaStream_t st);
+cudaError_t launch_sv_observations(const OrbitSnap* changes, const int* change_counts, int change_stride, int n_channels,
+                                   int n_ms, SvObservation* out, cudaStream_t st);
+
 // acquire_fused: one CTA per (PRN, Doppler) cell, the whole pipeline in one kernel (fused.cu).
 struct FusedArgs {
     const float2* iq;       // [M*N] one block

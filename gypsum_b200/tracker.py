@@ -355,4 +355,43 @@ class TrackerBank:
         """Navigation-message subframes of every channel from the bit events the last `integrate_bits` call left on the
         device (navigation_message_decoder.py:173-196; one decoder per channel, persistent across calls).  Returns one
         _native.SUBFRAME_DTYPE array per channel; _native.subframe_bits gives an event's 300 upright bits."""
-        return self.native.decode_subframes()
+        self._last_subframes = self.native.decode_subframes()
+        return self._last_subframes
+
+    def parse_subframes(self) -> list:
+        """The subframes the last `decode_subframes` call produced, parsed on the device (navigation_message_parser.py),
+        and the world model's per-satellite state advanced over the same milliseconds (world_model.py:707-861, one
+        satellite per channel).  Returns per channel a list of (subframe, receiver_timestamp,
+        trailing_edge_receiver_timestamp, ms) with `subframe` a NavigationMessageSubframe1..5."""
+        from gypsum_b200.navigation_message_parser import subframe_from_fields
+
+        fields = self.native.parse_subframes()
+        out = []
+        for c, rows in enumerate(fields):
+            evs = [self._last_subframes[c][int(r["event_index"])] for r in rows]
+            out.append([(subframe_from_fields(r), float(e["receiver_timestamp"]), float(e["trailing_edge_receiver_timestamp"]),
+                         int(r["ms"])) for r, e in zip(rows, evs)])
+        return out
+
+    def orbital_parameters(self, channel: int) -> dict:
+        """One channel's OrbitalParameters (world_model.py:151-199) as {OrbitalParameterType name: value or None}."""
+        st = self.native.orbit_state(channel)
+        return {name: (float(st["params"][k]) if st["set_mask"] >> k & 1 else None)
+                for k, name in enumerate(ORBITAL_PARAMETER_NAMES)}
+
+    def observations(self) -> np.ndarray:
+        """_native.OBSERVATION_DTYPE [channel][ms] over the milliseconds of the last parse_subframes call: satellite
+        time of week, clock correction and ECEF position as the world model computes them (world_model.py:379-487,
+        :635-705), the PRN count and flags."""
+        return self.native.observations()
+
+
+# OrbitalParameterType (world_model.py:151-199), in order
+ORBITAL_PARAMETER_NAMES = (
+    "SQRT_SEMI_MAJOR_AXIS", "SEMI_MAJOR_AXIS", "ECCENTRICITY", "INCLINATION", "LONGITUDE_OF_ASCENDING_NODE",
+    "ARGUMENT_OF_PERIGEE", "MEAN_ANOMALY_AT_REFERENCE_TIME", "MEAN_MOTION_DIFFERENCE",
+    "CORRECTION_TO_ARGUMENT_OF_LATITUDE_COS", "CORRECTION_TO_ARGUMENT_OF_LATITUDE_SIN", "CORRECTION_TO_ORBITAL_RADIUS_COS",
+    "CORRECTION_TO_ORBITAL_RADIUS_SIN", "CORRECTION_TO_INCLINATION_ANGLE_COS", "CORRECTION_TO_INCLINATION_ANGLE_SIN",
+    "RATE_OF_RIGHT_ASCENSION", "RATE_OF_INCLINATION_ANGLE", "WEEK_NUMBER", "EPHEMERIS_REFERENCE_TIME",
+    "GPS_TIME_OF_WEEK_AT_LAST_TIMESTAMP", "RECEIVER_TIMESTAMP_AT_LAST_HOW_TIMESTAMP", "PRN_TIMESTAMP_OF_LEADING_EDGE_OF_TOW",
+    "A_F0", "A_F1", "A_F2", "T_OC", "ESTIMATED_GROUP_DELAY_DIFFERENTIAL")

@@ -259,8 +259,9 @@ int gb200_tracker_bit_state(gb200_tracker* t, int channel, int64_t out[8]);
  *   2  CannotDetermineSubframePhaseEvent (:170): no preamble pair among >= 3600 queued bits, on every such bit;
  *   3  the reference raises ValueError here (subframe 5 whose data id is not 01, navigation_message_parser.py:626):
  *      the channel's decoder stops, and events the same bit produced before are dropped, as the exception drops them.
- * Field parsing (NavigationMessageSubframe1..5) stays with the caller: `words` holds the 300 bits the reference's
- * NavigationMessageSubframeParser is given.                                                                     */
+ * `words` holds the 300 bits the reference's NavigationMessageSubframeParser is given;
+ * gb200_tracker_parse_subframes below parses them into NavigationMessageSubframe1..5 fields.  A channel whose decoder
+ * raised (kind 3) freezes its orbit state there, as the reference receiver's step never returns from the exception. */
 typedef struct gb200_subframe_event {
     double receiver_timestamp;               /* receiver_timestamp of the subframe's first bit             (:203) */
     double trailing_edge_receiver_timestamp; /* trailing edge of its last bit                              (:204) */
@@ -291,6 +292,80 @@ int gb200_tracker_decode_subframes(gb200_tracker* t, const void* bits_device, co
  * (+1 / -1 / 0 = None), queued bits, stopped (0 running, 1 raised, 2 queue overflow, 3 the integrator stopped),
  * bit events processed. */
 int gb200_tracker_subframe_state(gb200_tracker* t, int channel, int64_t out[6]);
+
+/* Subframe fields (gypsum/navigation_message_parser.py:426-673), one per kind-0 subframe event, 144 bytes.  Bit-list
+ * fields are packed with their first bit most significant.  By subframe id (dataclass order):
+ *   1  ints: week_num_mod_1024_bits, l2_p_data_flag; bits: ca_or_p_on_l2 (2), ura_index (4), sv_health (6),
+ *      issue_of_data_clock (10); values: estimated_group_delay_differential, t_oc, a_f2, a_f1, a_f0
+ *   2  ints: fit_interval_flag; bits: issue_of_data_ephemeris (8), age_of_data_offset (5); values:
+ *      correction_to_orbital_radius_sin, mean_motion_difference_from_computed_value, mean_anomaly_at_reference_time,
+ *      correction_to_latitude_cos, eccentricity, correction_to_latitude_sin, sqrt_semi_major_axis,
+ *      reference_time_ephemeris
+ *   3  bits: issue_of_data_ephemeris (8); values: correction_to_inclination_angle_cos, longitude_of_ascending_node,
+ *      correction_to_inclination_angle_sin, inclination_angle, correction_to_orbital_radius_cos, argument_of_perigee,
+ *      rate_of_right_ascension, rate_of_inclination_angle
+ *   4  ints: data_id, page_id
+ *   5  bits: data_id (2), satellite_id (6), sv_health (8); values: eccentricity, time_of_ephemeris,
+ *      delta_inclination_angle, right_ascension_rate, semi_major_axis_sqrt, longitude_of_ascension_mode,
+ *      argument_of_perigree, mean_anomaly_at_reference_time, a_f0, a_f1
+ * Every value is exact (powers of two on integers of at most 32 bits).                                            */
+typedef struct gb200_subframe_fields {
+    int32_t event_index;  /* index of the event among the channel's events of the decode call                      */
+    int32_t ms;           /* millisecond (within the call chain) whose bit completed the subframe                  */
+    int32_t subframe_id;  /* 1..5                                                                                 */
+    int32_t reserved;
+    double tow_seconds;   /* HandoverWord.time_of_week_in_seconds (:85-93)                                         */
+    int32_t ints[2];
+    uint32_t bits[4];
+    int32_t bit_widths[4];
+    double values[10];
+} gb200_subframe_fields;
+typedef char gb200_subframe_fields_is_144_bytes[sizeof(gb200_subframe_fields) == 144 ? 1 : -1]; /* C99 static assert */
+
+/* The world model's per-satellite state (gypsum/world_model.py GpsWorldModel), one per channel and kept across calls:
+ * handle_subframe_emitted (:707-861) for every subframe, handle_prn_observed once per millisecond while the channel is
+ * tracked, and handle_lost_satellite_lock when it is dropped, in the receiver's order (receiver.py:106-137): within a
+ * millisecond the dropped channels go first (none of their events of that millisecond count), then every tracked
+ * channel counts one PRN, then the subframes of that millisecond reset the count to 0.  Like the reference, parameters
+ * of different IODE / IODC issues mix.  A channel's drop is per call: it counts again from the next call on.
+ *
+ * events_device: a device array [channel][stride] of gb200_subframe_event with counts_host[channel] events, their
+ * milliseconds event_ms_host[channel * stride + j] (non-decreasing per channel, in [0, n_ms)), drop_ms_host[channel]
+ * (-1 = none) and n_ms; or NULL for the chain: the events the last gb200_tracker_decode_subframes(NULL) call left on the
+ * device, of bits from gb200_tracker_integrate_bits(NULL records) over the records of the last gb200_tracker_process
+ * call.  On the chain an event's millisecond is its bit's ms_index and a channel drops at its first tracking record
+ * with `lost` set or at its first CannotDetermine event (kind 2), and the explicit arguments are ignored; GB200_ESTATE
+ * if the chain is broken or already parsed.  GB200_EINVAL if two seeded channels track the same replica row (the world
+ * model is keyed by satellite).  fields_host: [channel][max_fields]; field_counts_host: [channel] (> max: truncated). */
+int gb200_tracker_parse_subframes(gb200_tracker* t, const void* events_device, const int32_t* counts_host, int32_t stride,
+                                  const int32_t* event_ms_host, const int32_t* drop_ms_host, int32_t n_ms,
+                                  gb200_subframe_fields* fields_host, int32_t max_fields, int32_t* field_counts_host);
+/* One channel's state after the last parse call: params[26] in OrbitalParameterType order (SQRT_SEMI_MAJOR_AXIS ..
+ * ESTIMATED_GROUP_DELAY_DIFFERENTIAL), set_mask bit k = params[k] is not None, the PRN count and whether it counts. */
+int gb200_tracker_orbit_state(gb200_tracker* t, int channel, double params[26], uint32_t* set_mask, int64_t* prn_count,
+                              int32_t* counting);
+
+/* What the world model knows of one satellite at the end of one millisecond (56 bytes).  flags:
+ *   1  _can_interrogate_precise_timings_for_satellite (:330-360): tow and dsv are set
+ *   2  is_complete(): with flag 1, x, y, z are set
+ *   4  counting and prn_count <= 6000 (attempt_position_fix, :582-585)
+ *   8  counting (the channel is tracked)
+ *  16  frozen (the decoder raised)
+ * Values that are not set are NaN.                                                                                  */
+typedef struct gb200_sv_observation {
+    double tow;        /* _gps_observed_system_time_of_week_for_satellite (:635-705)                               */
+    double dsv;        /* its delta_sv_time after the 10th iteration                                               */
+    double x, y, z;    /* _get_satellite_position_at_time_of_week(tow) (:410-487), ECEF metres                     */
+    int64_t prn_count; /* PRNs since the last HOW, -1 when not counting                                            */
+    int32_t flags;
+    int32_t reserved;
+} gb200_sv_observation;
+typedef char gb200_sv_observation_is_56_bytes[sizeof(gb200_sv_observation) == 56 ? 1 : -1]; /* C99 static assert */
+
+/* Every (channel, millisecond) of the last gb200_tracker_parse_subframes call: out[channel * n_ms + ms].  The _device
+ * variant only enqueues (out_device: n_channels * n_ms records), for a solver on the device. */
+int gb200_tracker_observations(gb200_tracker* t, gb200_sv_observation* out_host);
+int gb200_tracker_observations_device(gb200_tracker* t, void* out_device);
 
 /* Kernel selection for gb200_acquire_cells.  Two implementations of the same arithmetic exist:
  *   0  doppler_spectra + correlate_cells: the PRN-independent half of the pipeline (wipe-off, forward transform) is

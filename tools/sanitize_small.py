@@ -39,6 +39,8 @@ for n, m in ((2046, 2), (4092, 1)):
             bits = t.integrate_bits(12, ts, ts + 0.001)
             sub = t.decode_subframes()  # subframe decoding of the bits just integrated
         assert len(bits) == 2 and t.bit_state(0)["processed_pseudosymbol_count"] == 108
+        t.parse_subframes()  # subframe fields and world-model state over the chain just decoded
+        assert t.observations().shape == (2, 12)
         # subframe decoding over caller bit events: full warp preamble scan, phase, drain, a reset and a re-sync
         import torch
 
