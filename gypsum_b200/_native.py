@@ -82,6 +82,10 @@ SYMBOLS = {
                                             C.POINTER(C.c_int32)]),
     "gb200_tracker_observations": (C.c_int, [_P, _P]),
     "gb200_tracker_observations_device": (C.c_int, [_P, _P]),
+    "gb200_tracker_position_fixes": (C.c_int, [_P, _P, _P]),
+    "gb200_tracker_position_fixes_device": (C.c_int, [_P, _P, _P]),
+    "gb200_tracker_receiver_state": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_int32), _P]),
+    "gb200_tracker_fix_repairs": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "gb200_set_fused": (C.c_int, [_P, C.c_int]),
     "gb200_launch_count": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "gb200_enable_kernel_timing": (C.c_int, [_P, C.c_int]),
@@ -635,6 +639,41 @@ class Tracker:
         self._engine._check(self._lib.gb200_tracker_observations_device(self._h, _P(out_device_ptr)),
                             "gb200_tracker_observations_device")
 
+    def _fix_times(self, receiver_timestamps) -> np.ndarray:
+        rx = np.ascontiguousarray(receiver_timestamps, dtype=np.float64)
+        if rx.shape != (self._orbit_n_ms,):
+            raise ValueError(f"receiver_timestamps must hold one start time per millisecond of the last parse_subframes "
+                             f"call ({self._orbit_n_ms})")
+        return rx
+
+    def position_fixes(self, receiver_timestamps) -> np.ndarray:
+        """FIX_DTYPE [n_ms]: the world model's position fix (world_model.py:567-633) for every millisecond of the last
+        parse_subframes call, receiver_timestamps being the chunk start times.  The receiver's clock slide, world-model
+        order and stop carry from call to call (gb200_tracker_position_fixes)."""
+        rx = self._fix_times(receiver_timestamps)
+        out = np.empty(self._orbit_n_ms, dtype=FIX_DTYPE)
+        self._engine._check(self._lib.gb200_tracker_position_fixes(self._h, _ptr(rx), _ptr(out)),
+                            "gb200_tracker_position_fixes")
+        return out
+
+    def position_fixes_device(self, receiver_timestamps, out_device_ptr: int) -> None:
+        """Enqueue only: n_ms FIX_DTYPE records to device memory."""
+        rx = self._fix_times(receiver_timestamps)
+        self._engine._check(self._lib.gb200_tracker_position_fixes_device(self._h, _ptr(rx), _P(out_device_ptr)),
+                            "gb200_tracker_position_fixes_device")
+
+    def receiver_state(self) -> dict:
+        """After the last fix call: slide (receiver_clock_slide, None before any), stopped, order: the channels in
+        the world model's order, and repaired: the fixes the serial chain recomputed where the parallel passes' chain
+        check failed (gb200_tracker_fix_repairs)."""
+        slide, stopped, repaired = C.c_double(), C.c_int32(), C.c_int64()
+        order = np.empty(self.n_channels, dtype=np.int32)
+        self._engine._check(self._lib.gb200_tracker_receiver_state(self._h, C.byref(slide), C.byref(stopped), _ptr(order)),
+                            "gb200_tracker_receiver_state")
+        self._engine._check(self._lib.gb200_tracker_fix_repairs(self._h, C.byref(repaired)), "gb200_tracker_fix_repairs")
+        return {"slide": None if np.isnan(slide.value) else slide.value, "stopped": bool(stopped.value),
+                "order": [int(c) for c in order if c >= 0], "repaired": int(repaired.value)}
+
     def subframe_state(self, channel: int) -> dict:
         out = np.zeros(6, dtype=np.int64)
         self._engine._check(self._lib.gb200_tracker_subframe_state(self._h, channel, _ptr(out)), "gb200_tracker_subframe_state")
@@ -680,6 +719,12 @@ OBSERVATION_DTYPE = np.dtype([  # gb200_sv_observation
 assert OBSERVATION_DTYPE.itemsize == 56
 ORBIT_PARAMS = 26
 OBS_TIMING, OBS_COMPLETE, OBS_FIX_GATE, OBS_COUNTING, OBS_FROZEN = 1, 2, 4, 8, 16  # OBSERVATION_DTYPE["flags"]
+FIX_DTYPE = np.dtype([  # gb200_position_fix
+    ("receiver_timestamp", "<f8"), ("slide_in", "<f8"), ("slide_out", "<f8"), ("clock_bias", "<f8"), ("x", "<f8"),
+    ("y", "<f8"), ("z", "<f8"), ("pseudorange", "<f8", (4,)), ("status", "<i4"), ("n_ready", "<i4"),
+    ("channel", "<i4", (4,))])
+assert FIX_DTYPE.itemsize == 112
+FIX_NONE, FIX_SOLVED, FIX_RAISED, FIX_STOPPED = 0, 1, 2, 3  # FIX_DTYPE["status"]
 
 
 def subframe_event_capacity(n_bits: int) -> int:

@@ -16,6 +16,7 @@
 #include "../../include/gypsum_b200.h"
 #include "bits_core.cuh"
 #include "kernels.cuh"
+#include "fix_core.cuh"
 #include "nav_core.cuh"
 #include "orbit_core.cuh"
 
@@ -200,6 +201,15 @@ struct gb200_tracker {
     int change_stride = 0;
     DevBuf<SvObservation> d_obs;
     PinnedBuf<SvObservation> h_obs;
+    // position fixes: the receiver state (d_fix_bank, d_fix_rank) exists from the first fix call on
+    DevBuf<FixBank> d_fix_bank;
+    DevBuf<int> d_fix_rank, d_fix_order, d_fix_touch, d_fix_prev;
+    DevBuf<double> d_fix_rx, d_fix_reset, d_fix_slide1;
+    DevBuf<FixRecord> d_fixes;
+    PinnedBuf<double> h_fix_rx;
+    PinnedBuf<FixRecord> h_fixes;
+    bool fix_pending = false;  // the last parse call's fixes are not computed yet
+    bool fix_gap = false;      // a parse call's fixes were skipped after the first fix call
 };
 // A pipelined stream of grid batches: slot k's host->device copy, compute and device->host copy run on three streams.
 struct gb200_grid_stream {
@@ -245,6 +255,11 @@ static_assert(sizeof(gb200_sv_observation) == sizeof(SvObservation) &&
                   offsetof(gb200_sv_observation, prn_count) == offsetof(SvObservation, prn_count) &&
                   offsetof(gb200_sv_observation, flags) == offsetof(SvObservation, flags),
               "ABI observation and device observation must match");
+static_assert(sizeof(gb200_position_fix) == sizeof(FixRecord) &&
+                  offsetof(gb200_position_fix, pseudorange) == offsetof(FixRecord, pseudorange) &&
+                  offsetof(gb200_position_fix, status) == offsetof(FixRecord, status) &&
+                  offsetof(gb200_position_fix, channel) == offsetof(FixRecord, channel),
+              "ABI position fix and device fix must match");
 static_assert(offsetof(gb200_subframe_event, words) == offsetof(SubframeEvent, words) &&
                   offsetof(gb200_subframe_event, kind) == offsetof(SubframeEvent, kind) &&
                   offsetof(gb200_subframe_event, parity_ok) == offsetof(SubframeEvent, parity_ok),
@@ -1695,6 +1710,8 @@ int gb200_tracker_parse_subframes(gb200_tracker* t, const void* events_device, c
     if (!events_device) t->chain_sub_n_ms = 0;
     t->orbit_n_ms = n_ms;
     t->change_stride = stride + 2;
+    if (t->d_fix_bank.p && t->fix_pending) t->fix_gap = true;
+    t->fix_pending = true;
     // the counts' copy is enqueued first, so the fields' download waits for both
     GB_CUDA(e, cudaMemcpyAsync(t->h_field_counts.p, t->d_field_counts.p, nc * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
     GB_CUDA(e, cudaStreamSynchronize(e->stream));
@@ -1750,6 +1767,111 @@ int gb200_tracker_observations(gb200_tracker* t, gb200_sv_observation* out_host)
     if (n) GB_CUDA(e, t->d_obs.ensure(n));
     GB_TRY(observations_launch(t, t->d_obs.p));
     return download(e, reinterpret_cast<SvObservation*>(out_host), t->d_obs.p, n, t->h_obs);
+}
+
+// The observations of the last parse call and the fixes over them (fix.cu), enqueued into out_dev.
+static int fixes_launch(gb200_tracker* t, const double* rx_host, FixRecord* out_dev) {
+    gb200_engine* e = t->e;
+    if (!rx_host) GB_FAIL(e, GB200_EINVAL, "null receiver timestamps");
+    if (!t->orbit_n_ms) GB_FAIL(e, GB200_ESTATE, "no gb200_tracker_parse_subframes call yet");
+    if (t->fix_gap)
+        GB_FAIL(e, GB200_ESTATE, "the fixes of an earlier parse call were skipped: the receiver's clock slide chain has a gap");
+    if (!t->fix_pending) GB_FAIL(e, GB200_ESTATE, "the fixes of the last parse call were already computed");
+    const int nc = t->n_channels, n_ms = t->orbit_n_ms;
+    GB_CUDA(e, cudaStreamSynchronize(e->stream));  // pinned staging may still be in flight
+    if (!t->d_fix_bank.p) {
+        FixBank b{};
+        b.slide = NAN;
+        const std::vector<int> rank(nc, -1);
+        GB_CUDA(e, t->d_fix_bank.ensure(1));
+        GB_CUDA(e, t->d_fix_rank.ensure(nc));
+        GB_CUDA(e, cudaMemcpy(t->d_fix_bank.p, &b, sizeof(b), cudaMemcpyHostToDevice));
+        GB_CUDA(e, cudaMemcpy(t->d_fix_rank.p, rank.data(), sizeof(int) * nc, cudaMemcpyHostToDevice));
+    }
+    GB_CUDA(e, t->d_obs.ensure(static_cast<size_t>(nc) * n_ms));
+    GB_CUDA(e, t->d_fix_order.ensure(nc));
+    GB_CUDA(e, t->d_fix_touch.ensure(nc));
+    GB_CUDA(e, t->d_fix_prev.ensure(n_ms));
+    GB_CUDA(e, t->d_fix_rx.ensure(n_ms));
+    GB_CUDA(e, t->d_fix_reset.ensure(n_ms));
+    GB_CUDA(e, t->d_fix_slide1.ensure(n_ms));
+    GB_TRY(upload(e, t->d_fix_rx.p, rx_host, n_ms, t->h_fix_rx));
+    GB_TRY(observations_launch(t, t->d_obs.p));
+    FixArgs a{};
+    a.changes = t->d_changes.p;
+    a.change_counts = t->d_change_counts.p;
+    a.change_stride = t->change_stride;
+    a.obs = t->d_obs.p;
+    a.rx = t->d_fix_rx.p;
+    a.bank = t->d_fix_bank.p;
+    a.rank = t->d_fix_rank.p;
+    a.order = t->d_fix_order.p;
+    a.touch_ms = t->d_fix_touch.p;
+    a.reset = t->d_fix_reset.p;
+    a.prev = t->d_fix_prev.p;
+    a.slide1 = t->d_fix_slide1.p;
+    a.out = out_dev;
+    a.n_channels = nc;
+    a.n_ms = n_ms;
+    GB_LAUNCH(e, -1, launch_position_fixes(a, e->stream));
+    e->launches += 4;  // plan, two passes, repair and finish
+    t->fix_pending = false;
+    return GB200_OK;
+}
+
+int gb200_tracker_position_fixes_device(gb200_tracker* t, const double* receiver_timestamps_host, void* out_device) {
+    if (!t) return GB200_EINVAL;
+    if (!out_device) GB_FAIL(t->e, GB200_EINVAL, "null output");
+    GB_CUDA(t->e, cudaSetDevice(t->e->device));
+    return fixes_launch(t, receiver_timestamps_host, static_cast<FixRecord*>(out_device));
+}
+
+int gb200_tracker_position_fixes(gb200_tracker* t, const double* receiver_timestamps_host, gb200_position_fix* out_host) {
+    if (!t) return GB200_EINVAL;
+    gb200_engine* e = t->e;
+    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
+    GB_CUDA(e, cudaSetDevice(e->device));
+    const size_t n = static_cast<size_t>(t->orbit_n_ms);
+    if (n) GB_CUDA(e, t->d_fixes.ensure(n));
+    GB_TRY(fixes_launch(t, receiver_timestamps_host, t->d_fixes.p));
+    return download(e, reinterpret_cast<FixRecord*>(out_host), t->d_fixes.p, n, t->h_fixes);
+}
+
+int gb200_tracker_fix_repairs(gb200_tracker* t, int64_t* n) {
+    if (!t) return GB200_EINVAL;
+    gb200_engine* e = t->e;
+    if (!n) GB_FAIL(e, GB200_EINVAL, "null output");
+    FixBank b{};
+    if (t->d_fix_bank.p) {
+        GB_CUDA(e, cudaSetDevice(e->device));
+        GB_CUDA(e, cudaStreamSynchronize(e->stream));
+        GB_CUDA(e, cudaMemcpy(&b, t->d_fix_bank.p, sizeof(b), cudaMemcpyDeviceToHost));
+    }
+    *n = b.n_repaired;
+    return GB200_OK;
+}
+
+int gb200_tracker_receiver_state(gb200_tracker* t, double* slide, int32_t* stopped, int32_t* order) {
+    if (!t) return GB200_EINVAL;
+    gb200_engine* e = t->e;
+    const int nc = t->n_channels;
+    FixBank b{};
+    b.slide = NAN;
+    std::vector<int> rank(nc, -1);
+    if (t->d_fix_bank.p) {
+        GB_CUDA(e, cudaSetDevice(e->device));
+        GB_CUDA(e, cudaStreamSynchronize(e->stream));
+        GB_CUDA(e, cudaMemcpy(&b, t->d_fix_bank.p, sizeof(b), cudaMemcpyDeviceToHost));
+        GB_CUDA(e, cudaMemcpy(rank.data(), t->d_fix_rank.p, sizeof(int) * nc, cudaMemcpyDeviceToHost));
+    }
+    if (slide) *slide = b.has_slide ? b.slide : NAN;
+    if (stopped) *stopped = b.stopped;
+    if (order) {
+        for (int k = 0; k < nc; ++k) order[k] = -1;
+        for (int c = 0; c < nc; ++c)
+            if (rank[c] >= 0 && rank[c] < nc) order[rank[c]] = c;
+    }
+    return GB200_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -145,6 +145,27 @@ cudaError_t launch_parse_subframes(const OrbitArgs& a, cudaStream_t st);
 cudaError_t launch_sv_observations(const OrbitSnap* changes, const int* change_counts, int change_stride, int n_channels,
                                    int n_ms, SvObservation* out, cudaStream_t st);
 
+// position_fixes: the world model's fix for every millisecond of the last parse call (fix.cu, fix_core.cuh).
+struct FixBank;
+struct FixRecord;
+struct FixArgs {
+    const OrbitSnap* changes;    // the last parse call's change tables, [n_channels][change_stride]
+    const int* change_counts;    // [n_channels]
+    int change_stride;
+    const SvObservation* obs;    // [n_channels][n_ms]
+    const double* rx;            // [n_ms] receiver timestamps (chunk start times)
+    FixBank* bank;               // the receiver's state, carried from call to call
+    int* rank;                   // [n_channels] world-model order, -1 = not in it; carried
+    int* order;                  // [n_channels] scratch: the channels by rank
+    int* touch_ms;               // [n_channels] scratch: 2 * first-touch ms + (1 subframe, 0 drop); -1 before the call
+    double* reset;               // [n_ms] scratch: the slide the millisecond's subframes set, NaN = none
+    int* prev;                   // [n_ms] scratch: the previous fixing millisecond of the segment, -1 = none
+    double* slide1;              // [n_ms] scratch: pass 1's slide after each fix
+    FixRecord* out;              // [n_ms]
+    int n_channels, n_ms;
+};
+cudaError_t launch_position_fixes(const FixArgs& a, cudaStream_t st);
+
 // acquire_fused: one CTA per (PRN, Doppler) cell, the whole pipeline in one kernel (fused.cu).
 struct FusedArgs {
     const float2* iq;       // [M*N] one block

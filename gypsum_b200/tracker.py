@@ -385,6 +385,13 @@ class TrackerBank:
         :635-705), the PRN count and flags."""
         return self.native.observations()
 
+    def position_fixes(self, start_times) -> np.ndarray:
+        """_native.FIX_DTYPE [ms] over the milliseconds of the last parse_subframes call: the position fix the world
+        model attempts every millisecond (world_model.py:567-633), start_times being the chunk start times.  The bank is
+        one receiver: its clock slide, world-model order and stop carry from call to call.
+        gypsum_b200.world_model.solution_from_fix turns a status-1 record into a ReceiverSolution."""
+        return self.native.position_fixes(start_times)
+
 
 # OrbitalParameterType (world_model.py:151-199), in order
 ORBITAL_PARAMETER_NAMES = (

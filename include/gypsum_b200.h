@@ -367,6 +367,47 @@ typedef char gb200_sv_observation_is_56_bytes[sizeof(gb200_sv_observation) == 56
 int gb200_tracker_observations(gb200_tracker* t, gb200_sv_observation* out_host);
 int gb200_tracker_observations_device(gb200_tracker* t, void* out_device);
 
+/* The world model's position fix for one millisecond (112 bytes): GpsWorldModel.attempt_position_fix (:567-633), which
+ * the reference receiver calls every millisecond with the chunk's start time.  A tracker is one receiver: it has one
+ * clock slide, which every subframe of any channel resets to tow - trailing_edge_receiver_timestamp (:749-752, the last
+ * one of a millisecond wins, channels in order), and one world-model order, in which satellites enter at their first
+ * subframe or lost lock.  A millisecond's ready channels have flags 2 and 4; with exactly 4, _compute_position runs 5
+ * rounds of 20 Newton iterations from zero, and after each round the slide drops by the clock bias.  status:
+ *   0  no fix: fewer than 4 ready, or no slide yet
+ *   1  fixed: everything set
+ *   2  the reference raises here (5 or more ready: numpy's non-square solve; or an exactly singular system); slide_in
+ *      and slide_out hold the slide at the raise
+ *   3  stopped: the receiver raised earlier, or a channel's decoder raised (event kind 3) at or before this ms
+ * Values that are not set are NaN.  Parity with the reference is a bound (DESIGN.md §6): numpy's LAPACK cannot be
+ * matched bit for bit. */
+typedef struct gb200_position_fix {
+    double receiver_timestamp;
+    double slide_in;        /* receiver_clock_slide entering _compute_position                                   */
+    double slide_out;       /* and after it                                                                      */
+    double clock_bias;      /* ReceiverSolution.clock_bias, seconds                                              */
+    double x, y, z;         /* ReceiverSolution.receiver_pos, ECEF metres                                        */
+    double pseudorange[4];  /* round 0's get_pseudorange_for_satellite of each row, seconds                      */
+    int32_t status;
+    int32_t n_ready;        /* channels with flags 2 and 4                                                       */
+    int32_t channel[4];     /* the rows in world-model order, -1 where unused                                    */
+} gb200_position_fix;
+typedef char gb200_position_fix_is_112_bytes[sizeof(gb200_position_fix) == 112 ? 1 : -1]; /* C99 static assert */
+
+/* One record per millisecond of the last gb200_tracker_parse_subframes call, receiver_timestamps_host[n_ms] being the
+ * chunk start times; the receiver's slide, order and stop carry to the next call.  GB200_ESTATE if there has been no
+ * parse call, if that call's fixes were already computed, or if an earlier parse call's fixes were skipped after the
+ * first fix call (the slide chain would have a gap).  The _device variant only enqueues (out_device: n_ms records). */
+int gb200_tracker_position_fixes(gb200_tracker* t, const double* receiver_timestamps_host, gb200_position_fix* out_host);
+int gb200_tracker_position_fixes_device(gb200_tracker* t, const double* receiver_timestamps_host, void* out_device);
+/* The receiver's state after the last fix call: the clock slide (NaN = None), whether it has stopped, and
+ * order[n_channels]: the channels in world-model order, -1 after the last. */
+int gb200_tracker_receiver_state(gb200_tracker* t, double* slide, int32_t* stopped, int32_t* order);
+/* Fixes the serial chain recomputed so far.  The fixes of a call run in two parallel passes (DESIGN.md §8c): each fix
+ * from the slide its segment's last reset set, then again from the slide the first pass left at the previous fix.
+ * Every fix checks that it left the slide the next one started from; from the first one that did not, the call's
+ * chain runs again serially, each fix from the slide the fix before it left.  This counts the fixes so recomputed. */
+int gb200_tracker_fix_repairs(gb200_tracker* t, int64_t* n);
+
 /* Kernel selection for gb200_acquire_cells.  Two implementations of the same arithmetic exist:
  *   0  doppler_spectra + correlate_cells: the PRN-independent half of the pipeline (wipe-off, forward transform) is
  *      computed once per distinct Doppler bin and shared by every PRN -- the grid shape (gb200_acquire_grid always

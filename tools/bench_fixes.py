@@ -1,0 +1,110 @@
+"""Times gb200_tracker_position_fixes_device: 4 channels x 60 000 ms with a fix on every millisecond from the third,
+next to the tracking launch it follows (4 channels x 60 s of device-resident IQ, a 1-s synthetic base repeated).  The
+four channels carry their own planted ephemerides (oracle/orbit_oracle.py) with the same TOW counts: subframes 1-3 land
+in milliseconds 0-2 and then one every 6 s on all four, so their times of week stay consistent.  Each call is
+bracketed by CUDA events on the engine's stream (the fix call includes the upload of the receiver timestamps and the
+observations it computes first); one round is also profiled for the kernels alone.
+usage (GPU box): python tools/bench_fixes.py [--reps 5]"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from gypsum_b200 import _native  # noqa: E402
+from gypsum_b200 import synth as to  # noqa: E402
+from gypsum_b200.gps_ca_prn_codes import ca_code_chips  # noqa: E402
+from oracle import orbit_oracle as orb  # noqa: E402
+
+N, FS = 2046, 2046000
+N_CH, N_MS, N_SUB = 4, 60000, 12
+
+
+def timed(stream, fn):
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record(stream)
+    out = fn()
+    b.record(stream)
+    b.synchronize()
+    return a.elapsed_time(b), out
+
+
+def power_limit() -> str:
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception:  # noqa: BLE001
+        return "unknown"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=5)
+    args = ap.parse_args()
+    eng = _native.Engine(FS, N)
+    eng.set_replicas(np.stack([ca_code_chips(sv) for sv in range(1, 33)]).astype(np.uint8))
+    stream = torch.cuda.Stream()
+    eng.set_stream(stream.cuda_stream)
+    svs = (5, 12, 19, 27)
+    chans = [(sv, 1000.0 + 37.3 * c, 0.0, (53 * c) % N, 0.1 * c, 0.004) for c, sv in enumerate(svs)]
+    base = to.synth_tracking_iq(5, N, 1000, FS, chans)
+    xd = torch.from_numpy(base).cuda().repeat(N_MS // 1000)
+    eng.bind_iq_device(xd.data_ptr(), xd.numel())
+    times = np.array([round(k * N / FS, 6) for k in range(N_MS)])
+    rec = torch.empty(N_CH * N_MS * _native.TRACK_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+
+    rng = np.random.default_rng(1)
+    host = np.zeros((N_CH, N_SUB), dtype=_native.SUBFRAME_DTYPE)
+    ems = np.zeros((N_CH, N_SUB), dtype=np.int32)
+    for c, sv in enumerate(svs):
+        sfs = orb.ephemeris_subframes(orb.realistic_ephemeris(rng, sv), N_SUB, first_id=1, tow0=20000, seed=c)
+        for k, sf in enumerate(sfs):
+            m = k if k < 3 else 2 + 6000 * (k - 2)
+            host[c, k]["words"] = orb.words_of(sf)
+            host[c, k]["trailing_edge_receiver_timestamp"] = times[min(m, N_MS - 1)] - 0.0003 * c
+            ems[c, k] = min(m, N_MS - 1)
+    ev_dev = torch.from_numpy(host.view(np.uint8).reshape(N_CH, -1)).cuda()
+    counts = np.full(N_CH, N_SUB, dtype=np.int32)
+    drop = np.full(N_CH, -1, dtype=np.int32)
+    out = torch.empty(N_MS * _native.FIX_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+
+    track_ms, fix_ms, kernel_ms = [], [], {}
+    for rep in range(args.reps + 1):
+        trk = _native.Tracker(eng, list(range(N_CH)), [c[1] for c in chans], [0.0] * N_CH, [c[3] for c in chans])
+        dt, _ = timed(stream, lambda: trk.process_device(N_MS, times, rec.data_ptr()))
+        trk.parse_subframes(ev_dev.data_ptr(), counts, N_SUB, ems, drop, N_MS)
+        prof = torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) if rep == 1 else None
+        if prof:
+            prof.__enter__()
+        df, _ = timed(stream, lambda: trk.position_fixes_device(times, out.data_ptr()))
+        if prof:
+            prof.__exit__(None, None, None)
+            for k in prof.key_averages():
+                for name in ("k_sv_observations", "k_fix_plan", "k_fix_pass<1>", "k_fix_pass<2>", "k_fix_finish"):
+                    if name in k.key:
+                        kernel_ms[name] = getattr(k, "device_time_total", getattr(k, "cuda_time_total", 0.0)) / 1e3
+        if rep:  # the first round allocates
+            track_ms.append(dt)
+            fix_ms.append(df)
+        trk.close()
+    f = out.cpu().numpy().view(_native.FIX_DTYPE)
+    dev = torch.cuda.get_device_properties(0)
+    print(json.dumps({
+        "workload": f"position_fixes_device: {N_CH} channels x {N_MS} ms after the parse call",
+        "gpu": dev.name, "power_limit": power_limit(),
+        "fix_call_ms_median": float(np.median(fix_ms)), "fix_call_ms": fix_ms,
+        "kernel_ms_profiled": kernel_ms,
+        "tracking_launch_ms_median": float(np.median(track_ms)),
+        "fix_fraction_of_tracking": float(np.median(fix_ms) / np.median(track_ms)),
+        "fixes": int((f["status"] == _native.FIX_SOLVED).sum()),
+        "status_counts": [int(v) for v in np.bincount(f["status"], minlength=4)]}), flush=True)
+    eng.close()
+
+
+if __name__ == "__main__":
+    main()

@@ -41,6 +41,8 @@ for n, m in ((2046, 2), (4092, 1)):
         assert len(bits) == 2 and t.bit_state(0)["processed_pseudosymbol_count"] == 108
         t.parse_subframes()  # subframe fields and world-model state over the chain just decoded
         assert t.observations().shape == (2, 12)
+        assert t.position_fixes(ts).shape == (12,)  # plan, both passes and finish of the position fix
+        assert t.receiver_state()["slide"] is None
         # subframe decoding over caller bit events: full warp preamble scan, phase, drain, a reset and a re-sync
         import torch
 
