@@ -192,7 +192,9 @@ __global__ void __launch_bounds__(kFixThreads) k_fix_pass(const FixArgs a) {
 }
 
 // Where the chain check failed, the serial chain: from the first miss on, every fix that does not start from a reset
-// runs again from the slide the fix before it left, in order, in one thread.
+// runs again from the slide the fix before it left, in order, in one thread.  The comparison is exact, not the check's
+// 4 ulp: after a miss every fix of the call, in later segments too, is the serial chain's bit for bit, and n_repaired
+// counts each fix whose entering slide changed.
 __global__ void __launch_bounds__(32) k_fix_repair(const FixArgs a) {
     FixBank& bk = *a.bank;
     if (threadIdx.x != 0 || bk.first_miss >= a.n_ms) return;

@@ -404,8 +404,11 @@ int gb200_tracker_position_fixes_device(gb200_tracker* t, const double* receiver
 int gb200_tracker_receiver_state(gb200_tracker* t, double* slide, int32_t* stopped, int32_t* order);
 /* Fixes the serial chain recomputed so far.  The fixes of a call run in two parallel passes (DESIGN.md §8c): each fix
  * from the slide its segment's last reset set, then again from the slide the first pass left at the previous fix.
- * Every fix checks that it left the slide the next one started from; from the first one that did not, the call's
- * chain runs again serially, each fix from the slide the fix before it left.  This counts the fixes so recomputed. */
+ * Every fix checks that it left, to 4 ulp, the slide the next one started from; from the first one that did not, the
+ * call's chain runs again serially, each fix from the slide the fix before it left.  This counts the fixes so
+ * recomputed: those after the first miss, up to the first raise, that do not start a segment and whose entering slide
+ * differed in any bit from the slide the fix before them left.  A receiver-clock jump inside a segment (a gap in the
+ * sample stream) is an input that makes the check fail. */
 int gb200_tracker_fix_repairs(gb200_tracker* t, int64_t* n);
 
 /* Kernel selection for gb200_acquire_cells.  Two implementations of the same arithmetic exist:

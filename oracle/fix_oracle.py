@@ -69,6 +69,7 @@ class ReceiverOracle:
         self.order: list[int] = []
         self.stopped = False
         self.rows: dict = {}  # ms of the last call -> the rows [(tow, x, y, z)] of its fix
+        self.resets: dict = {}  # ms of the last call -> the slide its subframes set
 
     def _touch(self, ch: int) -> None:
         if ch not in self.order:
@@ -91,7 +92,7 @@ class ReceiverOracle:
                 by[ch].setdefault(m, []).append((kind, w, te))
         drops = [d for _, d in chans]
         tracked = [True] * len(chans)
-        self.rows = {}
+        self.rows, self.resets = {}, {}
         out = np.zeros(n_ms, dtype=FIX_DTYPE)
         for m in range(n_ms):
             f = out[m]
@@ -123,6 +124,7 @@ class ReceiverOracle:
                             self._touch(ch)
                             self.sats[ch].subframe(fields, te)
                             self.slide = fields["tow_seconds"] - te  # world_model.py:749-752
+                            self.resets[m] = self.slide
             ready = [ch for ch in self.order if self._ready(ch)]
             f["n_ready"] = len(ready)
             f["channel"][:min(4, len(ready))] = ready[:4]
@@ -158,6 +160,72 @@ class ReceiverOracle:
             f["slide_out"], f["clock_bias"], f["x"], f["y"], f["z"] = slide, cb, *pos
             f["pseudorange"] = pr
         return out
+
+
+def same_slide(a, b) -> bool:
+    """fix_same_slide: the device's chain check, 4 units in the last place."""
+    return abs(a - b) <= 4.0 * 2.0 ** -52 * abs(b)
+
+
+def device_passes(compute, rec, rows, resets, carried):
+    """The device's fix kernels (gypsum_b200/csrc/fix.cu) on one call, from the receiver's decisions: rec, rows and
+    resets are ReceiverOracle.call's records, .rows and .resets, carried the slide entering the call (None: none), and
+    compute(rows, receiver_timestamp, slide) the fix (a FIX_DTYPE record; the host core makes this exact for the
+    device).  Pass 1 fixes every millisecond from its segment's slide (the last reset's, or the carried one); pass 2
+    from pass 1's slide at the previous fix of the segment (at a reset: the reset value); a pass-2 fix whose slide is
+    not within 4 ulp of pass 1's is a miss; from the first miss on, up to the first raise, every fix that does not start
+    a segment and whose entering slide is not bit-equal to the slide the fix before it left is fixed again from that
+    slide (k_fix_repair).  Fixes after a singular raise, which the device computes and then discards, are not modelled.
+    Returns a dict: pass1 and out (ms -> record: pass 1's, and the final one), first_miss / first_raise (None: none),
+    repaired (the milliseconds k_fix_repair fixes again) and slide (what the call carries to the next)."""
+    fixing = [m for m in range(len(rec)) if rec[m]["status"] in (FIX_SOLVED, FIX_RAISED)]
+
+    def fix(m, s):
+        r = rec[m]
+        if r["n_ready"] > 4:  # the non-square system: raised before anything changes
+            f = r.copy()
+            f["status"], f["slide_in"], f["slide_out"] = FIX_RAISED, s, s
+            return f
+        return compute(rows[m], r["receiver_timestamp"], s)
+
+    seg, prev, prevs, pass1, out = carried, None, {}, {}, {}
+    for m in range(len(rec)):
+        if m in resets:
+            seg, prev = resets[m], None
+        if rec[m]["status"] not in (FIX_SOLVED, FIX_RAISED):
+            continue
+        pass1[m] = fix(m, seg)
+        s = seg if prev is None else pass1[prev]["slide_out"]
+        out[m] = pass1[m] if s == seg else fix(m, s)
+        prevs[m], prev = prev, m
+    miss = [m for m in fixing if not same_slide(out[m]["slide_out"], pass1[m]["slide_out"])]
+    raised = [m for m in fixing if out[m]["status"] == FIX_RAISED]
+    first_miss = miss[0] if miss else None
+    first_raise = raised[0] if raised else len(rec)
+    repaired = []
+    if first_miss is not None:
+        last = first_miss
+        for m in fixing:
+            if m <= first_miss:
+                continue
+            if m > first_raise:
+                break
+            s = out[last]["slide_out"]
+            if prevs[m] is not None and not out[m]["slide_in"] == s:
+                out[m] = fix(m, s)
+                repaired.append(m)
+                if out[m]["status"] == FIX_RAISED:
+                    first_raise = min(first_raise, m)
+            last = m
+    out = {m: f for m, f in out.items() if m <= first_raise}
+    if first_raise < len(rec):
+        slide = float(out[first_raise]["slide_out"])
+    elif fixing and fixing[-1] >= max(resets, default=-1):
+        slide = float(out[fixing[-1]]["slide_out"])
+    else:
+        slide = resets[max(resets)] if resets else carried
+    return {"pass1": pass1, "out": out, "first_miss": first_miss, "repaired": repaired,
+            "first_raise": first_raise if first_raise < len(rec) else None, "slide": slide}
 
 
 def golden_fix_rows(z, name: str, call: int) -> np.ndarray:

@@ -4,7 +4,12 @@ four channels carry their own planted ephemerides (oracle/orbit_oracle.py) with 
 in milliseconds 0-2 and then one every 6 s on all four, so their times of week stay consistent.  Each call is
 bracketed by CUDA events on the engine's stream (the fix call includes the upload of the receiver timestamps and the
 observations it computes first); one round is also profiled for the kernels alone.
-usage (GPU box): python tools/bench_fixes.py [--reps 5]"""
+
+--jump J puts a receiver-clock jump of J seconds (a gap in the sample stream) at millisecond --jump-ms: from there on,
+J is added to the fix call's receiver timestamps and to every later trailing edge.  Inside a segment that makes the
+device's chain check miss, and k_fix_repair recomputes the rest of the segment serially (DESIGN.md §8c); the result
+line then also reports the repaired fixes and the cost of each.
+usage (GPU box): python tools/bench_fixes.py [--reps 5] [--jump -0.2 [--jump-ms 1000]]"""
 import argparse
 import json
 import os
@@ -45,6 +50,8 @@ def power_limit() -> str:
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--jump", type=float, default=0.0, help="receiver-clock jump in seconds (0: none)")
+    ap.add_argument("--jump-ms", type=int, default=1000, help="the millisecond the jump lands on")
     args = ap.parse_args()
     eng = _native.Engine(FS, N)
     eng.set_replicas(np.stack([ca_code_chips(sv) for sv in range(1, 33)]).astype(np.uint8))
@@ -57,6 +64,8 @@ def main():
     eng.bind_iq_device(xd.data_ptr(), xd.numel())
     times = np.array([round(k * N / FS, 6) for k in range(N_MS)])
     rec = torch.empty(N_CH * N_MS * _native.TRACK_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+    fix_times = times.copy()
+    fix_times[args.jump_ms:] += args.jump
 
     rng = np.random.default_rng(1)
     host = np.zeros((N_CH, N_SUB), dtype=_native.SUBFRAME_DTYPE)
@@ -66,14 +75,14 @@ def main():
         for k, sf in enumerate(sfs):
             m = k if k < 3 else 2 + 6000 * (k - 2)
             host[c, k]["words"] = orb.words_of(sf)
-            host[c, k]["trailing_edge_receiver_timestamp"] = times[min(m, N_MS - 1)] - 0.0003 * c
+            host[c, k]["trailing_edge_receiver_timestamp"] = fix_times[min(m, N_MS - 1)] - 0.0003 * c
             ems[c, k] = min(m, N_MS - 1)
     ev_dev = torch.from_numpy(host.view(np.uint8).reshape(N_CH, -1)).cuda()
     counts = np.full(N_CH, N_SUB, dtype=np.int32)
     drop = np.full(N_CH, -1, dtype=np.int32)
     out = torch.empty(N_MS * _native.FIX_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
 
-    track_ms, fix_ms, kernel_ms = [], [], {}
+    track_ms, fix_ms, kernel_ms, repaired = [], [], {}, []
     for rep in range(args.reps + 1):
         trk = _native.Tracker(eng, list(range(N_CH)), [c[1] for c in chans], [0.0] * N_CH, [c[3] for c in chans])
         dt, _ = timed(stream, lambda: trk.process_device(N_MS, times, rec.data_ptr()))
@@ -81,19 +90,25 @@ def main():
         prof = torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) if rep == 1 else None
         if prof:
             prof.__enter__()
-        df, _ = timed(stream, lambda: trk.position_fixes_device(times, out.data_ptr()))
+        df, _ = timed(stream, lambda: trk.position_fixes_device(fix_times, out.data_ptr()))
         if prof:
             prof.__exit__(None, None, None)
             for k in prof.key_averages():
-                for name in ("k_sv_observations", "k_fix_plan", "k_fix_pass<1>", "k_fix_pass<2>", "k_fix_finish"):
+                for name in ("k_sv_observations", "k_fix_plan", "k_fix_pass<1>", "k_fix_pass<2>", "k_fix_repair",
+                             "k_fix_finish"):
                     if name in k.key:
                         kernel_ms[name] = getattr(k, "device_time_total", getattr(k, "cuda_time_total", 0.0)) / 1e3
         if rep:  # the first round allocates
             track_ms.append(dt)
             fix_ms.append(df)
+        repaired.append(trk.receiver_state()["repaired"])
         trk.close()
     f = out.cpu().numpy().view(_native.FIX_DTYPE)
     dev = torch.cuda.get_device_properties(0)
+    jump = {}
+    if args.jump:
+        jump = {"jump_s": args.jump, "jump_ms": args.jump_ms, "repaired_fixes": repaired[-1],
+                "repair_kernel_us_per_fix": kernel_ms.get("k_fix_repair", 0.0) * 1e3 / max(1, repaired[-1])}
     print(json.dumps({
         "workload": f"position_fixes_device: {N_CH} channels x {N_MS} ms after the parse call",
         "gpu": dev.name, "power_limit": power_limit(),
@@ -102,7 +117,7 @@ def main():
         "tracking_launch_ms_median": float(np.median(track_ms)),
         "fix_fraction_of_tracking": float(np.median(fix_ms) / np.median(track_ms)),
         "fixes": int((f["status"] == _native.FIX_SOLVED).sum()),
-        "status_counts": [int(v) for v in np.bincount(f["status"], minlength=4)]}), flush=True)
+        "status_counts": [int(v) for v in np.bincount(f["status"], minlength=4)], **jump}), flush=True)
     eng.close()
 
 
