@@ -86,6 +86,7 @@ SYMBOLS = {
     "gb200_tracker_position_fixes_device": (C.c_int, [_P, _P, _P]),
     "gb200_tracker_receiver_state": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_int32), _P]),
     "gb200_tracker_fix_repairs": (C.c_int, [_P, C.POINTER(C.c_int64)]),
+    "gb200_tracker_chain_sizes": (C.c_int, [_P, _P]),
     "gb200_set_fused": (C.c_int, [_P, C.c_int]),
     "gb200_launch_count": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "gb200_enable_kernel_timing": (C.c_int, [_P, C.c_int]),
@@ -482,8 +483,6 @@ class Tracker:
     def undo_channel(self, channel: int) -> None:
         self._engine._check(self._lib.gb200_tracker_undo_channel(self._h, int(channel)), "gb200_tracker_undo_channel")
 
-    _last_bit_stride = 0  # events per channel the last integrate_bits call could hold
-
     def __init__(self, engine: Engine, prn_idx, doppler_hz, carrier_phase, code_phase):
         self._engine = engine
         self._lib = engine._lib
@@ -534,17 +533,26 @@ class Tracker:
         if t0.shape != (n_ms,) or t1.shape != (n_ms,):
             raise ValueError("start_times / end_times must hold one timestamp per millisecond")
         cap = n_ms // 20 + 8  # whole bits in the call + the backlog a first phase decision releases (<= 81 symbols)
-        ev = np.empty((self.n_channels, cap), dtype=BIT_DTYPE)
+        records = None if records_device_ptr is None else _P(records_device_ptr)
+        return self._per_channel("gb200_tracker_integrate_bits", BIT_DTYPE, cap, "bit event",  # cannot truncate: see `cap`
+                                 n_ms, _ptr(t0), _ptr(t1), records)
+
+    def _per_channel(self, name: str, dtype, cap: int, what: str, *args) -> list:
+        """Calls the C function `name` with (handle, *args, out, cap, counts), out being [n_channels, cap] of dtype, and
+        returns the events of each channel."""
+        out = np.empty((self.n_channels, cap), dtype=dtype)
         cnt = np.empty(self.n_channels, dtype=np.int32)
-        self._engine._check(
-            self._lib.gb200_tracker_integrate_bits(self._h, n_ms, _ptr(t0), _ptr(t1),
-                                                   None if records_device_ptr is None else _P(records_device_ptr),
-                                                   _ptr(ev), cap, _ptr(cnt)), "gb200_tracker_integrate_bits")
+        self._engine._check(getattr(self._lib, name)(self._h, *args, _ptr(out), cap, _ptr(cnt)), name)
         if (cnt > cap).any():
-            raise RuntimeError("bit event buffer too small")  # cannot happen: see `cap`
-        self._last_bit_stride = cap
-        self._chain_bits_n_ms = n_ms if records_device_ptr is None else 0
-        return [ev[c, : cnt[c]].copy() for c in range(self.n_channels)]
+            raise RuntimeError(f"{what} buffer too small")
+        return [out[c, : cnt[c]].copy() for c in range(self.n_channels)]
+
+    def _chain_sizes(self) -> list[int]:
+        """Bit events per channel the last integrate_bits call kept, subframe events per channel the last
+        decode_subframes call kept, and the milliseconds of the last parse_subframes call (gb200_tracker_chain_sizes)."""
+        out = np.zeros(3, dtype=np.int32)
+        self._engine._check(self._lib.gb200_tracker_chain_sizes(self._h, _ptr(out)), "gb200_tracker_chain_sizes")
+        return [int(v) for v in out]
 
     def bit_state(self, channel: int) -> dict:
         out = np.zeros(8, dtype=np.int64)
@@ -564,28 +572,16 @@ class Tracker:
         if bits_device_ptr is None:
             if counts is not None or stride is not None:
                 raise ValueError("counts / stride describe a caller's device array only")
-            n_bits = self._last_bit_stride
-            cnt_in = None
+            n_bits = self._chain_sizes()[0]
+            args = (None, None, 0)
         else:
             cnt_in = np.ascontiguousarray(counts, dtype=np.int32)
             if cnt_in.shape != (self.n_channels,) or stride is None:
                 raise ValueError("a device bit array needs one count per channel and its stride")
             n_bits = int(cnt_in.max(initial=0))
-        cap = subframe_event_capacity(n_bits)
-        ev = np.empty((self.n_channels, cap), dtype=SUBFRAME_DTYPE)
-        cnt = np.empty(self.n_channels, dtype=np.int32)
-        self._engine._check(
-            self._lib.gb200_tracker_decode_subframes(self._h, None if bits_device_ptr is None else _P(bits_device_ptr),
-                                                     None if cnt_in is None else _ptr(cnt_in), int(stride or 0), _ptr(ev),
-                                                     cap, _ptr(cnt)), "gb200_tracker_decode_subframes")
-        if (cnt > cap).any():
-            raise RuntimeError("subframe event buffer too small")  # cannot happen: see subframe_event_capacity
-        self._chain_sub = (self._chain_bits_n_ms if bits_device_ptr is None else 0, cap)
-        return [ev[c, : cnt[c]].copy() for c in range(self.n_channels)]
-
-    _chain_bits_n_ms = 0  # n_ms of the last integrate_bits call over the tracker's own records
-    _chain_sub = (0, 0)  # (n_ms, events per channel) of the last decode_subframes call on that chain
-    _orbit_n_ms = 0  # milliseconds the last parse_subframes call covered
+            args = (_P(bits_device_ptr), _ptr(cnt_in), int(stride))
+        return self._per_channel("gb200_tracker_decode_subframes", SUBFRAME_DTYPE, subframe_event_capacity(n_bits),
+                                 "subframe event", *args)  # cannot truncate: see subframe_event_capacity
 
     def parse_subframes(self, events_device_ptr: int | None = None, counts=None, stride: int | None = None,
                         event_ms=None, drop_ms=None, n_ms: int | None = None) -> list:
@@ -597,7 +593,7 @@ class Tracker:
         if events_device_ptr is None:
             if any(v is not None for v in (counts, stride, event_ms, drop_ms, n_ms)):
                 raise ValueError("counts / stride / event_ms / drop_ms / n_ms describe a caller's device array only")
-            n_ms, cap = self._chain_sub
+            cap = self._chain_sizes()[1]
             args = (None, None, 0, None, None, 0)
         else:
             cnt_in = np.ascontiguousarray(counts, dtype=np.int32)
@@ -607,17 +603,10 @@ class Tracker:
                 raise ValueError("a device event array needs one count and one drop per channel, its stride and n_ms")
             if ems.shape != (self.n_channels, int(stride)):
                 raise ValueError("event_ms must be [n_channels, stride]")
-            cap = max(1, int(cnt_in.max(initial=0)))
+            cap = int(cnt_in.max(initial=0))
             args = (_P(events_device_ptr), _ptr(cnt_in), int(stride), _ptr(ems), _ptr(drop), int(n_ms))
-        cap = max(1, int(cap))
-        out = np.empty((self.n_channels, cap), dtype=FIELDS_DTYPE)
-        cnt = np.empty(self.n_channels, dtype=np.int32)
-        self._engine._check(self._lib.gb200_tracker_parse_subframes(self._h, *args, _ptr(out), cap, _ptr(cnt)),
-                            "gb200_tracker_parse_subframes")
-        self._orbit_n_ms = int(n_ms)
-        if events_device_ptr is None:
-            self._chain_sub = (0, 0)
-        return [out[c, : cnt[c]].copy() for c in range(self.n_channels)]
+        # a channel's fields are at most its events
+        return self._per_channel("gb200_tracker_parse_subframes", FIELDS_DTYPE, max(1, cap), "field", *args)
 
     def orbit_state(self, channel: int) -> dict:
         """One channel's world-model entry: params (float64[26], OrbitalParameterType order), set_mask, prn_count,
@@ -630,7 +619,7 @@ class Tracker:
 
     def observations(self) -> np.ndarray:
         """OBSERVATION_DTYPE [n_channels, n_ms] over the milliseconds of the last parse_subframes call."""
-        out = np.empty((self.n_channels, self._orbit_n_ms), dtype=OBSERVATION_DTYPE)
+        out = np.empty((self.n_channels, self._chain_sizes()[2]), dtype=OBSERVATION_DTYPE)
         self._engine._check(self._lib.gb200_tracker_observations(self._h, _ptr(out)), "gb200_tracker_observations")
         return out
 
@@ -641,9 +630,10 @@ class Tracker:
 
     def _fix_times(self, receiver_timestamps) -> np.ndarray:
         rx = np.ascontiguousarray(receiver_timestamps, dtype=np.float64)
-        if rx.shape != (self._orbit_n_ms,):
+        n_ms = self._chain_sizes()[2]
+        if rx.shape != (n_ms,):
             raise ValueError(f"receiver_timestamps must hold one start time per millisecond of the last parse_subframes "
-                             f"call ({self._orbit_n_ms})")
+                             f"call ({n_ms})")
         return rx
 
     def position_fixes(self, receiver_timestamps) -> np.ndarray:
@@ -651,7 +641,7 @@ class Tracker:
         parse_subframes call, receiver_timestamps being the chunk start times.  The receiver's clock slide, world-model
         order and stop carry from call to call (gb200_tracker_position_fixes)."""
         rx = self._fix_times(receiver_timestamps)
-        out = np.empty(self._orbit_n_ms, dtype=FIX_DTYPE)
+        out = np.empty(rx.size, dtype=FIX_DTYPE)
         self._engine._check(self._lib.gb200_tracker_position_fixes(self._h, _ptr(rx), _ptr(out)),
                             "gb200_tracker_position_fixes")
         return out

@@ -154,12 +154,55 @@ struct gb200_engine {
     }
 };
 
+// What a tracker's device memory holds for the next stage of its call chain process -> integrate_bits ->
+// decode_subframes -> parse_subframes -> observations / position_fixes, and the one place that changes it.  A stage's
+// output is on the chain when it came, stage by stage, from the records of one whole-bank process call: its n_ms is
+// that call's milliseconds (0 = off the chain).  Each transition runs when its call has succeeded, except
+// process_begin, which runs before the tracking launch of process and process_channels.
+struct TrackerChain {
+    struct Output {
+        std::vector<int> counts;  // events per channel, `stride` apart on the device
+        int stride = 0;
+        int n_ms = 0;          // the chain it belongs to (0 = not on the chain)
+        bool pending = false;  // the next stage's chain call has not consumed it yet
+    };
+    Output records;    // the last whole-bank process call's [channel][n_ms] records (n_ms only)
+    Output bits;       // the last integrate call's bit events
+    Output subframes;  // the last decode call's subframe events
+    Output orbit;      // the change tables of the last parse call: stride and n_ms (0 = no parse call yet)
+    bool fix_pending = false;  // the last parse call's fixes are not computed yet
+    bool fix_gap = false;      // a parse call's fixes were skipped after the first fix call: for the tracker's lifetime
+
+    // the records are about to be rewritten: nothing behind them is on the chain any more; pending bits stay pending
+    void process_begin() { records.n_ms = bits.n_ms = subframes.n_ms = 0; }
+    void processed(int n_ms) { records.n_ms = n_ms; }  // whole-bank calls only
+    void integrated(const int* counts, int nc, int stride, bool own_records) {
+        bits = {{counts, counts + nc}, stride, own_records ? records.n_ms : 0, true};
+        subframes.n_ms = 0;
+    }
+    void decoded(const int* counts, int nc, int stride, bool own_bits) {
+        subframes = {{counts, counts + nc}, stride, own_bits ? bits.n_ms : 0, true};
+        if (own_bits) bits.pending = false;
+    }
+    // fixing_began: the receiver state exists (a fix call has run)
+    void parsed(int n_ms, int change_stride, bool own_subframes, bool fixing_began) {
+        if (own_subframes) subframes.pending = false;
+        orbit.n_ms = n_ms;
+        orbit.stride = change_stride;
+        if (fixing_began && fix_pending) fix_gap = true;
+        fix_pending = true;
+    }
+    void fixed() { fix_pending = false; }
+    bool subframes_on_chain() const { return subframes.n_ms && subframes.pending; }
+};
+
 struct gb200_tracker {
     gb200_engine* e = nullptr;
     int n_channels = 0;
     std::vector<char> seeded;     // pool slots that hold a channel (gb200_tracker_create seeds all)
     std::vector<char> undo_ok;    // shadow[c] holds channel c's state before its last keep_undo launch
     std::vector<int> sel_cache;   // what d_sel currently holds
+    std::vector<int> prn;         // replica row per channel, -1 for a pool slot never seeded
     DevBuf<TrackState> states, shadow;
     DevBuf<int> d_sel;
     PinnedBuf<int> h_sel;
@@ -169,47 +212,40 @@ struct gb200_tracker {
     PinnedBuf<TrackMsRecord> h_out;
     PinnedBuf<double> h_times;
     PinnedBuf<float> h_prof;
-    int last_n_ms = 0;  // records of the last gb200_tracker_process call still in d_out
-    DevBuf<BitState> bit_states;
-    DevBuf<BitEvent> d_events;
-    DevBuf<int> d_counts;
-    DevBuf<double> d_bit_times;
-    PinnedBuf<BitEvent> h_events;
-    PinnedBuf<int> h_counts;
-    PinnedBuf<double> h_bit_times;
-    // the bit events of the last gb200_tracker_integrate_bits call, still in d_events, until they are decoded
-    std::vector<int> bit_counts;
-    int bit_stride = 0;
-    bool bits_pending = false;
-    DevBuf<NavState> nav_states;
-    DevBuf<SubframeEvent> d_sub;
-    DevBuf<int> d_sub_counts, d_bit_counts;
-    PinnedBuf<SubframeEvent> h_sub;
-    PinnedBuf<int> h_sub_counts, h_bit_counts;
-    std::vector<int> prn;  // replica row per channel, -1 for a pool slot never seeded
-    // The call chain parse_subframes(NULL) reads: n_ms of the integrate call whose bit events still sit in d_events and
-    // came from the records in d_out (0 = none), and of the decode call whose events in d_sub came from those bits.
-    int chain_bits_n_ms = 0, chain_sub_n_ms = 0;
-    std::vector<int> sub_counts;  // events per channel of the last decode call, `sub_stride` apart in d_sub
-    int sub_stride = 0;
-    DevBuf<OrbitSnap> orbit_states, d_changes;
-    DevBuf<SubframeFields> d_fields;
-    DevBuf<int> d_field_counts, d_change_counts, d_event_ms, d_drop_ms, d_orbit_counts;
-    PinnedBuf<SubframeFields> h_fields;
-    PinnedBuf<int> h_field_counts, h_event_ms, h_drop_ms, h_orbit_counts;
-    int orbit_n_ms = 0;  // milliseconds the change table of the last parse call covers (0 = no call yet)
-    int change_stride = 0;
-    DevBuf<SvObservation> d_obs;
-    PinnedBuf<SvObservation> h_obs;
-    // position fixes: the receiver state (d_fix_bank, d_fix_rank) exists from the first fix call on
-    DevBuf<FixBank> d_fix_bank;
-    DevBuf<int> d_fix_rank, d_fix_order, d_fix_touch, d_fix_prev;
-    DevBuf<double> d_fix_rx, d_fix_reset, d_fix_slide1;
-    DevBuf<FixRecord> d_fixes;
-    PinnedBuf<double> h_fix_rx;
-    PinnedBuf<FixRecord> h_fixes;
-    bool fix_pending = false;  // the last parse call's fixes are not computed yet
-    bool fix_gap = false;      // a parse call's fixes were skipped after the first fix call
+    TrackerChain chain;
+    // Each later stage's per-channel state (created by its first call) and scratch.
+    struct {  // bits.cu
+        DevBuf<BitState> states;
+        DevBuf<BitEvent> d_events;
+        DevBuf<int> d_counts;
+        DevBuf<double> d_times;
+        PinnedBuf<BitEvent> h_events;
+        PinnedBuf<int> h_counts;
+        PinnedBuf<double> h_times;
+    } bits;
+    struct {  // nav.cu
+        DevBuf<NavState> states;
+        DevBuf<SubframeEvent> d_events;
+        DevBuf<int> d_counts, d_bit_counts;
+        PinnedBuf<SubframeEvent> h_events;
+        PinnedBuf<int> h_counts, h_bit_counts;
+    } nav;
+    struct {  // orbit.cu
+        DevBuf<OrbitSnap> states, d_changes;
+        DevBuf<SubframeFields> d_fields;
+        DevBuf<int> d_field_counts, d_change_counts, d_event_ms, d_drop_ms, d_counts;
+        PinnedBuf<int> h_field_counts, h_event_ms, h_drop_ms, h_counts;
+        DevBuf<SvObservation> d_obs;
+        PinnedBuf<SvObservation> h_obs;
+    } orbit;
+    struct {  // fix.cu: the receiver state is `bank` and `rank`
+        DevBuf<FixBank> bank;
+        DevBuf<int> rank, order, touch, prev;
+        DevBuf<double> rx, reset, slide1;
+        DevBuf<FixRecord> d_fixes;
+        PinnedBuf<double> h_rx;
+        PinnedBuf<FixRecord> h_fixes;
+    } fix;
 };
 // A pipelined stream of grid batches: slot k's host->device copy, compute and device->host copy run on three streams.
 struct gb200_grid_stream {
@@ -692,6 +728,51 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
 // Records to the caller (see download).
 int fetch_records(gb200_engine* e, size_t n, gb200_cell_record* out_host) {
     return download(e, reinterpret_cast<CellRecord*>(out_host), e->d_records.p, n, e->h_records);
+}
+
+// ---- the tracker's call chain (gb200_tracker_integrate_bits .. gb200_tracker_receiver_state) ----
+
+// A chain stage's per-channel device state, created by the stage's first call from init on zeroed host objects.
+template <class T, class Init>
+int ensure_state(gb200_engine* e, DevBuf<T>& state, int n, Init init) {
+    if (state.p) return GB200_OK;
+    std::vector<T> host(n);
+    for (T& s : host) {
+        memset(&s, 0, sizeof(T));
+        init(s);
+    }
+    GB_CUDA(e, state.ensure(n));
+    GB_CUDA(e, cudaMemcpy(state.p, host.data(), sizeof(T) * n, cudaMemcpyHostToDevice));
+    return GB200_OK;
+}
+
+// A getter's copy of `bytes` of a stage's device state from state.p[i] on, once the work in flight is done.  Before the
+// stage's first call the state does not exist and dst keeps the host default.
+template <class T>
+int read_state(gb200_engine* e, void* dst, const DevBuf<T>& state, int i = 0, size_t bytes = sizeof(T)) {
+    if (!state.p) return GB200_OK;
+    GB_CUDA(e, cudaSetDevice(e->device));
+    GB_CUDA(e, cudaStreamSynchronize(e->stream));
+    GB_CUDA(e, cudaMemcpy(dst, state.p + i, bytes, cudaMemcpyDeviceToHost));
+    return GB200_OK;
+}
+static_assert(offsetof(BitState, h) == 0 && offsetof(NavState, h) == 0, "the getters read a state's head at its start");
+
+// Channel c's `count` events fit the `stride` they sit apart at; fmt formats (c, count, stride).
+int check_fits(gb200_engine* e, const char* fmt, int c, int count, int stride) {
+    if (count < 0 || count > stride) GB_FAIL(e, GB200_EINVAL, fmt, c, count, stride);
+    return GB200_OK;
+}
+
+// A stage's per-channel output to the caller: the counts' copy is enqueued first, so that copy_events, which waits for
+// the stream, waits for both; then the counts go to counts_out.  h_counts keeps them for the chain's record.
+template <class CopyEvents>
+int fetch_output(gb200_engine* e, int nc, const DevBuf<int>& d_counts, PinnedBuf<int>& h_counts, int32_t* counts_out,
+                 CopyEvents copy_events) {
+    GB_CUDA(e, cudaMemcpyAsync(h_counts.p, d_counts.p, nc * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+    GB_TRY(copy_events());
+    memcpy(counts_out, h_counts.p, nc * sizeof(int));
+    return GB200_OK;
 }
 
 }  // namespace
@@ -1350,10 +1431,9 @@ static int tracker_process_host(gb200_tracker* t, int n_sel, const int32_t* sel,
         GB_CUDA(e, t->d_prof.ensure(np));
         GB_CUDA(e, t->h_prof.ensure(np));
     }
-    t->last_n_ms = 0;
-    t->chain_bits_n_ms = t->chain_sub_n_ms = 0;  // d_out is about to be rewritten
+    t->chain.process_begin();  // d_out is about to be rewritten
     GB_TRY(tracker_launch(t, n_sel, sel, n_ms, start_times, t->d_out.p, np ? t->d_prof.p : nullptr, keep_undo));
-    if (!sel) t->last_n_ms = n_ms;  // gb200_tracker_integrate_bits reads [channel][n_ms] of the whole bank
+    if (!sel) t->chain.processed(n_ms);  // gb200_tracker_integrate_bits reads [channel][n_ms] of the whole bank
     // the profiles' copy is enqueued first, so the records' download waits for both
     if (np) GB_CUDA(e, cudaMemcpyAsync(t->h_prof.p, t->d_prof.p, np * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
     GB_TRY(download(e, reinterpret_cast<TrackMsRecord*>(out_host), t->d_out.p, n, t->h_out));
@@ -1469,75 +1549,53 @@ int gb200_tracker_integrate_bits(gb200_tracker* t, int n_ms, const double* start
                                  int32_t* counts_host) {
     if (!t) return GB200_EINVAL;
     gb200_engine* e = t->e;
+    auto& s = t->bits;
+    const int nc = t->n_channels, chain_ms = t->chain.records.n_ms;
     if (n_ms < 1 || !start_times || !end_times) GB_FAIL(e, GB200_EINVAL, "need at least one millisecond and its timestamps");
     if (!events_host || !counts_host || max_events < 1) GB_FAIL(e, GB200_EINVAL, "null / empty event buffer");
-    if (!records_device && t->last_n_ms != n_ms)
-        GB_FAIL(e, GB200_ESTATE, "no records of %d ms on the device (last gb200_tracker_process call held %d)", n_ms, t->last_n_ms);
+    if (!records_device && chain_ms != n_ms)
+        GB_FAIL(e, GB200_ESTATE, "no records of %d ms on the device (last gb200_tracker_process call held %d)", n_ms, chain_ms);
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_CUDA(e, cudaStreamSynchronize(e->stream));  // pinned staging may still be in flight
-    const int nc = t->n_channels;
-    if (!t->bit_states.p) {
-        std::vector<BitState> init(nc);
-        for (int c = 0; c < nc; ++c) {
-            memset(&init[c], 0, sizeof(BitState));
-            bit_state_init(init[c]);
-        }
-        GB_CUDA(e, t->bit_states.ensure(nc));
-        GB_CUDA(e, cudaMemcpy(t->bit_states.p, init.data(), sizeof(BitState) * nc, cudaMemcpyHostToDevice));
-    }
+    GB_TRY(ensure_state(e, s.states, nc, [](BitState& b) { bit_state_init(b); }));
     const size_t ne = static_cast<size_t>(nc) * max_events;
-    GB_CUDA(e, t->d_events.ensure(ne));
-    GB_CUDA(e, t->d_counts.ensure(nc));
-    GB_CUDA(e, t->h_counts.ensure(nc));
-    GB_CUDA(e, t->d_bit_times.ensure(2 * static_cast<size_t>(n_ms)));
-    GB_CUDA(e, t->h_bit_times.ensure(2 * static_cast<size_t>(n_ms)));
-    memcpy(t->h_bit_times.p, start_times, sizeof(double) * n_ms);
-    memcpy(t->h_bit_times.p + n_ms, end_times, sizeof(double) * n_ms);
-    GB_CUDA(e, cudaMemcpyAsync(t->d_bit_times.p, t->h_bit_times.p, 2 * sizeof(double) * n_ms, cudaMemcpyHostToDevice, e->stream));
+    GB_CUDA(e, s.d_events.ensure(ne));
+    GB_CUDA(e, s.d_counts.ensure(nc));
+    GB_CUDA(e, s.h_counts.ensure(nc));
+    GB_CUDA(e, s.d_times.ensure(2 * static_cast<size_t>(n_ms)));
+    GB_CUDA(e, s.h_times.ensure(2 * static_cast<size_t>(n_ms)));
+    memcpy(s.h_times.p, start_times, sizeof(double) * n_ms);
+    memcpy(s.h_times.p + n_ms, end_times, sizeof(double) * n_ms);
+    GB_CUDA(e, cudaMemcpyAsync(s.d_times.p, s.h_times.p, 2 * sizeof(double) * n_ms, cudaMemcpyHostToDevice, e->stream));
     BitArgs a{};
     a.records = records_device ? static_cast<const TrackMsRecord*>(records_device) : t->d_out.p;
-    a.start_times = t->d_bit_times.p;
-    a.end_times = t->d_bit_times.p + n_ms;
-    a.states = t->bit_states.p;
-    a.events = t->d_events.p;
-    a.counts = t->d_counts.p;
+    a.start_times = s.d_times.p;
+    a.end_times = s.d_times.p + n_ms;
+    a.states = s.states.p;
+    a.events = s.d_events.p;
+    a.counts = s.d_counts.p;
     a.n_ms = n_ms;
     a.n_channels = nc;
     a.max_events = max_events;
     GB_LAUNCH(e, -1, launch_integrate_bits(a, e->stream));
-    // the counts' copy is enqueued first, so the events' download waits for both
-    GB_CUDA(e, cudaMemcpyAsync(t->h_counts.p, t->d_counts.p, nc * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-    GB_TRY(download(e, reinterpret_cast<BitEvent*>(events_host), t->d_events.p, ne, t->h_events));
-    memcpy(counts_host, t->h_counts.p, nc * sizeof(int));
-    t->bit_counts.assign(t->h_counts.p, t->h_counts.p + nc);
-    t->bit_stride = max_events;
-    t->bits_pending = true;
-    t->chain_bits_n_ms = records_device ? 0 : n_ms;
-    t->chain_sub_n_ms = 0;
+    GB_TRY(fetch_output(e, nc, s.d_counts, s.h_counts, counts_host, [&]() -> int {
+        return download(e, reinterpret_cast<BitEvent*>(events_host), s.d_events.p, ne, s.h_events);
+    }));
+    t->chain.integrated(s.h_counts.p, nc, max_events, !records_device);
     return GB200_OK;
 }
 
 int gb200_tracker_bit_state(gb200_tracker* t, int channel, int64_t out[8]) {
     if (!t) return GB200_EINVAL;
-    gb200_engine* e = t->e;
     GB_TRY(check_channel(t, channel));
-    if (!out) GB_FAIL(e, GB200_EINVAL, "channel %d out of range", channel);
+    if (!out) GB_FAIL(t->e, GB200_EINVAL, "null output");
     BitState st;
     memset(&st, 0, sizeof(st));
     bit_state_init(st);
-    if (t->bit_states.p) {
-        GB_CUDA(e, cudaSetDevice(e->device));
-        GB_CUDA(e, cudaStreamSynchronize(e->stream));
-        GB_CUDA(e, cudaMemcpy(&st, t->bit_states.p + channel, sizeof(BitHead), cudaMemcpyDeviceToHost));
-    }
-    out[0] = st.h.emitted;
-    out[1] = st.h.failed;
-    out[2] = st.h.processed;
-    out[3] = st.h.slide;
-    out[4] = st.h.determined;
-    out[5] = st.h.prev_decision;
-    out[6] = st.h.cursor;
-    out[7] = st.h.stopped;
+    GB_TRY(read_state(t->e, &st, t->bits.states, channel, sizeof(BitHead)));
+    const BitHead& h = st.h;
+    const int64_t v[8] = {h.emitted, h.failed, h.processed, h.slide, h.determined, h.prev_decision, h.cursor, h.stopped};
+    memcpy(out, v, sizeof(v));
     return GB200_OK;
 }
 
@@ -1546,83 +1604,59 @@ int gb200_tracker_decode_subframes(gb200_tracker* t, const void* bits_device, co
                                    int32_t* counts_host) {
     if (!t) return GB200_EINVAL;
     gb200_engine* e = t->e;
+    auto& s = t->nav;
+    const TrackerChain::Output& bits = t->chain.bits;
     const int nc = t->n_channels;
     if (!events_host || !counts_host || max_events < 1) GB_FAIL(e, GB200_EINVAL, "null / empty event buffer");
-    const int* counts = nullptr;
-    int stride = 0;
+    const int* counts = bit_counts_host;
+    int stride = bits_stride;
     if (bits_device) {
         if (!bit_counts_host || bits_stride < 1) GB_FAIL(e, GB200_EINVAL, "bit events need their counts and a stride >= 1");
         for (int c = 0; c < nc; ++c)
-            if (bit_counts_host[c] < 0 || bit_counts_host[c] > bits_stride)
-                GB_FAIL(e, GB200_EINVAL, "channel %d: %d bit events do not fit a stride of %d", c, bit_counts_host[c], bits_stride);
-        counts = bit_counts_host;
-        stride = bits_stride;
+            GB_TRY(check_fits(e, "channel %d: %d bit events do not fit a stride of %d", c, counts[c], stride));
     } else {
-        if (!t->bits_pending) GB_FAIL(e, GB200_ESTATE, "no undecoded bit events on the device (call gb200_tracker_integrate_bits first)");
+        if (!bits.pending) GB_FAIL(e, GB200_ESTATE, "no undecoded bit events on the device (call gb200_tracker_integrate_bits first)");
+        counts = bits.counts.data();
+        stride = bits.stride;
         for (int c = 0; c < nc; ++c)
-            if (t->bit_counts[c] > t->bit_stride)
-                GB_FAIL(e, GB200_EINVAL, "channel %d: the last integrate call produced %d bit events but kept %d", c,
-                        t->bit_counts[c], t->bit_stride);
-        counts = t->bit_counts.data();
-        stride = t->bit_stride;
+            GB_TRY(check_fits(e, "channel %d: the last integrate call produced %d bit events but kept %d", c, counts[c], stride));
     }
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_CUDA(e, cudaStreamSynchronize(e->stream));  // pinned staging may still be in flight
-    if (!t->nav_states.p) {
-        std::vector<NavState> init(nc);
-        for (int c = 0; c < nc; ++c) {
-            memset(&init[c], 0, sizeof(NavState));
-            nav_state_init(init[c].h);
-        }
-        GB_CUDA(e, t->nav_states.ensure(nc));
-        GB_CUDA(e, cudaMemcpy(t->nav_states.p, init.data(), sizeof(NavState) * nc, cudaMemcpyHostToDevice));
-    }
+    GB_TRY(ensure_state(e, s.states, nc, [](NavState& n) { nav_state_init(n.h); }));
     const size_t ne = static_cast<size_t>(nc) * max_events;
-    GB_CUDA(e, t->d_sub.ensure(ne));
-    GB_CUDA(e, t->d_sub_counts.ensure(nc));
-    GB_CUDA(e, t->h_sub_counts.ensure(nc));
-    GB_CUDA(e, t->d_bit_counts.ensure(nc));
-    GB_TRY(upload(e, t->d_bit_counts.p, counts, nc, t->h_bit_counts));
+    GB_CUDA(e, s.d_events.ensure(ne));
+    GB_CUDA(e, s.d_counts.ensure(nc));
+    GB_CUDA(e, s.h_counts.ensure(nc));
+    GB_CUDA(e, s.d_bit_counts.ensure(nc));
+    GB_TRY(upload(e, s.d_bit_counts.p, counts, nc, s.h_bit_counts));
     NavArgs a{};
-    a.bits = bits_device ? static_cast<const BitEvent*>(bits_device) : t->d_events.p;
-    a.counts = t->d_bit_counts.p;
-    a.bit_states = bits_device ? nullptr : t->bit_states.p;
-    a.states = t->nav_states.p;
-    a.events = t->d_sub.p;
-    a.event_counts = t->d_sub_counts.p;
+    a.bits = bits_device ? static_cast<const BitEvent*>(bits_device) : t->bits.d_events.p;
+    a.counts = s.d_bit_counts.p;
+    a.bit_states = bits_device ? nullptr : t->bits.states.p;
+    a.states = s.states.p;
+    a.events = s.d_events.p;
+    a.event_counts = s.d_counts.p;
     a.stride = stride;
     a.n_channels = nc;
     a.max_events = max_events;
     GB_LAUNCH(e, -1, launch_decode_subframes(a, e->stream));
-    t->chain_sub_n_ms = bits_device ? 0 : t->chain_bits_n_ms;
-    if (!bits_device) t->bits_pending = false;
-    // the counts' copy is enqueued first, so the events' download waits for both
-    GB_CUDA(e, cudaMemcpyAsync(t->h_sub_counts.p, t->d_sub_counts.p, nc * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-    GB_TRY(download(e, reinterpret_cast<SubframeEvent*>(events_host), t->d_sub.p, ne, t->h_sub));
-    memcpy(counts_host, t->h_sub_counts.p, nc * sizeof(int));
-    t->sub_counts.assign(t->h_sub_counts.p, t->h_sub_counts.p + nc);
-    t->sub_stride = max_events;
+    GB_TRY(fetch_output(e, nc, s.d_counts, s.h_counts, counts_host, [&]() -> int {
+        return download(e, reinterpret_cast<SubframeEvent*>(events_host), s.d_events.p, ne, s.h_events);
+    }));
+    t->chain.decoded(s.h_counts.p, nc, max_events, !bits_device);
     return GB200_OK;
 }
 
 int gb200_tracker_subframe_state(gb200_tracker* t, int channel, int64_t out[6]) {
     if (!t) return GB200_EINVAL;
-    gb200_engine* e = t->e;
     GB_TRY(check_channel(t, channel));
-    if (!out) GB_FAIL(e, GB200_EINVAL, "null output");
+    if (!out) GB_FAIL(t->e, GB200_EINVAL, "null output");
     NavHead h;
     nav_state_init(h);
-    if (t->nav_states.p) {
-        GB_CUDA(e, cudaSetDevice(e->device));
-        GB_CUDA(e, cudaStreamSynchronize(e->stream));
-        GB_CUDA(e, cudaMemcpy(&h, &t->nav_states.p[channel].h, sizeof(NavHead), cudaMemcpyDeviceToHost));
-    }
-    out[0] = h.phase;
-    out[1] = h.emitted;
-    out[2] = h.polarity;
-    out[3] = h.qlen;
-    out[4] = h.stopped;
-    out[5] = h.bits;
+    GB_TRY(read_state(t->e, &h, t->nav.states, channel, sizeof(NavHead)));
+    const int64_t v[6] = {h.phase, h.emitted, h.polarity, h.qlen, h.stopped, h.bits};
+    memcpy(out, v, sizeof(v));
     return GB200_OK;
 }
 
@@ -1631,6 +1665,8 @@ int gb200_tracker_parse_subframes(gb200_tracker* t, const void* events_device, c
                                   gb200_subframe_fields* fields_host, int32_t max_fields, int32_t* field_counts_host) {
     if (!t) return GB200_EINVAL;
     gb200_engine* e = t->e;
+    auto& s = t->orbit;
+    const TrackerChain::Output& sub = t->chain.subframes;
     const int nc = t->n_channels;
     if (!fields_host || !field_counts_host || max_fields < 1) GB_FAIL(e, GB200_EINVAL, "null / empty field buffer");
     for (int c = 0; c < nc; ++c)
@@ -1638,104 +1674,86 @@ int gb200_tracker_parse_subframes(gb200_tracker* t, const void* events_device, c
             if (t->prn[c] >= 0 && t->prn[c] == t->prn[d])
                 GB_FAIL(e, GB200_EINVAL, "channels %d and %d track the same replica row %d (the world model is keyed by satellite)",
                         d, c, t->prn[c]);
-    const int* counts = nullptr;
+    const int* counts = counts_host;
     if (events_device) {
         if (!counts_host || !event_ms_host || !drop_ms_host || stride < 1 || n_ms < 1)
             GB_FAIL(e, GB200_EINVAL, "subframe events need their counts, milliseconds, drops, a stride >= 1 and n_ms >= 1");
         for (int c = 0; c < nc; ++c) {
-            if (counts_host[c] < 0 || counts_host[c] > stride)
-                GB_FAIL(e, GB200_EINVAL, "channel %d: %d events do not fit a stride of %d", c, counts_host[c], stride);
+            GB_TRY(check_fits(e, "channel %d: %d events do not fit a stride of %d", c, counts[c], stride));
             if (drop_ms_host[c] < -1 || drop_ms_host[c] >= n_ms)
                 GB_FAIL(e, GB200_EINVAL, "channel %d: drop millisecond %d outside [-1, %d)", c, drop_ms_host[c], n_ms);
-            for (int j = 0; j < counts_host[c]; ++j) {
+            for (int j = 0; j < counts[c]; ++j) {
                 const int m = event_ms_host[static_cast<size_t>(c) * stride + j];
                 const int prev = j ? event_ms_host[static_cast<size_t>(c) * stride + j - 1] : 0;
                 if (m < prev || m >= n_ms)
                     GB_FAIL(e, GB200_EINVAL, "channel %d: event %d's millisecond %d is out of order or outside [0, %d)", c, j, m, n_ms);
             }
         }
-        counts = counts_host;
     } else {
-        if (!t->chain_sub_n_ms)
+        if (!t->chain.subframes_on_chain())
             GB_FAIL(e, GB200_ESTATE, "no unparsed subframe events of a process -> integrate_bits -> decode_subframes chain on the device");
+        counts = sub.counts.data();
+        stride = sub.stride;
+        n_ms = sub.n_ms;
         for (int c = 0; c < nc; ++c)
-            if (t->sub_counts[c] > t->sub_stride)
-                GB_FAIL(e, GB200_EINVAL, "channel %d: the last decode call produced %d events but kept %d", c, t->sub_counts[c],
-                        t->sub_stride);
-        counts = t->sub_counts.data();
-        stride = t->sub_stride;
-        n_ms = t->chain_sub_n_ms;
+            GB_TRY(check_fits(e, "channel %d: the last decode call produced %d events but kept %d", c, counts[c], stride));
     }
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_CUDA(e, cudaStreamSynchronize(e->stream));  // pinned staging may still be in flight
-    if (!t->orbit_states.p) {
-        std::vector<OrbitSnap> init(nc);
-        for (int c = 0; c < nc; ++c) orbit_state_init(init[c]);
-        GB_CUDA(e, t->orbit_states.ensure(nc));
-        GB_CUDA(e, cudaMemcpy(t->orbit_states.p, init.data(), sizeof(OrbitSnap) * nc, cudaMemcpyHostToDevice));
-    }
+    GB_TRY(ensure_state(e, s.states, nc, [](OrbitSnap& o) { orbit_state_init(o); }));
     const size_t nf = static_cast<size_t>(nc) * stride;
-    GB_CUDA(e, t->d_fields.ensure(nf));
-    GB_CUDA(e, t->d_changes.ensure(static_cast<size_t>(nc) * (stride + 2)));
-    GB_CUDA(e, t->d_field_counts.ensure(nc));
-    GB_CUDA(e, t->d_change_counts.ensure(nc));
-    GB_CUDA(e, t->h_field_counts.ensure(nc));
-    GB_CUDA(e, t->d_orbit_counts.ensure(nc));
-    GB_TRY(upload(e, t->d_orbit_counts.p, counts, nc, t->h_orbit_counts));
+    GB_CUDA(e, s.d_fields.ensure(nf));
+    GB_CUDA(e, s.d_changes.ensure(static_cast<size_t>(nc) * (stride + 2)));
+    GB_CUDA(e, s.d_field_counts.ensure(nc));
+    GB_CUDA(e, s.d_change_counts.ensure(nc));
+    GB_CUDA(e, s.h_field_counts.ensure(nc));
+    GB_CUDA(e, s.d_counts.ensure(nc));
+    GB_TRY(upload(e, s.d_counts.p, counts, nc, s.h_counts));
     OrbitArgs a{};
     if (events_device) {
-        GB_CUDA(e, t->d_event_ms.ensure(nf));
-        GB_CUDA(e, t->d_drop_ms.ensure(nc));
-        GB_TRY(upload(e, t->d_event_ms.p, event_ms_host, nf, t->h_event_ms));
-        GB_TRY(upload(e, t->d_drop_ms.p, drop_ms_host, nc, t->h_drop_ms));
+        GB_CUDA(e, s.d_event_ms.ensure(nf));
+        GB_CUDA(e, s.d_drop_ms.ensure(nc));
+        GB_TRY(upload(e, s.d_event_ms.p, event_ms_host, nf, s.h_event_ms));
+        GB_TRY(upload(e, s.d_drop_ms.p, drop_ms_host, nc, s.h_drop_ms));
         a.events = static_cast<const SubframeEvent*>(events_device);
-        a.event_ms = t->d_event_ms.p;
-        a.drop_ms = t->d_drop_ms.p;
+        a.event_ms = s.d_event_ms.p;
+        a.drop_ms = s.d_drop_ms.p;
     } else {
-        a.events = t->d_sub.p;
-        a.bits = t->d_events.p;
-        a.bit_stride = t->bit_stride;
+        a.events = t->nav.d_events.p;
+        a.bits = t->bits.d_events.p;
+        a.bit_stride = t->chain.bits.stride;
         a.records = t->d_out.p;
     }
-    a.counts = t->d_orbit_counts.p;
-    a.states = t->orbit_states.p;
-    a.fields = t->d_fields.p;
-    a.field_counts = t->d_field_counts.p;
-    a.changes = t->d_changes.p;
-    a.change_counts = t->d_change_counts.p;
+    a.counts = s.d_counts.p;
+    a.states = s.states.p;
+    a.fields = s.d_fields.p;
+    a.field_counts = s.d_field_counts.p;
+    a.changes = s.d_changes.p;
+    a.change_counts = s.d_change_counts.p;
     a.stride = stride;
     a.n_ms = n_ms;
     a.n_channels = nc;
     GB_LAUNCH(e, -1, launch_parse_subframes(a, e->stream));
-    if (!events_device) t->chain_sub_n_ms = 0;
-    t->orbit_n_ms = n_ms;
-    t->change_stride = stride + 2;
-    if (t->d_fix_bank.p && t->fix_pending) t->fix_gap = true;
-    t->fix_pending = true;
-    // the counts' copy is enqueued first, so the fields' download waits for both
-    GB_CUDA(e, cudaMemcpyAsync(t->h_field_counts.p, t->d_field_counts.p, nc * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));
     // the fields are [channel][stride] on the device and [channel][max_fields] for the caller
     const int keep = std::min<int>(stride, max_fields);
-    GB_CUDA(e, cudaMemcpy2DAsync(fields_host, sizeof(SubframeFields) * max_fields, t->d_fields.p, sizeof(SubframeFields) * stride,
-                                 sizeof(SubframeFields) * keep, nc, cudaMemcpyDeviceToHost, e->stream));
-    GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    memcpy(field_counts_host, t->h_field_counts.p, nc * sizeof(int));
+    GB_TRY(fetch_output(e, nc, s.d_field_counts, s.h_field_counts, field_counts_host, [&]() -> int {
+        GB_CUDA(e, cudaStreamSynchronize(e->stream));
+        GB_CUDA(e, cudaMemcpy2DAsync(fields_host, sizeof(SubframeFields) * max_fields, s.d_fields.p, sizeof(SubframeFields) * stride,
+                                     sizeof(SubframeFields) * keep, nc, cudaMemcpyDeviceToHost, e->stream));
+        GB_CUDA(e, cudaStreamSynchronize(e->stream));
+        return GB200_OK;
+    }));
+    t->chain.parsed(n_ms, stride + 2, !events_device, t->fix.bank.p != nullptr);
     return GB200_OK;
 }
 
 int gb200_tracker_orbit_state(gb200_tracker* t, int channel, double params[26], uint32_t* set_mask, int64_t* prn_count,
                               int32_t* counting) {
     if (!t) return GB200_EINVAL;
-    gb200_engine* e = t->e;
     GB_TRY(check_channel(t, channel));
     OrbitSnap s;
     orbit_state_init(s);
-    if (t->orbit_states.p) {
-        GB_CUDA(e, cudaSetDevice(e->device));
-        GB_CUDA(e, cudaStreamSynchronize(e->stream));
-        GB_CUDA(e, cudaMemcpy(&s, t->orbit_states.p + channel, sizeof(OrbitSnap), cudaMemcpyDeviceToHost));
-    }
+    GB_TRY(read_state(t->e, &s, t->orbit.states, channel));
     if (params) memcpy(params, s.p, sizeof(s.p));
     if (set_mask) *set_mask = s.set;
     if (prn_count) *prn_count = s.count;
@@ -1743,11 +1761,21 @@ int gb200_tracker_orbit_state(gb200_tracker* t, int channel, double params[26], 
     return GB200_OK;
 }
 
+int gb200_tracker_chain_sizes(const gb200_tracker* t, int32_t out[3]) {
+    if (!t) return GB200_EINVAL;
+    if (!out) GB_FAIL(t->e, GB200_EINVAL, "null output");
+    out[0] = t->chain.bits.stride;
+    out[1] = t->chain.subframes.stride;
+    out[2] = t->chain.orbit.n_ms;
+    return GB200_OK;
+}
+
 static int observations_launch(gb200_tracker* t, SvObservation* out_dev) {
     gb200_engine* e = t->e;
-    if (!t->orbit_n_ms) GB_FAIL(e, GB200_ESTATE, "no gb200_tracker_parse_subframes call yet");
-    GB_LAUNCH(e, -1, launch_sv_observations(t->d_changes.p, t->d_change_counts.p, t->change_stride, t->n_channels, t->orbit_n_ms,
-                                            out_dev, e->stream));
+    const TrackerChain::Output& orbit = t->chain.orbit;
+    if (!orbit.n_ms) GB_FAIL(e, GB200_ESTATE, "no gb200_tracker_parse_subframes call yet");
+    GB_LAUNCH(e, -1, launch_sv_observations(t->orbit.d_changes.p, t->orbit.d_change_counts.p, orbit.stride, t->n_channels,
+                                            orbit.n_ms, out_dev, e->stream));
     return GB200_OK;
 }
 
@@ -1761,61 +1789,56 @@ int gb200_tracker_observations_device(gb200_tracker* t, void* out_device) {
 int gb200_tracker_observations(gb200_tracker* t, gb200_sv_observation* out_host) {
     if (!t) return GB200_EINVAL;
     gb200_engine* e = t->e;
+    auto& s = t->orbit;
     if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
     GB_CUDA(e, cudaSetDevice(e->device));
-    const size_t n = static_cast<size_t>(t->n_channels) * t->orbit_n_ms;
-    if (n) GB_CUDA(e, t->d_obs.ensure(n));
-    GB_TRY(observations_launch(t, t->d_obs.p));
-    return download(e, reinterpret_cast<SvObservation*>(out_host), t->d_obs.p, n, t->h_obs);
+    const size_t n = static_cast<size_t>(t->n_channels) * t->chain.orbit.n_ms;
+    if (n) GB_CUDA(e, s.d_obs.ensure(n));
+    GB_TRY(observations_launch(t, s.d_obs.p));
+    return download(e, reinterpret_cast<SvObservation*>(out_host), s.d_obs.p, n, s.h_obs);
 }
 
 // The observations of the last parse call and the fixes over them (fix.cu), enqueued into out_dev.
 static int fixes_launch(gb200_tracker* t, const double* rx_host, FixRecord* out_dev) {
     gb200_engine* e = t->e;
+    auto& s = t->fix;
     if (!rx_host) GB_FAIL(e, GB200_EINVAL, "null receiver timestamps");
-    if (!t->orbit_n_ms) GB_FAIL(e, GB200_ESTATE, "no gb200_tracker_parse_subframes call yet");
-    if (t->fix_gap)
+    if (!t->chain.orbit.n_ms) GB_FAIL(e, GB200_ESTATE, "no gb200_tracker_parse_subframes call yet");
+    if (t->chain.fix_gap)
         GB_FAIL(e, GB200_ESTATE, "the fixes of an earlier parse call were skipped: the receiver's clock slide chain has a gap");
-    if (!t->fix_pending) GB_FAIL(e, GB200_ESTATE, "the fixes of the last parse call were already computed");
-    const int nc = t->n_channels, n_ms = t->orbit_n_ms;
+    if (!t->chain.fix_pending) GB_FAIL(e, GB200_ESTATE, "the fixes of the last parse call were already computed");
+    const int nc = t->n_channels, n_ms = t->chain.orbit.n_ms;
     GB_CUDA(e, cudaStreamSynchronize(e->stream));  // pinned staging may still be in flight
-    if (!t->d_fix_bank.p) {
-        FixBank b{};
-        b.slide = NAN;
-        const std::vector<int> rank(nc, -1);
-        GB_CUDA(e, t->d_fix_bank.ensure(1));
-        GB_CUDA(e, t->d_fix_rank.ensure(nc));
-        GB_CUDA(e, cudaMemcpy(t->d_fix_bank.p, &b, sizeof(b), cudaMemcpyHostToDevice));
-        GB_CUDA(e, cudaMemcpy(t->d_fix_rank.p, rank.data(), sizeof(int) * nc, cudaMemcpyHostToDevice));
-    }
-    GB_CUDA(e, t->d_obs.ensure(static_cast<size_t>(nc) * n_ms));
-    GB_CUDA(e, t->d_fix_order.ensure(nc));
-    GB_CUDA(e, t->d_fix_touch.ensure(nc));
-    GB_CUDA(e, t->d_fix_prev.ensure(n_ms));
-    GB_CUDA(e, t->d_fix_rx.ensure(n_ms));
-    GB_CUDA(e, t->d_fix_reset.ensure(n_ms));
-    GB_CUDA(e, t->d_fix_slide1.ensure(n_ms));
-    GB_TRY(upload(e, t->d_fix_rx.p, rx_host, n_ms, t->h_fix_rx));
-    GB_TRY(observations_launch(t, t->d_obs.p));
+    GB_TRY(ensure_state(e, s.bank, 1, [](FixBank& b) { b.slide = NAN; }));
+    GB_TRY(ensure_state(e, s.rank, nc, [](int& r) { r = -1; }));
+    GB_CUDA(e, t->orbit.d_obs.ensure(static_cast<size_t>(nc) * n_ms));
+    GB_CUDA(e, s.order.ensure(nc));
+    GB_CUDA(e, s.touch.ensure(nc));
+    GB_CUDA(e, s.prev.ensure(n_ms));
+    GB_CUDA(e, s.rx.ensure(n_ms));
+    GB_CUDA(e, s.reset.ensure(n_ms));
+    GB_CUDA(e, s.slide1.ensure(n_ms));
+    GB_TRY(upload(e, s.rx.p, rx_host, n_ms, s.h_rx));
+    GB_TRY(observations_launch(t, t->orbit.d_obs.p));
     FixArgs a{};
-    a.changes = t->d_changes.p;
-    a.change_counts = t->d_change_counts.p;
-    a.change_stride = t->change_stride;
-    a.obs = t->d_obs.p;
-    a.rx = t->d_fix_rx.p;
-    a.bank = t->d_fix_bank.p;
-    a.rank = t->d_fix_rank.p;
-    a.order = t->d_fix_order.p;
-    a.touch_ms = t->d_fix_touch.p;
-    a.reset = t->d_fix_reset.p;
-    a.prev = t->d_fix_prev.p;
-    a.slide1 = t->d_fix_slide1.p;
+    a.changes = t->orbit.d_changes.p;
+    a.change_counts = t->orbit.d_change_counts.p;
+    a.change_stride = t->chain.orbit.stride;
+    a.obs = t->orbit.d_obs.p;
+    a.rx = s.rx.p;
+    a.bank = s.bank.p;
+    a.rank = s.rank.p;
+    a.order = s.order.p;
+    a.touch_ms = s.touch.p;
+    a.reset = s.reset.p;
+    a.prev = s.prev.p;
+    a.slide1 = s.slide1.p;
     a.out = out_dev;
     a.n_channels = nc;
     a.n_ms = n_ms;
     GB_LAUNCH(e, -1, launch_position_fixes(a, e->stream));
     e->launches += 4;  // plan, two passes, repair and finish
-    t->fix_pending = false;
+    t->chain.fixed();
     return GB200_OK;
 }
 
@@ -1829,24 +1852,20 @@ int gb200_tracker_position_fixes_device(gb200_tracker* t, const double* receiver
 int gb200_tracker_position_fixes(gb200_tracker* t, const double* receiver_timestamps_host, gb200_position_fix* out_host) {
     if (!t) return GB200_EINVAL;
     gb200_engine* e = t->e;
+    auto& s = t->fix;
     if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
     GB_CUDA(e, cudaSetDevice(e->device));
-    const size_t n = static_cast<size_t>(t->orbit_n_ms);
-    if (n) GB_CUDA(e, t->d_fixes.ensure(n));
-    GB_TRY(fixes_launch(t, receiver_timestamps_host, t->d_fixes.p));
-    return download(e, reinterpret_cast<FixRecord*>(out_host), t->d_fixes.p, n, t->h_fixes);
+    const size_t n = static_cast<size_t>(t->chain.orbit.n_ms);
+    if (n) GB_CUDA(e, s.d_fixes.ensure(n));
+    GB_TRY(fixes_launch(t, receiver_timestamps_host, s.d_fixes.p));
+    return download(e, reinterpret_cast<FixRecord*>(out_host), s.d_fixes.p, n, s.h_fixes);
 }
 
 int gb200_tracker_fix_repairs(gb200_tracker* t, int64_t* n) {
     if (!t) return GB200_EINVAL;
-    gb200_engine* e = t->e;
-    if (!n) GB_FAIL(e, GB200_EINVAL, "null output");
+    if (!n) GB_FAIL(t->e, GB200_EINVAL, "null output");
     FixBank b{};
-    if (t->d_fix_bank.p) {
-        GB_CUDA(e, cudaSetDevice(e->device));
-        GB_CUDA(e, cudaStreamSynchronize(e->stream));
-        GB_CUDA(e, cudaMemcpy(&b, t->d_fix_bank.p, sizeof(b), cudaMemcpyDeviceToHost));
-    }
+    GB_TRY(read_state(t->e, &b, t->fix.bank));
     *n = b.n_repaired;
     return GB200_OK;
 }
@@ -1858,12 +1877,9 @@ int gb200_tracker_receiver_state(gb200_tracker* t, double* slide, int32_t* stopp
     FixBank b{};
     b.slide = NAN;
     std::vector<int> rank(nc, -1);
-    if (t->d_fix_bank.p) {
-        GB_CUDA(e, cudaSetDevice(e->device));
-        GB_CUDA(e, cudaStreamSynchronize(e->stream));
-        GB_CUDA(e, cudaMemcpy(&b, t->d_fix_bank.p, sizeof(b), cudaMemcpyDeviceToHost));
-        GB_CUDA(e, cudaMemcpy(rank.data(), t->d_fix_rank.p, sizeof(int) * nc, cudaMemcpyDeviceToHost));
-    }
+    GB_TRY(read_state(e, &b, t->fix.bank));
+    // the rank is made after the bank, so read_state has waited for the stream if it exists
+    if (t->fix.rank.p) GB_CUDA(e, cudaMemcpy(rank.data(), t->fix.rank.p, sizeof(int) * nc, cudaMemcpyDeviceToHost));
     if (slide) *slide = b.has_slide ? b.slide : NAN;
     if (stopped) *stopped = b.stopped;
     if (order) {

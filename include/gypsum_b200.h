@@ -410,6 +410,12 @@ int gb200_tracker_receiver_state(gb200_tracker* t, double* slide, int32_t* stopp
  * differed in any bit from the slide the fix before them left.  A receiver-clock jump inside a segment (a gap in the
  * sample stream) is an input that makes the check fail. */
 int gb200_tracker_fix_repairs(gb200_tracker* t, int64_t* n);
+/* The sizes of what the chain holds, for sizing the outputs of the calls that read it: out[0] = bit events per
+ * channel the last gb200_tracker_integrate_bits call kept (its max_events), out[1] = subframe events per channel the
+ * last gb200_tracker_decode_subframes call kept (its max_events), out[2] = n_ms of the last
+ * gb200_tracker_parse_subframes call, which gb200_tracker_observations and gb200_tracker_position_fixes cover.  Each is
+ * 0 before the first such call. */
+int gb200_tracker_chain_sizes(const gb200_tracker* t, int32_t out[3]);
 
 /* Kernel selection for gb200_acquire_cells.  Two implementations of the same arithmetic exist:
  *   0  doppler_spectra + correlate_cells: the PRN-independent half of the pipeline (wipe-off, forward transform) is
