@@ -79,7 +79,7 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 5 : 1) k_doppler_
     extern __shared__ __align__(16) float2 smem[];
     float2* ypoly = smem;                                       // [S][1024], rows in zpos() order
     float2* tiles = spec_alias(S) ? smem : smem + S * kFft;     // [kSpecWarps][kTileF2]
-    float2* coarse = smem + spec_f2(S);                         // [kCarrierTable] carrier at samples 0, 256, 512, ...
+    float2* coarse = smem + spec_f2(S);                         // [kCarrierTable] carrier at samples 0, T, 2T, ... (T threads)
 
     const int unit = blockIdx.x / a.M, i = blockIdx.x % a.M;
     const int b = unit / a.n_doppler, d = unit % a.n_doppler;
@@ -91,12 +91,13 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 5 : 1) k_doppler_
     const float2* __restrict__ src = a.iq + static_cast<size_t>(b) * a.block_stride + static_cast<size_t>(i) * a.N;
     const int tid = threadIdx.x;
 
-    // Carrier exp(-j 2 pi f (n + i N)/fs) (utils.py:93-96) as coarse[n / 256] * fine[n % 256]: both factors get an
+    // Carrier exp(-j 2 pi f (n + i N)/fs) (utils.py:93-96) as coarse[n / T] * fine[n % T]: both factors get an
     // exact float64-reduced phase, so there is one sincos per thread instead of one per sample and no recurrence
     // error growth.
-    constexpr int kIter = (kChips * S + kSpecThreads - 1) / kSpecThreads;  // samples per thread (16 for every S but 16: 64)
+    // samples per thread: 16 at S <= 4; 20, 24, 32, 40, 48 and 64 at S = 5, 6, 8, 10, 12 and 16 (8 warps from S = 4 on)
+    constexpr int kIter = (kChips * S + kSpecThreads - 1) / kSpecThreads;
     // coalesced float2 loads of the 1-ms IQ vector, ALL issued before the carrier set-up and the first use (the loop form
-    // stalls on every load)
+    // stalls on every load); from S = 5 on the samples past the first 16 per thread go through the tail loop below
     constexpr int kBatch = kIter < 16 ? kIter : 16;
     float2 v[kBatch];
 #pragma unroll

@@ -19,7 +19,9 @@ def test_warp_fft1024(emu_lib, inverse):
 
 
 @pytest.mark.parametrize("n,n_ms,sv,f", [(2046, 1, 25, 1500.0), (2046, 3, 7, -3250.0), (4092, 2, 11, 4875.5),
-                                         (16368, 1, 32, -250.0), (1023, 2, 1, 700.0), (3069, 1, 19, 10000.0)])
+                                         (16368, 1, 32, -250.0), (1023, 2, 1, 700.0), (3069, 1, 19, 10000.0),
+                                         (5115, 2, 14, 2345.0), (6138, 1, 7, -4250.0), (8184, 3, 21, 6500.0),
+                                         (10230, 1, 30, -1250.0), (12276, 2, 2, 9000.0)])
 def test_polyphase_correlation_matches_oracle(emu_lib, n, n_ms, sv, f):
     emu_lib.emu_cell_profile.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_double,
                                          ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]

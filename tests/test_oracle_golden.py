@@ -1,4 +1,5 @@
-"""The oracle (oracle/gypsum_oracle.py) against fixtures produced by the live reference (tools/make_golden.py)
+"""The oracle (oracle/gypsum_oracle.py) against fixtures produced by the live reference (tools/make_golden.py, and
+tools/make_golden_rates.py for 5.115 .. 12.276 Msps)
 and against the only known-answer table the reference holds (IS-GPS-200 first ten chips)."""
 import os
 
@@ -63,6 +64,42 @@ def test_oracle_detector_matches_reference_detector():
         r = o.acquire_sv(int(row[0]), x, 2046000, 2046)
         assert (r.doppler, r.code_phase) == (int(row[1]), int(row[3]))
         assert r.carrier_phase == row[2] and r.strength == row[4]
+
+
+RATES_GOLDEN = os.path.join(GOLDEN, "acquisition_rates.npz")
+
+
+@pytest.mark.parametrize("s", [5, 6, 8, 10, 12])
+def test_oracle_profiles_bit_exact_with_reference_at_other_rates(s):
+    """tools/make_golden_rates.py: one planted cell at M = 2, the planted code phase on the last polyphase branch."""
+    z = np.load(RATES_GOLDEN)
+    n, key = 1023 * s, f"cell_n{1023 * s}"
+    planted = [(int(p[0]), p[1], int(p[2]), p[3], p[4]) for p in z[f"{key}__planted"]]
+    x = o.synth_iq(int(z["profile_seed"]), n, int(z["profile_ms"]), n * 1000, planted)
+    prn = o.replica(int(z[f"{key}__sv"]), n)
+    f = float(z[f"{key}__doppler"])
+    nc = o.integrate(o.NON_COHERENT, x, n * 1000, n, f, prn)
+    assert np.array_equal(nc, z[f"{key}__noncoherent"])
+    assert np.array_equal(o.integrate(o.COHERENT, x, n * 1000, n, f, prn), z[f"{key}__coherent"])
+    assert o.peak_strength(nc) == float(z[f"{key}__strength"])
+    assert int(nc.argmax()) == n - 1
+
+
+@pytest.mark.parametrize("s", [5, 12])
+def test_oracle_detector_matches_reference_detector_at_other_rates(s):
+    """acquisition.py:70-152 for two planted satellites and an absent one, and acquisition.py:52-68 over the three."""
+    z = np.load(RATES_GOLDEN)
+    n, key = 1023 * s, f"detect_n{1023 * s}"
+    planted = [(int(p[0]), p[1], int(p[2]), p[3], p[4]) for p in z[f"{key}__planted"]]
+    x = o.synth_iq(int(z[f"{key}__seed"]), n, int(z[f"{key}__n_ms"]), n * 1000, planted)
+    got = []
+    for row in z[f"{key}__results"]:
+        r = o.acquire_sv(int(row[0]), x, n * 1000, n)
+        assert (r.doppler, r.code_phase) == (int(row[1]), int(row[3]))
+        assert r.carrier_phase == row[2] and r.strength == row[4]
+        got.append(r)
+    assert [r.sv for r in got if r.strength > o.DETECTION_THRESHOLD] == list(z[f"{key}__detected"])
+    assert int(z[f"{key}__results"][0, 3]) == n - 1
 
 
 def test_doppler_bins_semantics():

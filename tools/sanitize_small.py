@@ -103,6 +103,23 @@ for n, m in ((2046, 2), (4092, 1)):
         pr = eng.correlation_profile_replica(odd, 250.0, 2, _native.NON_COHERENT)
         assert pr.shape == (n,)
     eng.close()
+# rates where doppler_spectra runs its tail loop with separate rows and tiles: S = 5 (odd N, correlate split 1) and S = 12
+# (split 12 at M = 1, 4 at M = 2)
+for n in (5115, 12276):
+    fs = n * 1000
+    eng = _native.Engine(fs, n)
+    eng.set_replicas(chips)
+    x = o.synth_iq(5, n, 2, fs, [(25, 1500.0, n - 1, 0.3, 0.3)])
+    eng.upload_iq(x)
+    dop = np.arange(-2000, 2001, 500.0)
+    for m in (1, 2):
+        g = eng.acquire_grid(1, m, [24, 0, 5], dop)
+        assert int(g["argmax"][0, 0, 7]) == n - 1
+    c = eng.acquire_cells([24, 3, 24], [1500.0, 0.0, 1000.0], 2, _native.COHERENT, probe_idx=[n - 1, 0, n // 2])
+    p = eng.correlation_profile(24, 1500.0, 2, _native.NON_COHERENT)
+    r = eng.detect([24, 2], 2)
+    assert int(p.argmax()) == n - 1 == int(c["argmax"][0]) == int(r["code_phase"][0])
+    eng.close()
 # 16.368 Msps tracking (k_track_channels_wide<16>): a channel bank with profiles, then a pool step with undo
 n = 16368
 fs = n * 1000
