@@ -86,6 +86,7 @@ SYMBOLS = {
     "gb200_tracker_position_fixes_device": (C.c_int, [_P, _P, _P]),
     "gb200_tracker_receiver_state": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_int32), _P]),
     "gb200_tracker_fix_repairs": (C.c_int, [_P, C.POINTER(C.c_int64)]),
+    "gb200_tracker_set_fix_solver": (C.c_int, [_P, C.c_int]),
     "gb200_tracker_chain_sizes": (C.c_int, [_P, _P]),
     "gb200_set_fused": (C.c_int, [_P, C.c_int]),
     "gb200_launch_count": (C.c_int, [_P, C.POINTER(C.c_int64)]),
@@ -646,6 +647,16 @@ class Tracker:
                             "gb200_tracker_position_fixes")
         return out
 
+    def set_fix_solver(self, solver: str) -> None:
+        """Which fix a millisecond with five or more ready satellites gets (gb200_tracker_set_fix_solver): "reference"
+        (the default) raises there as the reference does and stops the receiver; "least_squares" solves by least
+        squares over all of them.  Only before the first fix call (RuntimeError after it); ValueError for another
+        name."""
+        if solver not in FIX_SOLVERS:
+            raise ValueError(f"fix solver must be one of {sorted(FIX_SOLVERS)}, not {solver!r}")
+        self._engine._check(self._lib.gb200_tracker_set_fix_solver(self._h, FIX_SOLVERS[solver]),
+                            "gb200_tracker_set_fix_solver")
+
     def position_fixes_device(self, receiver_timestamps, out_device_ptr: int) -> None:
         """Enqueue only: n_ms FIX_DTYPE records to device memory."""
         rx = self._fix_times(receiver_timestamps)
@@ -715,6 +726,7 @@ FIX_DTYPE = np.dtype([  # gb200_position_fix
     ("channel", "<i4", (4,))])
 assert FIX_DTYPE.itemsize == 112
 FIX_NONE, FIX_SOLVED, FIX_RAISED, FIX_STOPPED = 0, 1, 2, 3  # FIX_DTYPE["status"]
+FIX_SOLVERS = {"reference": 0, "least_squares": 1}  # GB200_FIX_SOLVER_*
 
 
 def subframe_event_capacity(n_bits: int) -> int:

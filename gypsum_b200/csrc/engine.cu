@@ -239,6 +239,7 @@ struct gb200_tracker {
         PinnedBuf<SvObservation> h_obs;
     } orbit;
     struct {  // fix.cu: the receiver state is `bank` and `rank`
+        int solver = kFixSolverReference;  // gb200_tracker_set_fix_solver
         DevBuf<FixBank> bank;
         DevBuf<int> rank, order, touch, prev;
         DevBuf<double> rx, reset, slide1;
@@ -291,6 +292,8 @@ static_assert(sizeof(gb200_sv_observation) == sizeof(SvObservation) &&
                   offsetof(gb200_sv_observation, prn_count) == offsetof(SvObservation, prn_count) &&
                   offsetof(gb200_sv_observation, flags) == offsetof(SvObservation, flags),
               "ABI observation and device observation must match");
+static_assert(GB200_FIX_SOLVER_REFERENCE == kFixSolverReference && GB200_FIX_SOLVER_LEAST_SQUARES == kFixSolverLeastSquares,
+              "ABI and device fix solvers must match");
 static_assert(sizeof(gb200_position_fix) == sizeof(FixRecord) &&
                   offsetof(gb200_position_fix, pseudorange) == offsetof(FixRecord, pseudorange) &&
                   offsetof(gb200_position_fix, status) == offsetof(FixRecord, status) &&
@@ -1836,6 +1839,7 @@ static int fixes_launch(gb200_tracker* t, const double* rx_host, FixRecord* out_
     a.out = out_dev;
     a.n_channels = nc;
     a.n_ms = n_ms;
+    a.solver = s.solver;
     GB_LAUNCH(e, -1, launch_position_fixes(a, e->stream));
     e->launches += 4;  // plan, two passes, repair and finish
     t->chain.fixed();
@@ -1859,6 +1863,16 @@ int gb200_tracker_position_fixes(gb200_tracker* t, const double* receiver_timest
     if (n) GB_CUDA(e, s.d_fixes.ensure(n));
     GB_TRY(fixes_launch(t, receiver_timestamps_host, s.d_fixes.p));
     return download(e, reinterpret_cast<FixRecord*>(out_host), s.d_fixes.p, n, s.h_fixes);
+}
+
+int gb200_tracker_set_fix_solver(gb200_tracker* t, int solver) {
+    if (!t) return GB200_EINVAL;
+    if (solver != GB200_FIX_SOLVER_REFERENCE && solver != GB200_FIX_SOLVER_LEAST_SQUARES)
+        GB_FAIL(t->e, GB200_EINVAL, "unknown fix solver %d", solver);
+    // the receiver's stop and slide so far came from the mode they were computed in
+    if (t->fix.bank.p) GB_FAIL(t->e, GB200_ESTATE, "the fix solver cannot change after the tracker's first fix call");
+    t->fix.solver = solver;
+    return GB200_OK;
 }
 
 int gb200_tracker_fix_repairs(gb200_tracker* t, int64_t* n) {

@@ -19,6 +19,12 @@
 // from.  k_fix_repair: where that check fails anywhere, one thread runs the chain serially from the first miss, each
 // fix from the slide the fix before it left -- the reference's serial chain, at its serial cost.
 // k_fix_finish: one warp.  Everything after the first raise stops, and the receiver's slide is carried to the next call.
+//
+// The least-squares mode (FixArgs::solver) runs k_fix_plan_lsq, k_fix_pass_lsq<1/2> and k_fix_repair_lsq, the same
+// templates instantiated for it: five or more ready is a fix like any other, over all ready rows (fix_compute_lsq).
+// Such rows can change inside a segment, and a fix that has not converged can depend on its entering slide; the chain
+// check and the repair cover that as they cover a clock jump (DESIGN.md §8c).  The reference-mode kernels keep their
+// names and code.
 #include "fix_core.cuh"
 #include "kernels.cuh"
 
@@ -27,7 +33,8 @@ namespace gb {
 constexpr int kFixThreads = 128;
 constexpr unsigned kFixFull = 0xffffffffu;
 
-__global__ void __launch_bounds__(32) k_fix_plan(const FixArgs a) {
+template <int kSolver>
+__device__ __forceinline__ void fix_plan(const FixArgs& a) {
     const int lane = threadIdx.x;
     const int nc = a.n_channels, n_ms = a.n_ms;
     FixBank& bk = *a.bank;
@@ -108,13 +115,14 @@ __global__ void __launch_bounds__(32) k_fix_plan(const FixArgs a) {
         const double rv = __shfl_sync(kFixFull, r, reset_lane < 0 ? 0 : reset_lane);
         const double slide = reset_lane >= 0 ? rv : seg;
         const int has = reset_lane >= 0 ? 1 : have;
-        // five or more ready with a slide: the first such millisecond raises, and everything after it has stopped
-        const unsigned many = __ballot_sync(kFixFull, live && n_ready > kFixRows && has);
+        // five or more ready with a slide: the first such millisecond raises, and everything after it has stopped (in
+        // the least-squares mode they are fixes like any other)
+        const unsigned many = kSolver == kFixSolverReference ? __ballot_sync(kFixFull, live && n_ready > kFixRows && has) : 0u;
         const int first5 = many ? m0 + __ffs(many) - 1 : n_ms;
         const bool stopped = !live || m > first5;
         const bool raised = !stopped && m == first5;
         const unsigned resets = many ? live_resets & (kFixFull >> (31 - (__ffs(many) - 1))) : live_resets;
-        const bool cand = !stopped && n_ready == kFixRows && has;
+        const bool cand = !stopped && (kSolver == kFixSolverReference ? n_ready == kFixRows : n_ready >= kFixRows) && has;
         const unsigned links = __ballot_sync(kFixFull, cand || raised);
         // the previous link of the segment: before this millisecond, at or after the segment's reset
         unsigned earlier = links & ((1u << lane) - 1u);
@@ -155,6 +163,9 @@ __global__ void __launch_bounds__(32) k_fix_plan(const FixArgs a) {
     }
 }
 
+__global__ void __launch_bounds__(32) k_fix_plan(const FixArgs a) { fix_plan<kFixSolverReference>(a); }
+__global__ void __launch_bounds__(32) k_fix_plan_lsq(const FixArgs a) { fix_plan<kFixSolverLeastSquares>(a); }
+
 // The fix of millisecond m from slide s, over the rows the plan chose.
 __device__ int fix_at(const FixArgs& a, int m, double s, FixRecord& f) {
     FixRow r[kFixRows];
@@ -165,8 +176,29 @@ __device__ int fix_at(const FixArgs& a, int m, double s, FixRecord& f) {
     return fix_compute(r, f.receiver_timestamp, s, f);
 }
 
-template <int kPass>
-__global__ void __launch_bounds__(kFixThreads) k_fix_pass(const FixArgs a) {
+// The ready rows of millisecond m in the world model's order, for fix_compute_lsq: read from the observations again
+// on every iteration, so any number of rows needs no storage.
+struct FixReadyRows {
+    const FixArgs& a;
+    int m, n_touched;
+    template <class F>
+    __device__ __forceinline__ void operator()(F&& fn) const {
+        int i = 0;
+        for (int k = 0; k < n_touched; ++k) {
+            const SvObservation& o = a.obs[static_cast<size_t>(a.order[k]) * a.n_ms + m];
+            if ((o.flags & (kObsComplete | kObsFixGate)) == (kObsComplete | kObsFixGate)) fn(i++, FixRow{o.tow, o.x, o.y, o.z});
+        }
+    }
+};
+
+// fix_at in the least-squares mode: five or more rows take the least-squares fix.
+__device__ __forceinline__ int fix_at_lsq(const FixArgs& a, int m, double s, FixRecord& f) {
+    if (f.n_ready == kFixRows) return fix_at(a, m, s, f);
+    return fix_compute_lsq(FixReadyRows{a, m, a.bank->n_touched}, f.n_ready, f.receiver_timestamp, s, f);
+}
+
+template <int kSolver, int kPass>
+__device__ __forceinline__ void fix_pass(const FixArgs& a) {
     const int m = blockIdx.x * kFixThreads + threadIdx.x;
     if (m >= a.n_ms) return;
     FixRecord f = a.out[m];
@@ -174,7 +206,9 @@ __global__ void __launch_bounds__(kFixThreads) k_fix_pass(const FixArgs a) {
     double s = f.slide_in;
     if (kPass == 2 && a.prev[m] >= 0) s = a.slide1[a.prev[m]];
     int status = kFixRaised;
-    if (f.status == kFixRaised) {  // five or more ready: np.linalg.solve raises before anything changes
+    if (kSolver == kFixSolverLeastSquares) {  // the plan marks no raise in this mode
+        status = fix_at_lsq(a, m, s, f);
+    } else if (f.status == kFixRaised) {  // five or more ready: np.linalg.solve raises before anything changes
         f.slide_in = f.slide_out = s;
     } else {
         status = fix_at(a, m, s, f);
@@ -191,11 +225,21 @@ __global__ void __launch_bounds__(kFixThreads) k_fix_pass(const FixArgs a) {
     if (!fix_same_slide(f.slide_out, a.slide1[m])) atomicMin(&a.bank->first_miss, m);
 }
 
+template <int kPass>
+__global__ void __launch_bounds__(kFixThreads) k_fix_pass(const FixArgs a) {
+    fix_pass<kFixSolverReference, kPass>(a);
+}
+template <int kPass>
+__global__ void __launch_bounds__(kFixThreads) k_fix_pass_lsq(const FixArgs a) {
+    fix_pass<kFixSolverLeastSquares, kPass>(a);
+}
+
 // Where the chain check failed, the serial chain: from the first miss on, every fix that does not start from a reset
 // runs again from the slide the fix before it left, in order, in one thread.  The comparison is exact, not the check's
 // 4 ulp: after a miss every fix of the call, in later segments too, is the serial chain's bit for bit, and n_repaired
 // counts each fix whose entering slide changed.
-__global__ void __launch_bounds__(32) k_fix_repair(const FixArgs a) {
+template <int kSolver>
+__device__ __forceinline__ void fix_repair(const FixArgs& a) {
     FixBank& bk = *a.bank;
     if (threadIdx.x != 0 || bk.first_miss >= a.n_ms) return;
     int last = bk.first_miss;
@@ -204,10 +248,10 @@ __global__ void __launch_bounds__(32) k_fix_repair(const FixArgs a) {
         if (f.status != kFixSolved && f.status != kFixRaised) continue;
         const double s = a.out[last].slide_out;
         if (a.prev[m] >= 0 && !(f.slide_in == s)) {
-            if (f.n_ready > kFixRows) {
+            if (kSolver == kFixSolverReference && f.n_ready > kFixRows) {
                 f.slide_in = f.slide_out = s;
             } else {
-                f.status = fix_at(a, m, s, f);
+                f.status = kSolver == kFixSolverReference ? fix_at(a, m, s, f) : fix_at_lsq(a, m, s, f);
                 if (f.status == kFixRaised && m < bk.first_raise) bk.first_raise = m;
             }
             a.out[m] = f;
@@ -216,6 +260,9 @@ __global__ void __launch_bounds__(32) k_fix_repair(const FixArgs a) {
         last = m;
     }
 }
+
+__global__ void __launch_bounds__(32) k_fix_repair(const FixArgs a) { fix_repair<kFixSolverReference>(a); }
+__global__ void __launch_bounds__(32) k_fix_repair_lsq(const FixArgs a) { fix_repair<kFixSolverLeastSquares>(a); }
 
 __global__ void __launch_bounds__(32) k_fix_finish(const FixArgs a) {
     const int lane = threadIdx.x;
@@ -251,10 +298,17 @@ __global__ void __launch_bounds__(32) k_fix_finish(const FixArgs a) {
 
 cudaError_t launch_position_fixes(const FixArgs& a, cudaStream_t st) {
     const int blocks = (a.n_ms + kFixThreads - 1) / kFixThreads;
-    k_fix_plan<<<1, 32, 0, st>>>(a);
-    k_fix_pass<1><<<blocks, kFixThreads, 0, st>>>(a);
-    k_fix_pass<2><<<blocks, kFixThreads, 0, st>>>(a);
-    k_fix_repair<<<1, 32, 0, st>>>(a);
+    if (a.solver == kFixSolverLeastSquares) {
+        k_fix_plan_lsq<<<1, 32, 0, st>>>(a);
+        k_fix_pass_lsq<1><<<blocks, kFixThreads, 0, st>>>(a);
+        k_fix_pass_lsq<2><<<blocks, kFixThreads, 0, st>>>(a);
+        k_fix_repair_lsq<<<1, 32, 0, st>>>(a);
+    } else {
+        k_fix_plan<<<1, 32, 0, st>>>(a);
+        k_fix_pass<1><<<blocks, kFixThreads, 0, st>>>(a);
+        k_fix_pass<2><<<blocks, kFixThreads, 0, st>>>(a);
+        k_fix_repair<<<1, 32, 0, st>>>(a);
+    }
     k_fix_finish<<<1, 32, 0, st>>>(a);
     return cudaGetLastError();
 }

@@ -8,6 +8,15 @@
 // multiply-add contraction) in the reference's order of operations; np.linalg.solve is Gaussian elimination with partial
 // pivoting, the kind of solve LAPACK's dgesv does, with IEEE division.  It cannot round as OpenBLAS does, so parity with
 // the reference is a bound (DESIGN.md §6), while the host and device builds of this file agree bit for bit.
+//
+// The least-squares mode (gb200_tracker_set_fix_solver) solves where the reference raises, with five or more ready
+// rows: the same rounds, iterations and squared-range system over all N rows, each step the least-squares solution of
+// J v = -r (Gauss-Newton, what np.linalg.lstsq(J, -r) gives in place of solve).  Each row of [J | -r] is rotated into
+// a 4x4 upper triangle and a 4-vector by Givens rotations as it is read, so the solve keeps no per-row storage, and
+// back-substitution gives v.  The normal equations J^T J are no option: the clock column (2 c^2 dt) is about 1e8 times
+// the position columns (2 dx), and J^T J would square a condition number already near 1e8-1e9.  numpy's lstsq is an
+// SVD (LAPACK gelsd) and rounds differently, so parity with numpy is a bound here too (DESIGN.md §8c); the host and
+// device builds agree bit for bit (o_add / o_mul, IEEE sqrt and division).  Exactly four rows take fix_compute.
 #pragma once
 #include <math.h>
 
@@ -25,8 +34,15 @@ constexpr int kFixRows = 4;
 enum FixStatus {
     kFixNone = 0,     // fewer than 4 satellites ready, or no clock slide yet
     kFixSolved = 1,   // the solution of _compute_position
-    kFixRaised = 2,   // the reference raises here (5 or more ready, or an exactly singular system)
+    kFixRaised = 2,   // the reference raises here (5 or more ready, or an exactly singular system); in the
+                      // least-squares mode: an exactly singular 4-row system or a rank-deficient one of 5 or more
     kFixStopped = 3,  // the receiver stopped at or before this millisecond
+};
+
+// gb200_tracker_set_fix_solver
+enum FixSolver {
+    kFixSolverReference = 0,     // the reference: 5 or more ready raises
+    kFixSolverLeastSquares = 1,  // 5 or more ready: the least-squares fix (fix_compute_lsq)
 };
 
 struct FixRecord {  // mirrors include/gypsum_b200.h gb200_position_fix, 112 bytes
@@ -73,20 +89,24 @@ GB_HD inline void fix_record_clear(FixRecord& f, double receiver_timestamp) {
     f.n_ready = 0;
 }
 
+// One row of the system at pseudorange t: its negated residual and its Jacobian row.
+GB_HD GB_INLINE void fix_row(const FixRow& r, double t, double gx, double gy, double gz, double cb, double a[kFixRows],
+                             double& rhs) {
+    const double dx = o_sub(gx, r.x), dy = o_sub(gy, r.y), dz = o_sub(gz, r.z);
+    const double dt = o_sub(t, cb);
+    const double ct = o_mul(kSpeedOfLight, dt);
+    rhs = -o_sub(o_add(o_add(o_mul(dx, dx), o_mul(dy, dy)), o_mul(dz, dz)), o_mul(ct, ct));
+    a[0] = o_mul(2.0, dx);
+    a[1] = o_mul(2.0, dy);
+    a[2] = o_mul(2.0, dz);
+    a[3] = o_mul(2.0, o_mul(kSpeedOfLight2, dt));
+}
+
 // _compute_solution_residuals (:489-507), negated as np.linalg.solve gets them, and _compute_jacobian_matrix (:509-526).
 GB_HD GB_INLINE void fix_system(const FixRow* r, const double* t, double gx, double gy, double gz, double cb,
                                 double a[kFixRows][kFixRows], double rhs[kFixRows]) {
 #pragma unroll
-    for (int i = 0; i < kFixRows; ++i) {
-        const double dx = o_sub(gx, r[i].x), dy = o_sub(gy, r[i].y), dz = o_sub(gz, r[i].z);
-        const double dt = o_sub(t[i], cb);
-        const double ct = o_mul(kSpeedOfLight, dt);
-        rhs[i] = -o_sub(o_add(o_add(o_mul(dx, dx), o_mul(dy, dy)), o_mul(dz, dz)), o_mul(ct, ct));
-        a[i][0] = o_mul(2.0, dx);
-        a[i][1] = o_mul(2.0, dy);
-        a[i][2] = o_mul(2.0, dz);
-        a[i][3] = o_mul(2.0, o_mul(kSpeedOfLight2, dt));
-    }
+    for (int i = 0; i < kFixRows; ++i) fix_row(r[i], t[i], gx, gy, gz, cb, a[i], rhs[i]);
 }
 
 // np.linalg.solve(a, b) for one 4x4 system, in place: Gaussian elimination with partial pivoting (the first largest
@@ -158,6 +178,106 @@ GB_HD inline int fix_compute(const FixRow* r, double rx, double slide, FixRecord
             cb = o_add(cb, v[3]);
         }
         slide = o_sub(slide, cb);  // self.receiver_clock_slide -= clock_bias
+    }
+    f.slide_out = slide;
+    f.clock_bias = cb;
+    f.x = gx;
+    f.y = gy;
+    f.z = gz;
+    return kFixSolved;
+}
+
+// The streaming least-squares solve: the upper triangle R (r[i][j], j >= i) and Q^T b of the rows added so far.
+struct FixLsq {
+    double r[kFixRows][kFixRows];
+    double q[kFixRows];
+};
+
+GB_HD GB_INLINE void fix_lsq_clear(FixLsq& s) {
+#pragma unroll
+    for (int i = 0; i < kFixRows; ++i) {
+        s.q[i] = 0.0;
+#pragma unroll
+        for (int j = 0; j < kFixRows; ++j) s.r[i][j] = 0.0;
+    }
+}
+
+// Rotates the row [a | b] into the triangle, column by column (a and b are consumed).  Each rotation zeroes a[k]
+// against r[k][k] and leaves r[k][k] >= 0.
+GB_HD GB_INLINE void fix_lsq_add(FixLsq& s, double a[kFixRows], double b) {
+#pragma unroll
+    for (int k = 0; k < kFixRows; ++k) {
+        if (a[k] == 0.0) continue;
+        const double h = sqrt(o_add(o_mul(s.r[k][k], s.r[k][k]), o_mul(a[k], a[k])));
+        const double c = s.r[k][k] / h, sn = a[k] / h;
+        s.r[k][k] = h;
+#pragma unroll
+        for (int j = k + 1; j < kFixRows; ++j) {
+            const double u = s.r[k][j], w = a[j];
+            s.r[k][j] = o_add(o_mul(c, u), o_mul(sn, w));
+            a[j] = o_sub(o_mul(c, w), o_mul(sn, u));
+        }
+        const double u = s.q[k];
+        s.q[k] = o_add(o_mul(c, u), o_mul(sn, b));
+        b = o_sub(o_mul(c, b), o_mul(sn, u));
+    }
+}
+
+// Back-substitution R v = Q^T b over n rows.  Returns false where the system has rank < 4 as np.linalg.lstsq judges it
+// with its default rcond (machine epsilon * max(n, 4)), here on R's diagonal: |r_kk| <= eps * max(n, 4) * max |r_jj|.
+GB_HD GB_INLINE bool fix_lsq_solve(const FixLsq& s, int n, double v[kFixRows]) {
+    double top = 0.0;
+#pragma unroll
+    for (int k = 0; k < kFixRows; ++k) top = fmax(top, s.r[k][k]);
+    const double tol = o_mul(o_mul(0x1p-52, static_cast<double>(n > kFixRows ? n : kFixRows)), top);
+#pragma unroll
+    for (int k = 0; k < kFixRows; ++k)
+        if (!(s.r[k][k] > tol)) return false;
+#pragma unroll
+    for (int i = kFixRows - 1; i >= 0; --i) {
+        double t = s.q[i];
+#pragma unroll
+        for (int j = i + 1; j < kFixRows; ++j) t = o_sub(t, o_mul(s.r[i][j], v[j]));
+        v[i] = t / s.r[i][i];
+    }
+    return true;
+}
+
+// fix_compute over n >= 5 rows in the least-squares mode.  rows(fn) calls fn(i, FixRow) for the rows i = 0..n-1 in the
+// world model's order; it runs once per iteration, so the rows are read again rather than kept.  pseudorange[] holds
+// round 0's of the first four rows.  Returns kFixSolved, or kFixRaised where the system is rank-deficient (slide_out is
+// then the slide at that point and the solution stays NaN).
+template <class Rows>
+GB_HD inline int fix_compute_lsq(const Rows& rows, int n, double rx, double slide, FixRecord& f) {
+    f.slide_in = slide;
+    double gx = 0.0, gy = 0.0, gz = 0.0, cb = 0.0;
+    for (int round = 0; round < kFixRounds; ++round) {
+        const double now = o_add(slide, rx);
+        if (round == 0)
+            rows([&](int i, const FixRow& r) {
+#pragma unroll
+                for (int j = 0; j < kFixRows; ++j)  // by compile-time index, so the record stays in registers
+                    if (i == j) f.pseudorange[j] = o_sub(now, r.tow);
+            });
+        for (int it = 0; it < kFixIterations; ++it) {
+            FixLsq s;
+            fix_lsq_clear(s);
+            rows([&](int, const FixRow& r) {
+                double a[kFixRows], b;
+                fix_row(r, o_sub(now, r.tow), gx, gy, gz, cb, a, b);
+                fix_lsq_add(s, a, b);
+            });
+            double v[kFixRows];
+            if (!fix_lsq_solve(s, n, v)) {
+                f.slide_out = slide;
+                return kFixRaised;
+            }
+            gx = o_add(gx, v[0]);
+            gy = o_add(gy, v[1]);
+            gz = o_add(gz, v[2]);
+            cb = o_add(cb, v[3]);
+        }
+        slide = o_sub(slide, cb);
     }
     f.slide_out = slide;
     f.clock_bias = cb;

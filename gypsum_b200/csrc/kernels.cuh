@@ -163,6 +163,7 @@ struct FixArgs {
     double* slide1;              // [n_ms] scratch: pass 1's slide after each fix
     FixRecord* out;              // [n_ms]
     int n_channels, n_ms;
+    int solver;                  // FixSolver: which kernels launch_position_fixes runs
 };
 cudaError_t launch_position_fixes(const FixArgs& a, cudaStream_t st);
 

@@ -320,9 +320,11 @@ class GpsSatelliteTracker:
 
 class TrackerBank:
     """Throughput interface: `n` channels advance through a block of milliseconds in one persistent-kernel launch
-    (BASELINE config 4).  channels: iterable of (satellite, doppler_hz, carrier_phase_rad, code_phase_samples)."""
+    (BASELINE config 4).  channels: iterable of (satellite, doppler_hz, carrier_phase_rad, code_phase_samples).
+    fix_solver: what position_fixes does with five or more ready satellites, "reference" (raise and stop, as the
+    reference receiver does) or "least_squares" (solve over all of them)."""
 
-    def __init__(self, channels, stream_attributes, device: int = 0):
+    def __init__(self, channels, stream_attributes, device: int = 0, fix_solver: str = "reference"):
         fs, n = int(stream_attributes.samples_per_second), int(stream_attributes.samples_per_prn_transmission)
         self.samples_per_ms = n
         self._ent = POOL.get(fs, n, device)
@@ -331,6 +333,7 @@ class TrackerBank:
         idx = [_replica_index(self._ent, c[0], n) for c in channels]
         self.native = _native.Tracker(self.engine, idx, [c[1] for c in channels], [c[2] for c in channels],
                                       [c[3] for c in channels])
+        self.native.set_fix_solver(fix_solver)
         self.n_channels = len(channels)
 
     def process(self, samples: np.ndarray, start_times, want_profiles: bool = False):
@@ -388,7 +391,10 @@ class TrackerBank:
     def position_fixes(self, start_times) -> np.ndarray:
         """_native.FIX_DTYPE [ms] over the milliseconds of the last parse_subframes call: the position fix the world
         model attempts every millisecond (world_model.py:567-633), start_times being the chunk start times.  The bank is
-        one receiver: its clock slide, world-model order and stop carry from call to call.
+        one receiver: its clock slide, world-model order and stop carry from call to call.  With five or more ready
+        satellites the reference raises: with fix_solver="reference" that millisecond has status 2 and the receiver
+        stops for good; with "least_squares" it is fixed over all of them (n_ready of them; channel and pseudorange
+        hold the first four), and only a rank-deficient system raises.
         gypsum_b200.world_model.solution_from_fix turns a status-1 record into a ReceiverSolution."""
         return self.native.position_fixes(start_times)
 

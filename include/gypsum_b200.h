@@ -372,10 +372,13 @@ int gb200_tracker_observations_device(gb200_tracker* t, void* out_device);
  * clock slide, which every subframe of any channel resets to tow - trailing_edge_receiver_timestamp (:749-752, the last
  * one of a millisecond wins, channels in order), and one world-model order, in which satellites enter at their first
  * subframe or lost lock.  A millisecond's ready channels have flags 2 and 4; with exactly 4, _compute_position runs 5
- * rounds of 20 Newton iterations from zero, and after each round the slide drops by the clock bias.  status:
+ * rounds of 20 Newton iterations from zero, and after each round the slide drops by the clock bias.  With 5 or more,
+ * the reference raises; in the least-squares mode (gb200_tracker_set_fix_solver) the same rounds run over all of them,
+ * each step the least-squares solution (n_ready holds their number, channel and pseudorange the first four).  status:
  *   0  no fix: fewer than 4 ready, or no slide yet
  *   1  fixed: everything set
- *   2  the reference raises here (5 or more ready: numpy's non-square solve; or an exactly singular system); slide_in
+ *   2  the reference raises here (5 or more ready: numpy's non-square solve; or an exactly singular system); in the
+ *      least-squares mode only an exactly singular 4-row system or a rank-deficient one of 5 or more rows; slide_in
  *      and slide_out hold the slide at the raise
  *   3  stopped: the receiver raised earlier, or a channel's decoder raised (event kind 3) at or before this ms
  * Values that are not set are NaN.  Parity with the reference is a bound (DESIGN.md §6): numpy's LAPACK cannot be
@@ -399,6 +402,14 @@ typedef char gb200_position_fix_is_112_bytes[sizeof(gb200_position_fix) == 112 ?
  * first fix call (the slide chain would have a gap).  The _device variant only enqueues (out_device: n_ms records). */
 int gb200_tracker_position_fixes(gb200_tracker* t, const double* receiver_timestamps_host, gb200_position_fix* out_host);
 int gb200_tracker_position_fixes_device(gb200_tracker* t, const double* receiver_timestamps_host, void* out_device);
+/* Which fix a millisecond with 5 or more ready satellites gets: GB200_FIX_SOLVER_REFERENCE (the default) raises as
+ * the reference does, and the receiver stops; GB200_FIX_SOLVER_LEAST_SQUARES solves the reference's equations over
+ * every ready satellite by least squares (Gauss-Newton; DESIGN.md §8c) and goes on.  Milliseconds with 4 ready fix
+ * alike in both.  GB200_EINVAL for another value; GB200_ESTATE after the tracker's first fix call, since the
+ * receiver's slide and stop depend on the mode. */
+#define GB200_FIX_SOLVER_REFERENCE 0
+#define GB200_FIX_SOLVER_LEAST_SQUARES 1
+int gb200_tracker_set_fix_solver(gb200_tracker* t, int solver);
 /* The receiver's state after the last fix call: the clock slide (NaN = None), whether it has stopped, and
  * order[n_channels]: the channels in world-model order, -1 after the last. */
 int gb200_tracker_receiver_state(gb200_tracker* t, double* slide, int32_t* stopped, int32_t* order);

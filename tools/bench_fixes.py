@@ -9,7 +9,11 @@ observations it computes first); one round is also profiled for the kernels alon
 J is added to the fix call's receiver timestamps and to every later trailing edge.  Inside a segment that makes the
 device's chain check miss, and k_fix_repair recomputes the rest of the segment serially (DESIGN.md §8c); the result
 line then also reports the repaired fixes and the cost of each.
-usage (GPU box): python tools/bench_fixes.py [--reps 5] [--jump -0.2 [--jump-ms 1000]]"""
+
+--channels N tracks and fixes N channels (4 to 12) on the same schedule, so every fixing millisecond has N ready;
+--solver least_squares fixes them by least squares (gb200_tracker_set_fix_solver).  The reference mode raises at the
+first fix with more than four channels.
+usage (GPU box): python tools/bench_fixes.py [--reps 5] [--jump -0.2 [--jump-ms 1000]] [--channels 8 --solver least_squares]"""
 import argparse
 import json
 import os
@@ -27,7 +31,8 @@ from gypsum_b200.gps_ca_prn_codes import ca_code_chips  # noqa: E402
 from oracle import orbit_oracle as orb  # noqa: E402
 
 N, FS = 2046, 2046000
-N_CH, N_MS, N_SUB = 4, 60000, 12
+N_MS, N_SUB = 60000, 12
+SVS = (5, 12, 19, 27, 2, 9, 15, 23, 30, 7, 17, 25)
 
 
 def timed(stream, fn):
@@ -52,24 +57,27 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--jump", type=float, default=0.0, help="receiver-clock jump in seconds (0: none)")
     ap.add_argument("--jump-ms", type=int, default=1000, help="the millisecond the jump lands on")
+    ap.add_argument("--channels", type=int, default=4, choices=range(4, len(SVS) + 1), metavar="N")
+    ap.add_argument("--solver", default="reference", choices=sorted(_native.FIX_SOLVERS))
     args = ap.parse_args()
+    n_ch = args.channels
     eng = _native.Engine(FS, N)
     eng.set_replicas(np.stack([ca_code_chips(sv) for sv in range(1, 33)]).astype(np.uint8))
     stream = torch.cuda.Stream()
     eng.set_stream(stream.cuda_stream)
-    svs = (5, 12, 19, 27)
+    svs = SVS[:n_ch]
     chans = [(sv, 1000.0 + 37.3 * c, 0.0, (53 * c) % N, 0.1 * c, 0.004) for c, sv in enumerate(svs)]
     base = to.synth_tracking_iq(5, N, 1000, FS, chans)
     xd = torch.from_numpy(base).cuda().repeat(N_MS // 1000)
     eng.bind_iq_device(xd.data_ptr(), xd.numel())
     times = np.array([round(k * N / FS, 6) for k in range(N_MS)])
-    rec = torch.empty(N_CH * N_MS * _native.TRACK_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+    rec = torch.empty(n_ch * N_MS * _native.TRACK_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
     fix_times = times.copy()
     fix_times[args.jump_ms:] += args.jump
 
     rng = np.random.default_rng(1)
-    host = np.zeros((N_CH, N_SUB), dtype=_native.SUBFRAME_DTYPE)
-    ems = np.zeros((N_CH, N_SUB), dtype=np.int32)
+    host = np.zeros((n_ch, N_SUB), dtype=_native.SUBFRAME_DTYPE)
+    ems = np.zeros((n_ch, N_SUB), dtype=np.int32)
     for c, sv in enumerate(svs):
         sfs = orb.ephemeris_subframes(orb.realistic_ephemeris(rng, sv), N_SUB, first_id=1, tow0=20000, seed=c)
         for k, sf in enumerate(sfs):
@@ -77,14 +85,15 @@ def main():
             host[c, k]["words"] = orb.words_of(sf)
             host[c, k]["trailing_edge_receiver_timestamp"] = fix_times[min(m, N_MS - 1)] - 0.0003 * c
             ems[c, k] = min(m, N_MS - 1)
-    ev_dev = torch.from_numpy(host.view(np.uint8).reshape(N_CH, -1)).cuda()
-    counts = np.full(N_CH, N_SUB, dtype=np.int32)
-    drop = np.full(N_CH, -1, dtype=np.int32)
+    ev_dev = torch.from_numpy(host.view(np.uint8).reshape(n_ch, -1)).cuda()
+    counts = np.full(n_ch, N_SUB, dtype=np.int32)
+    drop = np.full(n_ch, -1, dtype=np.int32)
     out = torch.empty(N_MS * _native.FIX_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
 
     track_ms, fix_ms, kernel_ms, repaired = [], [], {}, []
     for rep in range(args.reps + 1):
-        trk = _native.Tracker(eng, list(range(N_CH)), [c[1] for c in chans], [0.0] * N_CH, [c[3] for c in chans])
+        trk = _native.Tracker(eng, list(range(n_ch)), [c[1] for c in chans], [0.0] * n_ch, [c[3] for c in chans])
+        trk.set_fix_solver(args.solver)
         dt, _ = timed(stream, lambda: trk.process_device(N_MS, times, rec.data_ptr()))
         trk.parse_subframes(ev_dev.data_ptr(), counts, N_SUB, ems, drop, N_MS)
         prof = torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) if rep == 1 else None
@@ -95,8 +104,9 @@ def main():
             prof.__exit__(None, None, None)
             for k in prof.key_averages():
                 for name in ("k_sv_observations", "k_fix_plan", "k_fix_pass<1>", "k_fix_pass<2>", "k_fix_repair",
-                             "k_fix_finish"):
-                    if name in k.key:
+                             "k_fix_finish", "k_fix_plan_lsq", "k_fix_pass_lsq<1>", "k_fix_pass_lsq<2>",
+                             "k_fix_repair_lsq"):
+                    if name + "(" in k.key or k.key.endswith(name):
                         kernel_ms[name] = getattr(k, "device_time_total", getattr(k, "cuda_time_total", 0.0)) / 1e3
         if rep:  # the first round allocates
             track_ms.append(dt)
@@ -108,9 +118,9 @@ def main():
     jump = {}
     if args.jump:
         jump = {"jump_s": args.jump, "jump_ms": args.jump_ms, "repaired_fixes": repaired[-1],
-                "repair_kernel_us_per_fix": kernel_ms.get("k_fix_repair", 0.0) * 1e3 / max(1, repaired[-1])}
+                "repair_kernel_us_per_fix": kernel_ms.get("k_fix_repair_lsq" if args.solver == "least_squares" else "k_fix_repair", 0.0) * 1e3 / max(1, repaired[-1])}
     print(json.dumps({
-        "workload": f"position_fixes_device: {N_CH} channels x {N_MS} ms after the parse call",
+        "workload": f"position_fixes_device: {n_ch} channels x {N_MS} ms after the parse call, {args.solver} solver",
         "gpu": dev.name, "power_limit": power_limit(),
         "fix_call_ms_median": float(np.median(fix_ms)), "fix_call_ms": fix_ms,
         "kernel_ms_profiled": kernel_ms,

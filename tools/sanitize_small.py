@@ -60,6 +60,15 @@ for n, m in ((2046, 2), (4092, 1)):
         sub = t.decode_subframes(sbd.data_ptr(), [nb, nb - 100], nb)
         assert t.subframe_state(0)["processed_bit_count"] >= 600 and len(sub) == 2
         t.close()
+        # the least-squares fix: a second tracker on the same IQ and chain, in that mode
+        t = _native.Tracker(eng, [24, 6], [1500.0, -100.0], [0.0, 0.0], [777, 5])
+        t.set_fix_solver("least_squares")
+        t.process(12, ts)
+        t.integrate_bits(12, ts, ts + 0.001)
+        t.decode_subframes()
+        t.parse_subframes()
+        assert t.position_fixes(ts).shape == (12,)
+        t.close()
         # pipelined batch stream: three streams, pageable staging
         gs = _native.GridStream(eng, 2, 1, [24, 0, 5], dop, _native.NON_COHERENT, depth=2)
         xb = o.synth_iq(2, n, 2, fs, [(25, 1500.0, 777, 0.3, 0.3)])
