@@ -64,16 +64,17 @@ __host__ __device__ constexpr int spec_warps(int s) { return 2 * s >= 8 ? 8 : 2 
 constexpr int kCarrierTable = 64;  // >= ceil(N / threads) for every supported rate
 
 // When every (branch, parity) task has its own warp (2S <= 8) the transpose tiles take the place of the polyphase rows,
-// which are dead once every warp holds its vector in registers: 35 KB instead of 52 KB per 2.046 Msps CTA and, with the
-// register cap of five CTAs per SM, the 1312 units of a 32-block batch run in two waves instead of three.
+// which are dead once every warp holds its vector in registers: 35 KB instead of 52 KB per 2.046 Msps CTA.
 __host__ __device__ constexpr bool spec_alias(int s) { return 2 * s <= 8; }
 __host__ __device__ constexpr int spec_f2(int s) {  // float2 of rows + tiles
     return spec_alias(s) ? (s * kFft > spec_warps(s) * kTileF2 ? s * kFft : spec_warps(s) * kTileF2)
                          : s * kFft + spec_warps(s) * kTileF2;
 }
 
+// 2.046 Msps: a register cap of four CTAs per SM (128 registers).  The cap of five (96 registers) spilled 216 B per thread, and
+// the benchmark's 256-block launch took 0.214 ms against 0.168 ms at four (H100, DESIGN.md section 4).
 template <int S>
-__global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 5 : 1) k_doppler_spectra(const SpectraArgs a) {
+__global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_spectra(const SpectraArgs a) {
     constexpr int kSpecWarps = spec_warps(S);
     constexpr int kSpecThreads = kSpecWarps * 32;
     extern __shared__ __align__(16) float2 smem[];
@@ -379,7 +380,8 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
     constexpr int kCrepOdd = kFft;
     float2* crep_s = smem;              // [2][1024]
     float2* tw1_s = crep_s + 2 * kFft;  // [32][32]
-    float2* tiles = tw1_s + kFft;       // [NW][kTile64F2]
+    float2* tw1o_s = tw1_s + kFft;      // [16][32] odd-parity products, k1 >= 16
+    float2* tiles = tw1o_s + kFft / 2;  // [NW][kTile64F2]
     PeakPartial* partial = reinterpret_cast<PeakPartial*>(tiles + NW * kTile64F2);  // [NW]
     uint64_t* mbar = reinterpret_cast<uint64_t*>(partial + NW);
 
@@ -395,6 +397,8 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
     }
     mbar_wait(mbar, parity);
     parity ^= 1;
+    if (warp == 0) w2048_odd_twiddles(lane, tw1_s, tw1o_s);
+    __syncthreads();
     asm volatile("griddepcontrol.wait;" ::: "memory");  // PDL against doppler_spectra, see launch_correlate
 
     const int cells_per_group = NW / a.rsplit;
@@ -464,27 +468,25 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
                     {
                         float2 hx[32];
                         load_mul_vec(hx, lane, p + kFft, crep_s + kFft);  // odd bins
-                        w2048_phase1<1>(hx, lane, tw1_s, tile);
+                        w2048_phase1_odd(hx, lane, tw1_s, tw1o_s, tile);
                     }
                     __syncwarp();
                     float2 x[64];
                     w2048_phase2(x, lane, tile);
                     __syncwarp();  // the tile may be overwritten by the next transform
 #pragma unroll
-                    for (int k = 0; k < 32; ++k) acc[k] += gb_mag(x[k]);
+                    for (int k = 0; k < 32; ++k) {
+                        if (SINGLE_MS) acc[k] = gb_mag(x[k]);  // = 0 + |x|: magnitudes are never -0
+                        else acc[k] += gb_mag(x[k]);
+                    }
                 }
-                // lags q = lane + 32 k: k < 16 and k >= 16 are the two halves thread_peak16 knows as h = 0 / 1
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    float v[16];
-#pragma unroll
-                    for (int jj = 0; jj < 16; ++jj) v[jj] = acc[16 * hh + jj];
-                    Peak t;
-                    float fsum;
-                    thread_peak16(v, lane, hh, a.s, r, t, fsum);
-                    t.sum = static_cast<double>(fsum);
-                    peak_merge(pk, t);
-                }
+                // lags q = lane + 32 k; the two float sums are added in the order of thread_peak16's halves
+                Peak t;
+                float fsum[2];
+                thread_peak32(acc, lane, a.s, r, t, fsum);
+                t.sum = static_cast<double>(fsum[0]);
+                peak_merge(pk, t);
+                pk.sum += static_cast<double>(fsum[1]);
             }
             warp_reduce_peak(pk);
             if (lane == 0) {
@@ -699,7 +701,7 @@ size_t correlate_smem_bytes() {
 }
 
 size_t correlate_w2048_smem_bytes(int nw) {
-    return (3 * static_cast<size_t>(kFft) + static_cast<size_t>(nw) * kTile64F2) * sizeof(float2) +
+    return (3 * static_cast<size_t>(kFft) + kFft / 2 + static_cast<size_t>(nw) * kTile64F2) * sizeof(float2) +
            nw * sizeof(PeakPartial) + 16;
 }
 

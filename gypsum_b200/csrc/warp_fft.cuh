@@ -254,6 +254,37 @@ GB_HD GB_INLINE void thread_peak16(const float (&v)[16], int lane, int h, int s,
     fsum = sm;
 }
 
+// One thread's 32 finished lags q = lane + 32 k of a whole transform at once (one-warp kernel): the (max, first index of max,
+// count of max) of both thread_peak16 halves merged, from a bit mask of the lags equal to the max instead of a running first
+// index and count.  fsum[h] is thread_peak16's sum of half h, added in the same order, so the record's float64 sum is unchanged.
+GB_HD GB_INLINE void thread_peak32(const float (&v)[32], int lane, int s, int r, Peak& out, float (&fsum)[2]) {
+    const bool last_invalid = lane == 31;  // lag 1023
+    const float v31 = last_invalid ? -1.0f : v[31];
+    float m = v[0], s0 = v[0], s1 = v[16];
+#pragma unroll
+    for (int k = 1; k < 31; ++k) m = fmaxf(m, v[k]);
+    m = fmaxf(m, v31);
+#pragma unroll
+    for (int k = 1; k < 16; ++k) s0 += v[k];
+#pragma unroll
+    for (int k = 17; k < 31; ++k) s1 += v[k];
+    s1 += last_invalid ? 0.0f : v[31];
+    unsigned eq = v31 == m ? 1u << 31 : 0u;
+#pragma unroll
+    for (int k = 0; k < 31; ++k) eq |= v[k] == m ? 1u << k : 0u;
+#if defined(__CUDA_ARCH__)
+    const int first = __ffs(eq) - 1, c = __popc(eq);
+#else
+    const int first = eq ? __builtin_ctz(eq) : -1, c = __builtin_popcount(eq);
+#endif
+    out.mx = m;
+    out.idx = s * (lane + 32 * first) + r;
+    out.cnt = c;
+    out.sum = 0.0;
+    fsum[0] = s0;
+    fsum[1] = s1;
+}
+
 }  // namespace gb
 
 namespace gb {
@@ -332,6 +363,36 @@ GB_HD GB_INLINE void w2048_phase1(float2 (&x)[32], int lane, const float2* tw1, 
             if (k1 == 0 && H == 0) row[0] = x[0];
             else row[k1] = cmulc(x[k1], w);
         }
+    }
+}
+
+// The odd-parity twiddle product tw1[k1][lane] * W2048^k1 of w2048_phase1<1> depends on (k1, lane) only.  For k1 = 16..31
+// a CTA forms it once into tw1o[pidx(k1 - 16, lane)] (4 KB: what shared memory has left beside 12 tiles), with the same
+// complex product, so w2048_phase1_odd reads the same values w2048_phase1<1> computes on every transform.
+GB_HD GB_INLINE void w2048_odd_twiddles(int lane, const float2* tw1, float2* tw1o) {
+    constexpr float kW[32][2] = {GB_W2048_TABLE};
+#pragma unroll
+    for (int k1 = 16; k1 < 32; ++k1) tw1o[pidx(k1 - 16, lane)] = cmul(tw1[pidx(k1, lane)], make_float2(kW[k1][0], kW[k1][1]));
+}
+
+// w2048_phase1<1> with the products for k1 >= 16 read from w2048_odd_twiddles' table: bit-identical results, 64 fewer FP32
+// instructions per transform.
+GB_HD GB_INLINE void w2048_phase1_odd(float2 (&x)[32], int lane, const float2* tw1, const float2* tw1o, float2* tile) {
+    constexpr float kW[32][2] = {GB_W2048_TABLE};
+    fft32_inv(x);
+    float2* row = tile + (32 + lane) * kT64Stride;  // physical row of l' = 2*lane + 1
+#pragma unroll
+    for (int kp = 0; kp < 16; ++kp) {
+        float2 w0, w1;
+        if (kp < 8) {
+            ld_pair(tw1 + 2 * (kp * 32 + lane), w0, w1);
+            w0 = cmul(w0, make_float2(kW[2 * kp][0], kW[2 * kp][1]));
+            w1 = cmul(w1, make_float2(kW[2 * kp + 1][0], kW[2 * kp + 1][1]));
+        } else {
+            ld_pair(tw1o + 2 * ((kp - 8) * 32 + lane), w0, w1);
+        }
+        row[2 * kp] = cmulc(x[2 * kp], w0);
+        row[2 * kp + 1] = cmulc(x[2 * kp + 1], w1);
     }
 }
 
