@@ -8,20 +8,19 @@ import subprocess
 import numpy as np
 import pytest
 
+from fix_support import BIAS_S, POS_M, fix_emulator, slide_tol
+from hostbuild import host_library
 from oracle import fix_oracle as fx
 from oracle import orbit_oracle as orb
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "fix.npz")
 TIMELINES = ["realistic", "three", "gate", "lost", "five", "raise"]
-# parity bounds of the host and device core against the reference's numpy (DESIGN.md §6), a small multiple of the
-# spread measured on the recorded timelines (clock bias 1.2e-15 s, position 2.7e-7 m, slides identical)
-POS_M, BIAS_S, SLIDE_ULPS = 2e-6, 1e-14, 4
 
 
 def slide_close(a, b) -> bool:
     """Slides (about 3e5 s here) within SLIDE_ULPS units in the last place."""
-    return abs(a - b) <= SLIDE_ULPS * 2.0 ** -52 * abs(b)
+    return abs(a - b) <= slide_tol(b)
 
 
 @pytest.fixture(scope="module")
@@ -30,22 +29,8 @@ def golden():
 
 
 @pytest.fixture(scope="module")
-def fix_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "fix_emu.cu")
-    out = str(tmp_path_factory.mktemp("fix_emu") / "libfixemu.so")
-    subprocess.run(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", out, src], check=True,
-                   capture_output=True)
-    lib = C.CDLL(out)
-    lib.fix_emu_compute.restype = C.c_int
-    lib.fix_emu_compute.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_void_p]
-    return lib
-
-
-def emu_compute(lib, rows, rx, slide):
-    r = np.ascontiguousarray(rows, dtype=np.float64).reshape(4, 4)
-    out = np.zeros(1, dtype=fx.FIX_DTYPE)
-    lib.fix_emu_compute(r.ctypes.data, float(rx), float(slide), out.ctypes.data)
-    return out[0]
+def fix_emu():
+    return fix_emulator()
 
 
 def oracle_timeline(z, name):
@@ -97,7 +82,7 @@ def test_golden_covers_every_case(golden):
     assert s[5] == orb.parse(tuple(int(w) for w in z["realistic_words"][last]))["tow_seconds"] - ev[last, 5]
 
 
-def _emu_chain(lib, recs, rows):
+def _emu_chain(compute, recs, rows):
     """The host core along the oracle's chain: each fix from the slide the core's previous fix left, or from the
     oracle's slide where a reset set it.  Slides and pseudoranges within SLIDE_ULPS; returns the largest clock-bias
     (s) and position (m) differences."""
@@ -107,12 +92,11 @@ def _emu_chain(lib, recs, rows):
         for m in np.flatnonzero(rec["status"] == fx.FIX_SOLVED):
             r = rec[m]
             s = r["slide_in"] if prev_oracle is None or r["slide_in"] != prev_oracle else prev_emu
-            got = emu_compute(lib, rows[(c, m)], r["receiver_timestamp"], s)
+            got = compute(rows[(c, m)], r["receiver_timestamp"], s)
             assert got["status"] == fx.FIX_SOLVED
             assert slide_close(got["slide_in"], r["slide_in"]) and slide_close(got["slide_out"], r["slide_out"])
             # round 0's pseudoranges: (slide + receiver_timestamp) - tow, differences of numbers of the slide's size
-            tol = SLIDE_ULPS * 2.0 ** -52 * abs(r["slide_in"])
-            assert np.abs(got["pseudorange"] - r["pseudorange"]).max() <= tol
+            assert np.abs(got["pseudorange"] - r["pseudorange"]).max() <= slide_tol(r["slide_in"])
             worst_t = max(worst_t, abs(got["clock_bias"] - r["clock_bias"]))
             worst_m = max(worst_m, *(abs(got[k] - r[k]) for k in "xyz"))
             prev_oracle, prev_emu = r["slide_out"], got["slide_out"]
@@ -156,7 +140,7 @@ def test_solver_recovers_a_planted_position(fix_emu):
         for _, x, y, z in sats:
             rng_ = np.sqrt((pos[0] - x) ** 2 + (pos[1] - y) ** 2 + (pos[2] - z) ** 2)
             rows.append(((slide + rx) - (rng_ / fx.SPEED_OF_LIGHT + bias), x, y, z))
-        got = emu_compute(fix_emu, rows, rx, slide)
+        got = fix_emu(rows, rx, slide)
         assert got["status"] == fx.FIX_SOLVED
         err = max(abs(got[k] - p) for k, p in zip("xyz", pos))
         worst = max(worst, err)
@@ -180,8 +164,8 @@ def test_fix_from_the_segment_slide_equals_the_chained_fix(golden, fix_emu, name
             r = rec[m]
             if prev_out is None or r["slide_in"] != prev_out:
                 base = r["slide_in"]  # a reset set the slide here
-            a = emu_compute(fix_emu, rows[(c, m)], r["receiver_timestamp"], base)
-            b = emu_compute(fix_emu, rows[(c, m)], r["receiver_timestamp"], r["slide_in"])
+            a = fix_emu(rows[(c, m)], r["receiver_timestamp"], base)
+            b = fix_emu(rows[(c, m)], r["receiver_timestamp"], r["slide_in"])
             assert a["slide_out"] == b["slide_out"]  # what the device's chain check (fix_same_slide) relies on
             worst_t = max(worst_t, abs(a["clock_bias"] - b["clock_bias"]))
             worst_m = max(worst_m, *(abs(a[k] - b[k]) for k in "xyz"))
@@ -207,8 +191,8 @@ def test_fix_against_its_entering_slide(golden, fix_emu, name):
     for d in (1e-9, 3e-8, 1e-6, 1e-3, 0.01, 0.03, 0.05, 0.07, 0.1):
         worst_s = worst_t = worst_m = 0.0
         for rows_, rx, s in cases:
-            base = emu_compute(fix_emu, rows_, rx, s)
-            got = emu_compute(fix_emu, rows_, rx, s + d)
+            base = fix_emu(rows_, rx, s)
+            got = fix_emu(rows_, rx, s + d)
             worst_s = max(worst_s, abs(got["slide_out"] - base["slide_out"]))
             worst_t = max(worst_t, abs(got["clock_bias"] - base["clock_bias"]))
             worst_m = max(worst_m, *(abs(got[k] - base[k]) for k in "xyz"))
@@ -226,7 +210,7 @@ def test_fix_against_its_entering_slide(golden, fix_emu, name):
             assert ws == 0.0 and wt <= BIAS_S and wm <= POS_M, d
 
 
-def test_layout_python_c_and_cpp(fix_emu, tmp_path):
+def test_layout_python_c_and_cpp(tmp_path):
     from gypsum_b200._native import FIX_DTYPE
 
     names = ["receiver_timestamp", "slide_in", "slide_out", "clock_bias", "x", "y", "z", "pseudorange", "status", "n_ready",
@@ -235,7 +219,7 @@ def test_layout_python_c_and_cpp(fix_emu, tmp_path):
     assert py == [0, 8, 16, 24, 32, 40, 48, 56, 88, 92, 96, 112]
     assert fx.FIX_DTYPE == FIX_DTYPE
     cpp = np.zeros(12, dtype=np.int64)
-    fix_emu.fix_emu_layout(cpp.ctypes.data_as(C.c_void_p))
+    host_library("fix_emu").fix_emu_layout(cpp.ctypes.data_as(C.c_void_p))
     assert list(cpp) == py
     src = tmp_path / "layout.c"
     src.write_text("#include <stdio.h>\n#include <stddef.h>\n#include \"gypsum_b200.h\"\nint main(void) {\n"

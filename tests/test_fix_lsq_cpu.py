@@ -1,68 +1,27 @@
 """The position fix's least-squares mode on the CPU: fix_core.cuh's least-squares solve compiled for the host
-(tests/emu/fix_lsq_emu.cu) on exact pseudoranges from a planted position with 5 to 12 satellites, against the
+(tests/emu/fix_emu.cu) on exact pseudoranges from a planted position with 5 to 12 satellites, against the
 least-squares oracle (tests/fix_lsq_oracle.py, np.linalg.lstsq) on perturbed rows and on the five-ready golden timelines,
 the four-row case against the reference mode, and the rank-deficient raise."""
-import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import fix_lsq_oracle as lo
+from fix_support import BIAS_S, MANY_BIAS_S, MANY_POS_M, MANY_SLIDE_ULPS, POS_M, fix_emulator, slide_tol
 from oracle import fix_oracle as fx
 from oracle import orbit_oracle as orb
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-# the bounds of tests/test_fix_cpu.py (DESIGN.md §6)
-POS_M, BIAS_S = 2e-6, 1e-14
 # least squares against numpy's SVD where Gauss-Newton has converged (perturbed rows: numpy's last step below 1e-6 m),
 # a small multiple of the measured spread (DESIGN.md §8c: position 2.4e-5 m with 5 rows, 4.4e-9 m with 6 to 12; clock
 # bias 3.8e-14 s; slide 0 ulp)
 LSQ_POS_M, LSQ_BIAS_S, LSQ_SLIDE_ULPS = 1e-4, 2e-13, 4
-# five or more rows on the recorded and scripted timelines (DESIGN.md §8c).  The golden rows are 1e4 km off any common
-# solution, and Gauss-Newton on the squared ranges does not converge there (numpy's last step is up to 1.4e7 m in
-# `five`): host and numpy follow the same cycle apart by rounding, measured up to 1.3 m, 2.7e-9 s and 34 ulp of the
-# slide.  tests/test_gpu_fix_lsq.py's scripted six rows converge, on a poorer geometry: 5.6e-4 m, 6.1e-13 s, 0 ulp.
-MANY_POS_M, MANY_BIAS_S, MANY_SLIDE_ULPS = 4.0, 1e-8, 100
 
 
 @pytest.fixture(scope="module")
-def lsq_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "fix_lsq_emu.cu")
-    out = str(tmp_path_factory.mktemp("fix_lsq_emu") / "libfixlsqemu.so")
-    subprocess.run(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", out, src], check=True,
-                   capture_output=True)
-    lib = C.CDLL(out)
-    lib.fix_emu_compute_n.restype = C.c_int
-    lib.fix_emu_compute_n.argtypes = [C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p]
-
-    def compute(rows, rx, slide):
-        r = np.ascontiguousarray(rows, dtype=np.float64).reshape(-1, 4)
-        out = np.zeros(1, dtype=fx.FIX_DTYPE)
-        lib.fix_emu_compute_n(r.ctypes.data, len(r), float(rx), float(slide), out.ctypes.data)
-        return out[0]
-
-    return compute
-
-
-@pytest.fixture(scope="module")
-def ref_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "fix_emu.cu")
-    out = str(tmp_path_factory.mktemp("fix_emu") / "libfixemu.so")
-    subprocess.run(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", out, src], check=True,
-                   capture_output=True)
-    lib = C.CDLL(out)
-    lib.fix_emu_compute.restype = C.c_int
-    lib.fix_emu_compute.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_void_p]
-
-    def compute(rows, rx, slide):
-        r = np.ascontiguousarray(rows, dtype=np.float64).reshape(4, 4)
-        out = np.zeros(1, dtype=fx.FIX_DTYPE)
-        lib.fix_emu_compute(r.ctypes.data, float(rx), float(slide), out.ctypes.data)
-        return out[0]
-
-    return compute
+def lsq_emu():
+    return fix_emulator()
 
 
 def satellites(seed, n):
@@ -169,9 +128,10 @@ def test_golden_five_ready_against_numpy(lsq_emu, name):
 
 
 @pytest.mark.parametrize("name", ["realistic", "lost", "five"])
-def test_four_rows_are_the_reference_fix(lsq_emu, ref_emu, name):
-    """Four ready rows take the reference mode's code path: the record is byte-identical, and the oracle's
-    least-squares mode equals the reference oracle bit for bit up to the first five-ready millisecond."""
+def test_four_rows_are_the_reference_fix(lsq_emu, name):
+    """Four ready rows take the reference mode's code path: the host core's record is the reference oracle's within the
+    reference mode's bounds, and the oracle's least-squares mode equals the reference oracle bit for bit up to the
+    first five-ready millisecond."""
     z = np.load(os.path.join(ROOT, "tests", "golden", "fix.npz"))
     ref = ls = None
     n = 0
@@ -184,8 +144,12 @@ def test_four_rows_are_the_reference_fix(lsq_emu, ref_emu, name):
         assert a[:end].tobytes() == b[:end].tobytes()
         for m in np.flatnonzero(b["status"] == fx.FIX_SOLVED):
             if b[m]["n_ready"] == 4:
-                got, want = lsq_emu(ls.rows[m], rx[m], b[m]["slide_in"]), ref_emu(ls.rows[m], rx[m], b[m]["slide_in"])
-                assert got.tobytes() == want.tobytes(), m
+                got, want = lsq_emu(ls.rows[m], rx[m], b[m]["slide_in"]), a[m]
+                assert got["status"] == want["status"] and got["slide_in"] == want["slide_in"], m
+                assert abs(got["slide_out"] - want["slide_out"]) <= slide_tol(want["slide_out"]), m
+                assert np.abs(got["pseudorange"] - want["pseudorange"]).max() <= slide_tol(want["slide_in"]), m
+                assert abs(got["clock_bias"] - want["clock_bias"]) <= BIAS_S, m
+                assert max(abs(got[k] - want[k]) for k in "xyz") <= POS_M, m
                 n += 1
         if len(five):
             break

@@ -4,13 +4,12 @@ the segment's reset slide (the device's pass 1) on the other root of the squared
 stays on its own, so the device's chain check misses and k_fix_repair runs (DESIGN.md §8c).  fx.device_passes models the
 device's passes over the host core (fix_core.cuh compiled for the host): it predicts the first miss and the fixes the
 repair recomputes, and shows on the CPU that every gap timeline needs the repair."""
-import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from fix_support import BIAS_S, POS_M, fix_emulator, slide_tol
 from oracle import fix_oracle as fx
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -26,12 +25,6 @@ MISSES = {
     "gap_five": (0, 350, [49, 0]),  # 351-399; the LinAlgError at 400 is a reset millisecond
     "gap_raise": (0, 400, [99, 0]),  # 401-499; the decoder raise stops the receiver at 500
 }
-# DESIGN.md §6: the bounds of tests/test_fix_cpu.py
-POS_M, BIAS_S, SLIDE_ULPS = 2e-6, 1e-14, 4
-
-
-def slide_tol(s):
-    return SLIDE_ULPS * 2.0 ** -52 * np.abs(s)
 
 
 @pytest.fixture(scope="module")
@@ -40,22 +33,8 @@ def golden():
 
 
 @pytest.fixture(scope="module")
-def fix_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "fix_emu.cu")
-    out = str(tmp_path_factory.mktemp("fix_emu") / "libfixemu.so")
-    subprocess.run(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", out, src], check=True,
-                   capture_output=True)
-    lib = C.CDLL(out)
-    lib.fix_emu_compute.restype = C.c_int
-    lib.fix_emu_compute.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_void_p]
-
-    def compute(rows, rx, slide):
-        r = np.ascontiguousarray(rows, dtype=np.float64).reshape(4, 4)
-        out = np.zeros(1, dtype=fx.FIX_DTYPE)
-        lib.fix_emu_compute(r.ctypes.data, float(rx), float(slide), out.ctypes.data)
-        return out[0]
-
-    return compute
+def fix_emu():
+    return fix_emulator()
 
 
 def model_timeline(z, name, compute):

@@ -1,15 +1,14 @@
 """GPU parity of the position-fix kernels (fix.cu through gb200_tracker_position_fixes) against timelines recorded from
 the live reference's GpsWorldModel (tests/golden/fix.npz) and the oracle, and end to end behind the tracking, bit,
 subframe and orbit kernels on 60 s of IQ that carries four consistent planted ephemerides."""
-import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from fix_support import BIAS_S, POS_M, fix_emulator, parse_events, rows_at, run_golden, slide_tol
+from gpu_support import make_engine
 from oracle import fix_oracle as fx
-from oracle import gypsum_oracle as o
 from oracle import nav_oracle as nav
 from oracle import orbit_oracle as orb
 from oracle import tracker_oracle as t
@@ -19,60 +18,18 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "fix.npz")
 TIMELINES = ["realistic", "three", "gate", "lost", "five", "raise"]
 N, FS = 2046, 2046000
-# DESIGN.md §6: a small multiple of the spread measured on the recorded timelines
-POS_M, BIAS_S, SLIDE_ULPS = 2e-6, 1e-14, 4
-
-
-def slide_tol(s):
-    return SLIDE_ULPS * 2.0 ** -52 * np.abs(s)
 
 
 @pytest.fixture(scope="module")
 def engine(native_lib):
-    from gypsum_b200 import _native
-
-    e = _native.Engine(FS, N)
-    e.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
+    e = make_engine(FS, N)
     yield e
     e.close()
 
 
 @pytest.fixture(scope="module")
-def fix_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "fix_emu.cu")
-    out = str(tmp_path_factory.mktemp("fix_emu") / "libfixemu.so")
-    subprocess.run(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", out, src], check=True,
-                   capture_output=True)
-    lib = C.CDLL(out)
-    lib.fix_emu_compute.restype = C.c_int
-    lib.fix_emu_compute.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_void_p]
-    return lib
-
-
-def _emu(lib, rows, rx, slide):
-    r = np.ascontiguousarray(rows, dtype=np.float64).reshape(4, 4)
-    out = np.zeros(1, dtype=fx.FIX_DTYPE)
-    lib.fix_emu_compute(r.ctypes.data, float(rx), float(slide), out.ctypes.data)
-    return out[0]
-
-
-def _parse(trk, chans, n_ms):
-    """chans: [(events [(kind, words, trailing_edge, ms)], drop_ms)] through device event arrays."""
-    import torch
-
-    from gypsum_b200._native import SUBFRAME_DTYPE
-
-    n_ch = len(chans)
-    stride = max(1, max(len(ev) for ev, _ in chans))
-    host = np.zeros((n_ch, stride), dtype=SUBFRAME_DTYPE)
-    ems = np.zeros((n_ch, stride), dtype=np.int32)
-    counts = np.array([len(ev) for ev, _ in chans], dtype=np.int32)
-    for c, (events, _) in enumerate(chans):
-        for j, (kind, w, te, m) in enumerate(events):
-            host[c, j]["kind"], host[c, j]["words"], host[c, j]["trailing_edge_receiver_timestamp"] = kind, w, te
-            ems[c, j] = m
-    dev = torch.from_numpy(host.view(np.uint8).reshape(n_ch, -1)).cuda()
-    trk.parse_subframes(dev.data_ptr(), counts, stride, ems, np.array([d for _, d in chans], dtype=np.int32), n_ms)
+def fix_emu():
+    return fix_emulator()
 
 
 def _compare(got, want):
@@ -100,47 +57,22 @@ def _compare(got, want):
     return worst
 
 
-def _run_golden(engine, name, device_out=False):
-    import torch
-
-    from gypsum_b200 import _native
-
-    z = np.load(GOLDEN)
-    calls = fx.golden_calls(z, name)
-    n_ch = len(calls[0][1])
-    trk = _native.Tracker(engine, list(range(n_ch)), [0.0] * n_ch, [0.0] * n_ch, [0] * n_ch)
-    recs, obs = [], []
-    for rx, chans in calls:
-        _parse(trk, chans, len(rx))
-        if device_out:
-            dev = torch.empty(len(rx) * _native.FIX_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
-            trk.position_fixes_device(rx, dev.data_ptr())
-            torch.cuda.synchronize()
-            recs.append(dev.cpu().numpy().view(_native.FIX_DTYPE).copy())
-        else:
-            recs.append(trk.position_fixes(rx))
-        obs.append(trk.observations())
-    return trk, calls, recs, obs
-
-
 @pytest.mark.parametrize("name", TIMELINES)
 def test_golden_timelines_on_the_device(engine, fix_emu, name):
     """The recorded timelines through the kernels, receiver state carried across calls: status, ready count and rows
     exact, slides and solution within the bounds of the oracle's chain; every record equals the host core's fix from
     the record's own slide_in bit for bit; the chain relation holds (slide_in exact at a reset, else within 4 ulp of
     the previous fix's slide_out)."""
-    z = np.load(GOLDEN)
-    trk, calls, recs, obs = _run_golden(engine, name)
+    z, calls, out = run_golden(engine, GOLDEN, name)
     rcv = fx.ReceiverOracle(len(calls[0][1]))
     worst = [0.0, 0.0, 0.0]
-    for c, ((rx, chans), got) in enumerate(zip(calls, recs)):
+    for c, ((rx, chans), (got, obs, _)) in enumerate(zip(calls, out)):
         want = rcv.call(chans, rx)
         assert np.array_equal(got["status"], fx.golden_fix_rows(z, name, c)[:, 3].astype(int))
         worst = [max(a, b) for a, b in zip(worst, _compare(got, want))]
         for m in np.flatnonzero(got["status"] == fx.FIX_SOLVED):
             r = got[m]
-            rows = [(obs[c][ch, m]["tow"], obs[c][ch, m]["x"], obs[c][ch, m]["y"], obs[c][ch, m]["z"]) for ch in r["channel"]]
-            host = _emu(fix_emu, rows, r["receiver_timestamp"], r["slide_in"])
+            host = fix_emu(rows_at(obs, r["channel"], m), r["receiver_timestamp"], r["slide_in"])
             # the numbers (slides, solution, pseudoranges) and the status; the rows are the plan's
             assert host.tobytes()[:88] == r.tobytes()[:88] and host["status"] == r["status"], m
         # at a reset millisecond the slide is the reset value exactly; elsewhere it continues the chain
@@ -150,18 +82,17 @@ def test_golden_timelines_on_the_device(engine, fix_emu, name):
                 assert abs(got[b]["slide_in"] - got[a]["slide_out"]) <= slide_tol(got[a]["slide_out"])
             else:
                 assert got[b]["slide_in"] == want[b]["slide_in"]
-    st = trk.receiver_state()
+    st = out[-1][2]
     assert st["order"] == rcv.order and st["stopped"] == rcv.stopped and st["repaired"] == 0
     if rcv.slide is not None:
         assert abs(st["slide"] - rcv.slide) <= slide_tol(rcv.slide)
     print(f"{name}: worst slide / pseudorange {worst[0]:.3g} s, clock bias {worst[1]:.3g} s, position {worst[2]:.3g} m")
-    trk.close()
 
 
 def test_fixes_device_matches_host(engine):
-    _, _, host, _ = _run_golden(engine, "lost")
-    _, _, dev, _ = _run_golden(engine, "lost", device_out=True)
-    for a, b in zip(host, dev):
+    _, _, host = run_golden(engine, GOLDEN, "lost")
+    _, _, dev = run_golden(engine, GOLDEN, "lost", device_out=True)
+    for (a, _, _), (b, _, _) in zip(host, dev):
         assert a.tobytes() == b.tobytes()
 
 
@@ -175,21 +106,21 @@ def test_state_errors(engine):
         trk.position_fixes([])
     assert trk.receiver_state() == {"slide": None, "stopped": False, "order": [], "repaired": 0}
     rx, chans = calls[0]
-    _parse(trk, chans, len(rx))
+    parse_events(trk, chans, len(rx))
     with pytest.raises(ValueError, match="one start time per millisecond"):
         trk.position_fixes(rx[:-1])
     trk.position_fixes(rx)
     with pytest.raises(RuntimeError, match="already computed"):
         trk.position_fixes(rx)
-    _parse(trk, [([], -1)] * 4, 10)
-    _parse(trk, [([], -1)] * 4, 10)  # the fixes of the call before were skipped
+    parse_events(trk, [([], -1)] * 4, 10)
+    parse_events(trk, [([], -1)] * 4, 10)  # the fixes of the call before were skipped
     with pytest.raises(RuntimeError, match="gap"):
         trk.position_fixes(np.arange(10) * 0.001)
     trk.close()
     # parse calls before the first fix call may go without fixes
     trk = _native.Tracker(engine, [0, 1, 2, 3], [0.0] * 4, [0.0] * 4, [0] * 4)
-    _parse(trk, [([], -1)] * 4, 10)
-    _parse(trk, [([], -1)] * 4, 10)
+    parse_events(trk, [([], -1)] * 4, 10)
+    parse_events(trk, [([], -1)] * 4, 10)
     assert (trk.position_fixes(np.arange(10) * 0.001)["status"] == fx.FIX_NONE).all()
     trk.close()
 

@@ -1,19 +1,19 @@
 """The position fix's least-squares mode on the device (fix.cu through gb200_tracker_position_fixes after
 gb200_tracker_set_fix_solver): the golden timelines, a scripted timeline of six channels whose ready set goes from 6 to 5
 to 4 inside one segment, returns, and takes a receiver-clock jump, and 60 s of IQ through TrackerBank.  Against the
-least-squares oracle (tests/fix_lsq_oracle.py) within the bounds of tests/test_fix_lsq_cpu.py, against the model of the
+least-squares oracle (tests/fix_lsq_oracle.py) within the bounds of tests/fix_support.py, against the model of the
 passes (every record bit for bit, and the repair count), and against the reference mode up to the first five-ready
 millisecond (byte for byte)."""
-import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import fix_lsq_oracle as lo
+from fix_support import (BIAS_S, MANY_BIAS_S, MANY_POS_M, MANY_SLIDE_ULPS, POS_M, SLIDE_ULPS, fix_emulator, parse_events,
+                         run_calls)
+from gpu_support import make_engine
 from oracle import fix_oracle as fx
-from oracle import gypsum_oracle as o
 from oracle import nav_oracle as nav
 from oracle import orbit_oracle as orb
 from oracle import tracker_oracle as t
@@ -21,60 +21,20 @@ from oracle import tracker_oracle as t
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 N, FS = 2046, 2046000
-# tests/test_fix_lsq_cpu.py: the reference mode's bounds up to the first five-ready millisecond, the MANY_* bounds
-# (five or more rows on the recorded and scripted timelines) from there on
-POS_M, BIAS_S, SLIDE_ULPS = 2e-6, 1e-14, 4
-MANY_POS_M, MANY_BIAS_S, MANY_SLIDE_ULPS = 4.0, 1e-8, 100
 GOLDEN = [("fix", "realistic"), ("fix", "lost"), ("fix", "five"), ("fix", "raise"), ("fix_repair", "gap_five"),
           ("fix_repair", "gap_mid"), ("fix_repair", "singular")]
 
 
 @pytest.fixture(scope="module")
 def engine(native_lib):
-    from gypsum_b200 import _native
-
-    e = _native.Engine(FS, N)
-    e.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
+    e = make_engine(FS, N)
     yield e
     e.close()
 
 
 @pytest.fixture(scope="module")
-def lsq_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "fix_lsq_emu.cu")
-    out = str(tmp_path_factory.mktemp("fix_lsq_emu") / "libfixlsqemu.so")
-    subprocess.run(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", out, src], check=True,
-                   capture_output=True)
-    lib = C.CDLL(out)
-    lib.fix_emu_compute_n.restype = C.c_int
-    lib.fix_emu_compute_n.argtypes = [C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p]
-
-    def compute(rows, rx, slide):
-        r = np.ascontiguousarray(rows, dtype=np.float64).reshape(-1, 4)
-        out = np.zeros(1, dtype=fx.FIX_DTYPE)
-        lib.fix_emu_compute_n(r.ctypes.data, len(r), float(rx), float(slide), out.ctypes.data)
-        return out[0]
-
-    return compute
-
-
-def _parse(trk, chans, n_ms):
-    """chans: [(events [(kind, words, trailing_edge, ms)], drop_ms)] through device event arrays."""
-    import torch
-
-    from gypsum_b200._native import SUBFRAME_DTYPE
-
-    n_ch = len(chans)
-    stride = max(1, max(len(ev) for ev, _ in chans))
-    host = np.zeros((n_ch, stride), dtype=SUBFRAME_DTYPE)
-    ems = np.zeros((n_ch, stride), dtype=np.int32)
-    counts = np.array([len(ev) for ev, _ in chans], dtype=np.int32)
-    for c, (events, _) in enumerate(chans):
-        for j, (kind, w, te, m) in enumerate(events):
-            host[c, j]["kind"], host[c, j]["words"], host[c, j]["trailing_edge_receiver_timestamp"] = kind, w, te
-            ems[c, j] = m
-    dev = torch.from_numpy(host.view(np.uint8).reshape(n_ch, -1)).cuda()
-    trk.parse_subframes(dev.data_ptr(), counts, stride, ems, np.array([d for _, d in chans], dtype=np.int32), n_ms)
+def lsq_emu():
+    return fix_emulator()
 
 
 def scripted_timeline():
@@ -102,21 +62,6 @@ def scripted_timeline():
                    for k, m in sched[ch][c]], drops[c][ch]) for ch in range(len(svs))]
         out.append((rx, chans))
         t0 += 0.001 * n_ms
-    return out
-
-
-def _run(engine, calls, solver):
-    from gypsum_b200 import _native
-
-    n_ch = len(calls[0][1])
-    trk = _native.Tracker(engine, list(range(n_ch)), [0.0] * n_ch, [0.0] * n_ch, [0] * n_ch)
-    trk.set_fix_solver(solver)
-    out = []
-    for rx, chans in calls:
-        _parse(trk, chans, len(rx))
-        rec = trk.position_fixes(rx)
-        out.append((rec, trk.observations(), trk.receiver_state()))
-    trk.close()
     return out
 
 
@@ -182,8 +127,8 @@ def test_golden_timelines_least_squares(engine, lsq_emu, name):
     and `gap_five` the fixes go on past ms 400, where the reference mode stops."""
     z = np.load(os.path.join(ROOT, "tests", "golden", f"{name[0]}.npz"))
     calls = fx.golden_calls(z, name[1])
-    got = _run(engine, calls, "least_squares")
-    ref = _run(engine, calls, "reference")
+    got = run_calls(engine, calls, solver="least_squares")
+    ref = run_calls(engine, calls, solver="reference")
     first5, worst, per_call = _check(calls, got, ref, lsq_emu)
     if name[1] in ("five", "gap_five"):
         assert first5 == (0, 400)
@@ -200,8 +145,8 @@ def test_scripted_six_channels(engine, lsq_emu):
     return with call 1's subframe, and the clock jump in call 1 makes the repair solve six rows.  Checked as the golden
     timelines are."""
     calls = scripted_timeline()
-    got = _run(engine, calls, "least_squares")
-    ref = _run(engine, calls, "reference")
+    got = run_calls(engine, calls, solver="least_squares")
+    ref = run_calls(engine, calls, solver="reference")
     first5, worst, per_call = _check(calls, got, ref, lsq_emu)
     r0, r1 = got[0][0], got[1][0]
     assert first5 == (0, 300)
@@ -224,7 +169,7 @@ def test_fix_solver_errors(engine):
         engine._check(engine._lib.gb200_tracker_set_fix_solver(trk._h, 7), "gb200_tracker_set_fix_solver")
     trk.set_fix_solver("least_squares")
     trk.set_fix_solver("reference")  # as often as wanted before the first fix call
-    _parse(trk, [([], -1)] * 4, 10)
+    parse_events(trk, [([], -1)] * 4, 10)
     trk.position_fixes(np.arange(10) * 0.001)
     with pytest.raises(RuntimeError, match="first fix call"):
         trk.set_fix_solver("least_squares")

@@ -3,104 +3,32 @@ with a receiver-clock jump recorded from the live reference's GpsWorldModel (tes
 them the chain check misses and k_fix_repair runs; fx.device_passes over the host core and the device's own
 observations predicts every record and the repair count exactly (tests/test_fix_repair_cpu.py runs the same model on
 the CPU)."""
-import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from fix_support import BIAS_S, POS_M, fix_emulator, rows_at, run_golden, slide_tol
+from gpu_support import make_engine
 from oracle import fix_oracle as fx
-from oracle import gypsum_oracle as o
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "fix_repair.npz")
 GAPS = ["gap_mid", "gap_two", "gap_back", "gap_first", "gap_carry", "gap_five", "gap_raise"]
 N, FS = 2046, 2046000
-# DESIGN.md §6: the bounds of tests/test_gpu_fix.py
-POS_M, BIAS_S, SLIDE_ULPS = 2e-6, 1e-14, 4
-
-
-def slide_tol(s):
-    return SLIDE_ULPS * 2.0 ** -52 * np.abs(s)
 
 
 @pytest.fixture(scope="module")
 def engine(native_lib):
-    from gypsum_b200 import _native
-
-    e = _native.Engine(FS, N)
-    e.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
+    e = make_engine(FS, N)
     yield e
     e.close()
 
 
 @pytest.fixture(scope="module")
-def fix_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "fix_emu.cu")
-    out = str(tmp_path_factory.mktemp("fix_emu") / "libfixemu.so")
-    subprocess.run(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", out, src], check=True,
-                   capture_output=True)
-    lib = C.CDLL(out)
-    lib.fix_emu_compute.restype = C.c_int
-    lib.fix_emu_compute.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_void_p]
-
-    def compute(rows, rx, slide):
-        r = np.ascontiguousarray(rows, dtype=np.float64).reshape(4, 4)
-        out = np.zeros(1, dtype=fx.FIX_DTYPE)
-        lib.fix_emu_compute(r.ctypes.data, float(rx), float(slide), out.ctypes.data)
-        return out[0]
-
-    return compute
-
-
-def _parse(trk, chans, n_ms):
-    """chans: [(events [(kind, words, trailing_edge, ms)], drop_ms)] through device event arrays."""
-    import torch
-
-    from gypsum_b200._native import SUBFRAME_DTYPE
-
-    n_ch = len(chans)
-    stride = max(1, max(len(ev) for ev, _ in chans))
-    host = np.zeros((n_ch, stride), dtype=SUBFRAME_DTYPE)
-    ems = np.zeros((n_ch, stride), dtype=np.int32)
-    counts = np.array([len(ev) for ev, _ in chans], dtype=np.int32)
-    for c, (events, _) in enumerate(chans):
-        for j, (kind, w, te, m) in enumerate(events):
-            host[c, j]["kind"], host[c, j]["words"], host[c, j]["trailing_edge_receiver_timestamp"] = kind, w, te
-            ems[c, j] = m
-    dev = torch.from_numpy(host.view(np.uint8).reshape(n_ch, -1)).cuda()
-    trk.parse_subframes(dev.data_ptr(), counts, stride, ems, np.array([d for _, d in chans], dtype=np.int32), n_ms)
-
-
-def _run(engine, name, device_out=False):
-    """The timeline call after call; per call the records, the device's observations and receiver_state()."""
-    import torch
-
-    from gypsum_b200 import _native
-
-    z = np.load(GOLDEN)
-    calls = fx.golden_calls(z, name)
-    n_ch = len(calls[0][1])
-    trk = _native.Tracker(engine, list(range(n_ch)), [0.0] * n_ch, [0.0] * n_ch, [0] * n_ch)
-    out = []
-    for rx, chans in calls:
-        _parse(trk, chans, len(rx))
-        if device_out:
-            dev = torch.empty(len(rx) * _native.FIX_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
-            trk.position_fixes_device(rx, dev.data_ptr())
-            torch.cuda.synchronize()
-            rec = dev.cpu().numpy().view(_native.FIX_DTYPE).copy()
-        else:
-            rec = trk.position_fixes(rx)
-        out.append((rec, trk.observations(), trk.receiver_state()))
-    trk.close()
-    return z, calls, out
-
-
-def _rows(obs, channels, m):
-    return [(obs[ch, m]["tow"], obs[ch, m]["x"], obs[ch, m]["y"], obs[ch, m]["z"]) for ch in channels]
+def fix_emu():
+    return fix_emulator()
 
 
 @pytest.mark.parametrize("name", GAPS + ["singular"])
@@ -111,7 +39,7 @@ def test_repair_on_the_device(engine, fix_emu, name):
     the host core's fix from its own slide_in; a fix that does not start a segment starts from the slide the fix
     before it left, exactly where the repair ran and within 4 ulp elsewhere; slide, order and stopped are the
     oracle's."""
-    z, calls, out = _run(engine, name)
+    z, calls, out = run_golden(engine, GOLDEN, name)
     rcv = fx.ReceiverOracle(len(calls[0][1]))
     carried, repaired, worst = None, 0, [0.0, 0.0, 0.0]
     for c, ((rx, chans), (got, obs, state)) in enumerate(zip(calls, out)):
@@ -133,7 +61,7 @@ def test_repair_on_the_device(engine, fix_emu, name):
         assert worst[1] <= BIAS_S and worst[2] <= POS_M, worst
         assert np.isnan(got["x"][got["status"] != fx.FIX_SOLVED]).all()
         # the model of the passes, on the rows the device observed
-        rows = {m: _rows(obs, want[m]["channel"], m) for m in fixing if want[m]["n_ready"] == 4}
+        rows = {m: rows_at(obs, want[m]["channel"], m) for m in fixing if want[m]["n_ready"] == 4}
         model = fx.device_passes(fix_emu, want, rows, rcv.resets, carried)
         carried = model["slide"]
         assert sorted(model["out"]) == list(fixing)
@@ -169,7 +97,7 @@ def test_repair_on_the_device(engine, fix_emu, name):
 
 def test_carried_slide_needs_no_repair(engine):
     """gap_carry repairs to the end of call 0; call 1 continues from the repaired slide and repairs nothing."""
-    _, _, out = _run(engine, "gap_carry")
+    _, _, out = run_golden(engine, GOLDEN, "gap_carry")
     (first, _, s0), (second, _, s1) = out
     assert s0["repaired"] > 0 and s1["repaired"] == s0["repaired"]
     assert (first["status"][-100:] == fx.FIX_SOLVED).all() and second["status"][0] == fx.FIX_SOLVED
@@ -177,7 +105,7 @@ def test_carried_slide_needs_no_repair(engine):
 
 
 def test_gap_five_stops_at_the_raise(engine):
-    z, _, out = _run(engine, "gap_five")
+    z, _, out = run_golden(engine, GOLDEN, "gap_five")
     got, _, state = out[0]
     assert np.flatnonzero(got["status"] == fx.FIX_RAISED).tolist() == [400]
     assert (got["status"][401:] == fx.FIX_STOPPED).all() and (out[1][0]["status"] == fx.FIX_STOPPED).all()
@@ -187,7 +115,7 @@ def test_gap_five_stops_at_the_raise(engine):
 def test_singular_matrix_stops_the_receiver(engine):
     """Two channels with one ephemeris: the device raises at the millisecond the reference raised, with the slide the
     reference kept, and stops."""
-    z, _, out = _run(engine, "singular")
+    z, _, out = run_golden(engine, GOLDEN, "singular")
     want = fx.golden_fix_rows(z, "singular", 0)
     got, _, state = out[0]
     assert np.flatnonzero(got["status"] == fx.FIX_RAISED).tolist() == [300] == np.flatnonzero(want[:, 3] == 2).tolist()
@@ -197,8 +125,8 @@ def test_singular_matrix_stops_the_receiver(engine):
 
 
 def test_fixes_device_matches_host_on_a_repair(engine):
-    _, _, host = _run(engine, "gap_mid")
-    _, _, dev = _run(engine, "gap_mid", device_out=True)
+    _, _, host = run_golden(engine, GOLDEN, "gap_mid")
+    _, _, dev = run_golden(engine, GOLDEN, "gap_mid", device_out=True)
     assert host[0][2]["repaired"] > 0
     for (a, _, _), (b, _, _) in zip(host, dev):
         assert a.tobytes() == b.tobytes()

@@ -7,7 +7,7 @@ import os
 import numpy as np
 import pytest
 
-from oracle import gypsum_oracle as o
+from gpu_support import make_engine
 from oracle import nav_oracle as nav
 from oracle import orbit_oracle as orb
 from oracle import tracker_oracle as t
@@ -21,10 +21,7 @@ N, FS = 2046, 2046000
 
 @pytest.fixture(scope="module")
 def engine(native_lib):
-    from gypsum_b200 import _native
-
-    e = _native.Engine(FS, N)
-    e.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
+    e = make_engine(FS, N)
     yield e
     e.close()
 

@@ -6,7 +6,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from oracle import gypsum_oracle as o
+from gpu_support import make_engine
 
 pytestmark = pytest.mark.gpu
 N, FS = 2046, 2046000
@@ -26,10 +26,7 @@ def _ts(n_ms=CHUNK):
 
 @pytest.fixture(scope="module")
 def engine(native_lib):
-    from gypsum_b200 import _native
-
-    e = _native.Engine(FS, N)
-    e.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
+    e = make_engine(FS, N)
     yield e
     e.close()
 

@@ -9,6 +9,7 @@ import os
 import numpy as np
 import pytest
 
+from gpu_support import make_engine
 from oracle import gypsum_oracle as o
 from oracle import tracker_oracle as t
 
@@ -33,10 +34,7 @@ def load_case(name):
 
 @pytest.fixture(scope="module")
 def engine(native_lib):
-    from gypsum_b200 import _native
-
-    e = _native.Engine(FS, N)
-    e.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
+    e = make_engine(FS, N)
     yield e
     e.close()
 

@@ -8,6 +8,7 @@ import subprocess
 import numpy as np
 import pytest
 
+from hostbuild import host_library
 from oracle import nav_oracle as nav
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -21,12 +22,8 @@ def golden():
 
 
 @pytest.fixture(scope="module")
-def nav_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "nav_emu.cu")
-    out = str(tmp_path_factory.mktemp("nav_emu") / "libnavemu.so")
-    subprocess.run(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", out, src], check=True,
-                   capture_output=True)
-    lib = C.CDLL(out)
+def nav_emu():
+    lib = host_library("nav_emu")
     lib.nav_emu_run.restype = C.c_int
     return lib
 

@@ -8,6 +8,7 @@ import subprocess
 import numpy as np
 import pytest
 
+from hostbuild import host_library
 from oracle import nav_oracle as nav
 from oracle import orbit_oracle as orb
 
@@ -22,12 +23,8 @@ def golden():
 
 
 @pytest.fixture(scope="module")
-def orbit_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "orbit_emu.cu")
-    out = str(tmp_path_factory.mktemp("orbit_emu") / "liborbitemu.so")
-    subprocess.run(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", out, src], check=True,
-                   capture_output=True)
-    lib = C.CDLL(out)
+def orbit_emu():
+    lib = host_library("orbit_emu")
     lib.orbit_emu_call.restype = C.c_int
     return lib
 

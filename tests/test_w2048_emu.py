@@ -2,22 +2,16 @@
 emulator (tests/emu/w2048_emu.cu): each gives bit for bit what the per-transform twiddle product and the two half-transform
 reductions it replaces give, and matches numpy's transform and np.max / np.argmax / count / sum.  No GPU needed."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from hostbuild import host_library
 
 
 @pytest.fixture(scope="module")
-def w2048_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "w2048_emu.cu")
-    out = str(tmp_path_factory.mktemp("w2048_emu") / "libw2048emu.so")
-    subprocess.run(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", out, src], check=True,
-                   capture_output=True)
-    lib = C.CDLL(out)
+def w2048_emu():
+    lib = host_library("w2048_emu")
     lib.emu_ifft2048_odd.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     lib.emu_peak.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int), C.POINTER(C.c_int),
                              C.POINTER(C.c_double)]
