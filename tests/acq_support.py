@@ -1,0 +1,138 @@
+"""What the acquisition test modules share: the tolerances of DESIGN.md section 6, the float64 oracle's grids and searches
+spread over the host's cores (fork pool), and the rules that hold the device's records and searches to them."""
+import multiprocessing as mp
+import os
+
+import numpy as np
+
+from oracle import gypsum_oracle as o
+
+MAG_TOL = 1e-5
+DOP41 = np.arange(-10000.0, 10001.0, 500.0)
+
+
+def rate(s):
+    """(n, fs) at S = s samples per chip."""
+    return 1023 * s, 1023000 * s
+
+
+def mid_branch_lag(s):
+    """A lag in the middle of the code on the middle polyphase branch (branch s // 2)."""
+    return 511 * s + s // 2
+
+
+def _pool(jobs):
+    return mp.get_context("fork").Pool(max(1, min(jobs, os.cpu_count() or 1)))
+
+
+def _cells_worker(args):
+    x, fs, n, svs, dop, kind = args
+    return o.grid_cells(x, fs, n, svs, dop, kind)
+
+
+def oracle_grid(x, fs, n, svs, dop, kind=o.NON_COHERENT):
+    """o.grid_cells over all SVs, one process per SV group."""
+    procs = max(1, min(len(svs), os.cpu_count() or 1))
+    parts = [svs[i::procs] for i in range(procs)]
+    with _pool(procs) as pool:
+        res = pool.map(_cells_worker, [(x, fs, n, p, list(dop), kind) for p in parts])
+    shape = (len(svs), len(dop))
+    peak, arg, total, count = (np.zeros(shape), np.zeros(shape, np.int64), np.zeros(shape), np.zeros(shape, np.int64))
+    for i, (pk, ag, tt, ct) in enumerate(res):
+        rows = list(range(i, len(svs), procs))
+        peak[rows], arg[rows], total[rows], count[rows] = pk, ag, tt, ct
+    return peak, arg, total, count
+
+
+def check_grid(rec, x, fs, n, svs, dop, what, kind=o.NON_COHERENT):
+    """Every record of a (SV x Doppler) grid against the oracle: peak, sum and strength within the tolerance, count exact,
+    argmax exact bar near-ties proved on the float64 profile.  Returns the number of such proofs."""
+    peak, arg, total, count = oracle_grid(x, fs, n, svs, dop, kind)
+    assert rec.shape == peak.shape
+    assert np.abs(rec["peak"] - peak).max() <= MAG_TOL * peak.max(), what
+    assert np.abs(rec["sum"] - total).max() <= MAG_TOL * total.max(), what
+    assert np.array_equal(rec["count"], count), what
+    bad = np.argwhere(rec["argmax"] != arg)
+    for a, b in bad:  # a different index is only acceptable where the float64 profile itself ties to within the tolerance
+        prof = np.abs(o.integrate(kind, x, fs, n, dop[b], o.replica(svs[a], n)))
+        assert prof.max() - prof[rec["argmax"][a, b]] <= MAG_TOL * prof.max(), (what, a, b)
+    strength = rec["peak"].astype(np.float64) / ((rec["sum"] - rec["count"] * rec["peak"].astype(np.float64)) / (n - rec["count"]))
+    ref_strength = peak / ((total - count * peak) / (n - count))
+    assert np.abs(strength - ref_strength).max() <= 1e-4 * ref_strength.max(), what
+    return len(bad)
+
+
+def assert_records_equal(a, b, what, sum_rtol=0):
+    """peak, argmax and count exact; sum exact, or within sum_rtol * max(b's sums) where the two launches add a cell's
+    values in a different order."""
+    for k in ("peak", "argmax", "count"):
+        assert np.array_equal(a[k], b[k]), (what, k)
+    if sum_rtol:
+        assert np.abs(a["sum"] - b["sum"]).max() <= sum_rtol * b["sum"].max(), (what, "sum")
+    else:
+        assert np.array_equal(a["sum"], b["sum"]), (what, "sum")
+
+
+def _search_worker(args):
+    sv, x, fs, n = args
+    trace = []
+    r = o.acquire_sv(sv, x, fs, n, trace)
+    return r, o.search_is_ambiguous(trace, MAG_TOL)
+
+
+def oracle_searches(svs, x, fs, n):
+    """[(o.acquire_sv result, whether its search sits on a branch point)] per SV, one process each."""
+    with _pool(len(svs)) as pool:
+        return pool.map(_search_worker, [(sv, x, fs, n) for sv in svs])
+
+
+def check_search(got, sv, ref, ambiguous, x, fs, n, what):
+    """got: (doppler, code_phase, strength, carrier phase) of a search; ref: the same of the float64 search, which is
+    ambiguous if it sits on a branch point (two bins' maxima, two profile values or two passes' strengths within the
+    tolerance of each other, proved with the oracle's trace)."""
+    doppler, code_phase, strength, phase = got
+    if ref[2] > o.DETECTION_THRESHOLD:  # detected satellites: everything must agree
+        assert (doppler, code_phase) == (ref[0], ref[1]), what
+        assert abs(strength - ref[2]) <= 1e-4 * ref[2], what
+        d = abs(phase - ref[3])
+        assert min(d, 2 * np.pi - d) <= 1e-4, what
+    elif (doppler, code_phase) == (ref[0], ref[1]):
+        assert abs(strength - ref[2]) <= 1e-4 * ref[2], what
+    else:  # noise only: another answer only on a branch point, and then a true cell of the search
+        assert ambiguous, what
+        prof = o.integrate(o.NON_COHERENT, x, fs, n, doppler, o.replica(sv, n))
+        assert abs(o.peak_strength(prof) - strength) <= 1e-4 * strength, what
+
+
+def _is_ambiguous(sv, x, fs, n):
+    trace = []
+    o.acquire_sv(sv, x, fs, n, trace)
+    return o.search_is_ambiguous(trace, MAG_TOL)
+
+
+def check_detector_golden(det, ids, x, attrs, detected, rows, fs, n, what):
+    """GpsSatelliteDetector against the live reference's detector: the satellites found, each recorded result row (sv,
+    doppler, carrier phase, code phase, strength) by check_search, and the on-device search (_acquire_many) against the
+    pass-by-pass search from the host (_acquire_many_stepwise), the same algorithm on other kernels.  Returns the
+    on-device results by SV."""
+    found = det.detect_satellites_in_antenna_data(ids, x, attrs)
+    assert [r.satellite_id.id for r in found] == [int(sv) for sv in detected], what
+    many = det._acquire_many(ids, x, attrs)
+    results = {r.satellite_id.id: r for r in many}
+    for row in rows:
+        sv = int(row[0])
+        r = results[sv]
+        ambiguous = (r.doppler_shift, r.prn_phase_shift) != (int(row[1]), int(row[3])) and _is_ambiguous(sv, x, fs, n)
+        check_search((r.doppler_shift, r.prn_phase_shift, r.correlation_strength, r.carrier_wave_phase_shift), sv,
+                     (int(row[1]), int(row[3]), row[4], row[2]), ambiguous, x, fs, n, (what, sv))
+    # identical decisions for the detected satellites, values equal to float32 rounding
+    for a, b in zip(many, det._acquire_many_stepwise(ids, x, attrs)):
+        if (a.doppler_shift, a.prn_phase_shift) != (b.doppler_shift, b.prn_phase_shift):
+            sv = a.satellite_id.id
+            assert b.correlation_strength <= o.DETECTION_THRESHOLD, (what, sv)  # detected satellites: never
+            assert _is_ambiguous(sv, x, fs, n), (what, sv)
+            continue
+        assert abs(a.correlation_strength - b.correlation_strength) <= 1e-5 * b.correlation_strength, what
+        d = abs(a.carrier_wave_phase_shift - b.carrier_wave_phase_shift)
+        assert min(d, 2 * np.pi - d) <= 1e-4 or b.correlation_strength <= o.DETECTION_THRESHOLD, what
+    return results

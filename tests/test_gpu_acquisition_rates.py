@@ -7,40 +7,36 @@ thread, polyphase rows and transpose tiles in separate shared memory), correlate
 the multi-millisecond one-warp kernel above S = 4, and odd N (5115), where every other millisecond starts 8 but not 16 bytes
 into an aligned buffer.
 
-Tolerances (DESIGN.md section 6, as in tests/test_gpu_fullsize.py): magnitudes and sums |gpu - ref| <= 1e-5 * max(ref); count
+Tolerances (DESIGN.md section 6, checked by tests/acq_support.py): magnitudes and sums |gpu - ref| <= 1e-5 * max(ref); count
 exact; argmax, Doppler bin and code phase exact unless the oracle's own float64 profile ties within the tolerance, proved per
 mismatch; strength 1e-4 relative; carrier phase 1e-4 rad.  Oracle grids are spread over the host's cores (fork pool)."""
-import multiprocessing as mp
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
+from acq_support import (DOP41, MAG_TOL, assert_records_equal, check_detector_golden, check_grid, check_search,
+                         mid_branch_lag, oracle_searches, rate)
+from gpu_support import ROOT, Attrs, EngineCache, make_engine, run_child
 from oracle import gypsum_oracle as o
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "acquisition_rates.npz")
 RATES = [1, 2, 3, 4, 5, 6, 8, 10, 12, 16]
 NEW_RATES = [5, 6, 8, 10, 12]
-MAG_TOL = 1e-5
-DOP41 = np.arange(-10000.0, 10001.0, 500.0)
-KEYS = ("peak", "argmax", "sum", "count")
 
 _FIRST_RUN_SCRIPT = r"""
 import sys
 import numpy as np
-sys.path.insert(0, sys.argv[1])
+sys.path[:0] = [sys.argv[1], sys.argv[1] + "/tests"]
+from gpu_support import make_engine
 from gypsum_b200 import _native
 from oracle import gypsum_oracle as o
 
 for s in (5, 6, 8, 10, 12):
     n, fs = 1023 * s, 1023000 * s
     x = o.synth_iq(s, n, 3, fs, [(25, 1500.0, n - 1, 0.3, 0.3)])
-    eng = _native.Engine(fs, n)
-    eng.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
+    eng = make_engine(fs, n)
     eng.upload_iq(x)
     dop = np.arange(-2000.0, 2001.0, 500.0)
     for m in (1, 3):
@@ -60,94 +56,25 @@ print("rates ok")
 def test_first_run_of_the_new_instantiations_in_a_child_process(native_lib):
     """Runs first, in its own process, so that a fault in a never-exercised kernel cannot disturb the CUDA context of
     the tests below."""
-    proc = subprocess.run([sys.executable, "-c", _FIRST_RUN_SCRIPT, ROOT], capture_output=True, text=True, timeout=600)
-    assert proc.returncode == 0 and "rates ok" in proc.stdout, proc.stderr[-2000:]
+    run_child(_FIRST_RUN_SCRIPT, ok="rates ok")
 
 
-_ENGINES = {}
-
-
-def engine_for(s):
-    from gypsum_b200 import _native
-
-    if s not in _ENGINES:
-        e = _native.Engine(1023000 * s, 1023 * s)
-        e.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
-        _ENGINES[s] = e
-    return _ENGINES[s]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _close_engines(native_lib):
-    yield
-    for e in _ENGINES.values():
-        e.close()
-    _ENGINES.clear()
-
-
-def _cells_worker(args):
-    x, fs, n, svs, dop, kind = args
-    return o.grid_cells(x, fs, n, svs, dop, kind)
-
-
-def oracle_grid(x, fs, n, svs, dop, kind=o.NON_COHERENT):
-    """o.grid_cells over all SVs, one process per SV group."""
-    procs = max(1, min(len(svs), os.cpu_count() or 1))
-    parts = [svs[i::procs] for i in range(procs)]
-    with mp.get_context("fork").Pool(procs) as pool:
-        res = pool.map(_cells_worker, [(x, fs, n, p, list(dop), kind) for p in parts])
-    shape = (len(svs), len(dop))
-    peak, arg, total, count = (np.zeros(shape), np.zeros(shape, np.int64), np.zeros(shape), np.zeros(shape, np.int64))
-    for i, (pk, ag, tt, ct) in enumerate(res):
-        rows = list(range(i, len(svs), procs))
-        peak[rows], arg[rows], total[rows], count[rows] = pk, ag, tt, ct
-    return peak, arg, total, count
-
-
-def oracle_profile(kind, x, fs, n, f, sv):
-    prof = o.integrate(kind, x, fs, n, f, o.replica(sv, n))
-    return np.abs(prof) if kind == o.COHERENT else prof
-
-
-def check_grid(rec, x, fs, n, svs, dop, what, kind=o.NON_COHERENT):
-    peak, arg, total, count = oracle_grid(x, fs, n, svs, dop, kind)
-    assert rec.shape == peak.shape
-    assert np.abs(rec["peak"] - peak).max() <= MAG_TOL * peak.max(), what
-    assert np.abs(rec["sum"] - total).max() <= MAG_TOL * total.max(), what
-    assert np.array_equal(rec["count"], count), what
-    bad = np.argwhere(rec["argmax"] != arg)
-    for a, b in bad:  # a different index is only acceptable where the float64 profile itself ties to within the tolerance
-        prof = oracle_profile(kind, x, fs, n, dop[b], svs[a])
-        assert prof.max() - prof[rec["argmax"][a, b]] <= MAG_TOL * prof.max(), (what, a, b)
-    strength = rec["peak"].astype(np.float64) / ((rec["sum"] - rec["count"] * rec["peak"].astype(np.float64)) / (n - rec["count"]))
-    ref_strength = peak / ((total - count * peak) / (n - count))
-    assert np.abs(strength - ref_strength).max() <= 1e-4 * ref_strength.max(), what
-    return len(bad)
-
-
-def assert_records_equal(a, b, what):
-    for k in KEYS:
-        assert np.array_equal(a[k], b[k]), (what, k)
-
-
-def rate(s):
-    return 1023 * s, 1023000 * s
-
-
-def mid_branch_lag(s):
-    """A lag in the middle of the code on the middle polyphase branch (branch s // 2)."""
-    return 511 * s + s // 2
+@pytest.fixture(scope="module")
+def engines(native_lib):
+    cache = EngineCache()
+    yield cache
+    cache.close()
 
 
 # ---- 1. full grid, M = 1 --------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("s", RATES)
-def test_full_grid_one_ms_every_cell(s):
+def test_full_grid_one_ms_every_cell(engines, s):
     """32 PRN x 41 Doppler x 1 ms, every cell.  Planted code phases at 0, mid-code on branch s // 2 and at n - 1
     (branch s - 1); each planted satellite is found at its planted bin and phase."""
     n, fs = rate(s)
     planted = [(3, -3000.0, 0, 1.0, 0.3), (11, 4500.0, mid_branch_lag(s), 2.0, 0.3), (32, -9500.0, n - 1, 2.5, 0.3)]
     x = o.synth_iq(200 + s, n, 1, fs, planted)
-    eng = engine_for(s)
+    eng = engines(1023 * s)
     eng.upload_iq(x)
     rec = eng.acquire_grid(1, 1, np.arange(32), DOP41)[0]
     check_grid(rec, x, fs, n, list(range(1, 33)), DOP41, f"S={s}")
@@ -158,14 +85,14 @@ def test_full_grid_one_ms_every_cell(s):
 
 # ---- 2. multi-millisecond grid, M = 3, two blocks -------------------------------------------------------------------
 @pytest.mark.parametrize("s", RATES)
-def test_three_ms_grid_two_blocks(s):
+def test_three_ms_grid_two_blocks(engines, s):
     """8 PRNs x 9 Doppler, M = 3, two blocks in one call: the block stride M * N is odd at S = 5."""
     n, fs = rate(s)
     svs = [3, 7, 11, 14, 20, 25, 29, 32]
     dop = np.arange(-4000.0, 4001.0, 1000.0)
     planted = [(7, 2000.0, n - 1, 0.4, 0.15), (25, -3000.0, mid_branch_lag(s), 1.3, 0.15)]
     x = np.concatenate([o.synth_iq(300 + 10 * s + b, n, 3, fs, planted) for b in range(2)])
-    eng = engine_for(s)
+    eng = engines(1023 * s)
     eng.upload_iq(x)
     rec = eng.acquire_grid(2, 3, [sv - 1 for sv in svs], dop)
     for b in range(2):
@@ -177,7 +104,7 @@ def test_three_ms_grid_two_blocks(s):
 
 # ---- 3. coherent ----------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("s", RATES)
-def test_coherent_grid_and_probes(s):
+def test_coherent_grid_and_probes(engines, s):
     """A coherent grid at M = 2 (warp-pair kernel), and a coherent cell list whose probes sit at 0, at n - 1, on branch
     s - 1 and at the planted peak: each probe's complex value against the oracle's coherent profile."""
     from gypsum_b200 import _native
@@ -187,7 +114,7 @@ def test_coherent_grid_and_probes(s):
     dop = np.arange(-2000.0, 2001.0, 1000.0)
     planted = [(25, 1000.0, n - 1, 0.7, 0.3), (9, -2000.0, 300 * s + s - 1, 2.1, 0.3)]
     x = o.synth_iq(400 + s, n, 2, fs, planted)
-    eng = engine_for(s)
+    eng = engines(1023 * s)
     eng.upload_iq(x)
     rec = eng.acquire_grid(1, 2, [sv - 1 for sv in svs], dop, _native.COHERENT)[0]
     check_grid(rec, x, fs, n, svs, dop, f"S={s} coherent", o.COHERENT)
@@ -213,7 +140,7 @@ PROFILE_CELLS = {1: (19, 700.0), 2: (25, 1500.0), 3: (11, -3500.0), 4: (32, 4875
 
 
 @pytest.mark.parametrize("s", RATES)
-def test_full_profiles(s):
+def test_full_profiles(engines, s):
     """correlation_profile, non-coherent and coherent, M = 2, against the oracle and, at the five new rates, against the
     profiles recorded from the live reference.  The planted code phase is n - 1."""
     from gypsum_b200 import _native
@@ -228,7 +155,7 @@ def test_full_profiles(s):
         sv, f = PROFILE_CELLS[s]
         planted = [(sv, f + 0.25, n - 1, 0.6, 0.3)]
     x = o.synth_iq(int(z["profile_seed"]), n, 2, fs, planted)
-    eng = engine_for(s)
+    eng = engines(1023 * s)
     eng.upload_iq(x)
     nc = eng.correlation_profile(sv - 1, f, 2, _native.NON_COHERENT)
     co = eng.correlation_profile(sv - 1, f, 2, _native.COHERENT)
@@ -246,10 +173,14 @@ def test_full_profiles(s):
 
 # ---- 5. large-batch path (rsplit = 1) -------------------------------------------------------------------------------
 @pytest.mark.parametrize("s", [s for s in RATES if np.gcd(s, 12) > 1])
-def test_large_batch_whole_cell_per_warp_path(s):
+def test_large_batch_whole_cell_per_warp_path(engines, s):
     """Enough cells (more than 8 * SMs * 12) that every warp of the one-warp kernel keeps a whole cell: records
-    identical to the split launches of single blocks (gcd(S, 12) warps per cell), and to the oracle on sampled cells."""
+    identical to the split launches of single blocks (gcd(S, 12) warps per cell), and to the oracle on sampled cells.
+    At S = 2 also on a large launch: records DMA'd straight into a pinned caller buffer, a wrong-shaped buffer refused,
+    and a sub-block exact against the oracle."""
     import torch
+
+    from gypsum_b200 import _native
 
     n, fs = rate(s)
     cells_per_block = 32 * DOP41.size
@@ -257,88 +188,77 @@ def test_large_batch_whole_cell_per_warp_path(s):
     assert nb * cells_per_block >= 8 * torch.cuda.get_device_properties(0).multi_processor_count * 12
     planted = [(25, 1500.0, n - 1, 0.3, 0.3), (4, -7000.0, mid_branch_lag(s), 0.0, 0.25)]
     x = o.synth_iq(500 + s, n, nb, fs, planted)
-    eng = engine_for(s)
+    eng = engines(1023 * s)
     eng.upload_iq(x)
     big = eng.acquire_grid(nb, 1, np.arange(32), DOP41)
     for b in (0, nb - 1):
         eng.upload_iq(x[b * n:(b + 1) * n])
         one = eng.acquire_grid(1, 1, np.arange(32), DOP41)[0]
-        for k in ("peak", "argmax", "count"):
-            assert np.array_equal(big[b][k], one[k]), (s, b, k)
-        assert np.abs(big[b]["sum"] - one["sum"]).max() <= 1e-9 * one["sum"].max()
+        assert_records_equal(big[b], one, (s, b), sum_rtol=1e-9)
     b = nb // 2
     check_grid(big[b][[24, 3]][:, 15:26], x[b * n:(b + 1) * n], fs, n, [25, 4], DOP41[15:26], f"S={s} block {b}")
     assert int(big[b]["argmax"][24, 23]) == n - 1 and int(big[b]["argmax"][3, 6]) == mid_branch_lag(s)
+    if s != 2:
+        return
+    # eight blocks of seed 8, repeated up to nb blocks; their sub-block below has no near-tie, so argmax and count are exact
+    y = o.synth_iq(8, n, 8, fs, [(25, 1500.0, 777, 0.3, 0.3), (4, -7000.0, 2000, 0.0, 0.25)])
+    eng.upload_iq(np.tile(y, -(-nb // 8))[:nb * n])
+    want = eng.acquire_grid(nb, 1, np.arange(32), DOP41)
+    pinned = torch.empty(nb * 32 * DOP41.size * 32, dtype=torch.uint8).pin_memory()
+    view = pinned.numpy().view(_native.RECORD_DTYPE).reshape(nb, 32, DOP41.size)
+    assert eng.acquire_grid(nb, 1, np.arange(32), DOP41, out=view) is view
+    assert_records_equal(view, want, "pinned out")
+    with pytest.raises(ValueError):
+        eng.acquire_grid(nb, 1, np.arange(32), DOP41, out=view[:4])
+    peak, arg, total, count = o.grid_cells(y[3 * n:4 * n], fs, n, [25, 4], list(DOP41[20:26]))
+    sub = want[3][[24, 3]][:, 20:26]
+    assert np.abs(sub["peak"] - peak).max() <= MAG_TOL * peak.max()
+    assert np.array_equal(sub["argmax"], arg) and np.array_equal(sub["count"], count)
+    assert np.abs(sub["sum"] - total).max() <= MAG_TOL * total.max()
 
 
 # ---- 6. scratch batching --------------------------------------------------------------------------------------------
-def test_grid_split_into_scratch_sized_batches_at_12276_ksps(native_lib, monkeypatch):
-    """S = 12, M = 2: a grid whose spectra exceed the scratch budget runs as several (doppler_spectra, correlate)
-    batches of blocks; records land exactly where a single batch puts them."""
-    from gypsum_b200 import _native
-
-    n, fs, nb = 12276, 12276000, 5
-    x = o.synth_iq(13, n, 2 * nb, fs, [(25, 1500.0, n - 1, 0.3, 0.3), (2, 6000.0, 11, 0.0, 0.3)])
-    dop = np.arange(-8000.0, 8001.0, 1000.0)
-    monkeypatch.setenv("GB200_SPEC_BUDGET_MB", "14")  # 17 bins x 2 ms x 384 KB = 6.4 MB per block -> batches of 2 blocks
-    small = _native.Engine(fs, n)
+@pytest.mark.parametrize("s", [2, 12])
+def test_grid_split_into_scratch_sized_batches(engines, monkeypatch, s):
+    """A grid whose spectra exceed the scratch budget runs as several (doppler_spectra, correlate) batches of blocks;
+    records land exactly where a single batch puts them.  S = 2, M = 1: 33 bins x 32 KB ~ 1 MB per block and a 3 MB
+    budget; S = 12, M = 2: 17 bins x 2 ms x 384 KB = 6.4 MB per block and 14 MB; batches of 2 blocks either way."""
+    n, fs = rate(s)
+    if s == 2:
+        m, nb, budget_mb, lag, blocks = 1, 7, "3", 777, (0, 3, 6)
+        x = o.synth_iq(12, n, nb, fs, [(25, 1500.0, lag, 0.3, 0.3), (2, 6500.0, 11, 0.0, 0.3)])
+        dop = np.arange(-8000.0, 8001.0, 500.0)
+    else:
+        m, nb, budget_mb, lag, blocks = 2, 5, "14", n - 1, range(5)
+        x = o.synth_iq(13, n, 2 * nb, fs, [(25, 1500.0, lag, 0.3, 0.3), (2, 6000.0, 11, 0.0, 0.3)])
+        dop = np.arange(-8000.0, 8001.0, 1000.0)
+    monkeypatch.setenv("GB200_SPEC_BUDGET_MB", budget_mb)
+    small = make_engine(fs, n)
     monkeypatch.delenv("GB200_SPEC_BUDGET_MB")
     try:
-        big = engine_for(12)
+        big = engines(n)
         for e in (small, big):
-            e.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
             e.upload_iq(x)
-        a = small.acquire_grid(nb, 2, np.arange(32), dop)
-        b = big.acquire_grid(nb, 2, np.arange(32), dop)
+        a = small.acquire_grid(nb, m, np.arange(32), dop)
+        b = big.acquire_grid(nb, m, np.arange(32), dop)
     finally:
         small.close()
-    for k in ("peak", "argmax", "count"):
-        assert np.array_equal(a[k], b[k]), k
-    assert np.abs(a["sum"] - b["sum"]).max() <= 1e-9 * b["sum"].max()
-    for blk in range(nb):
-        assert a["argmax"][blk, 24, int(np.argmax(a["peak"][blk, 24]))] == n - 1
+    assert_records_equal(a, b, f"S={s}", sum_rtol=1e-9)
+    for blk in blocks:
+        assert a["argmax"][blk, 24, int(np.argmax(a["peak"][blk, 24]))] == lag
         assert a["argmax"][blk, 1, int(np.argmax(a["peak"][blk, 1]))] == 11
 
 
 # ---- 7. on-device search --------------------------------------------------------------------------------------------
-def _search_worker(args):
-    sv, x, fs, n = args
-    trace = []
-    r = o.acquire_sv(sv, x, fs, n, trace)
-    return r, o.search_is_ambiguous(trace, MAG_TOL)
-
-
-def oracle_searches(svs, x, fs, n):
-    with mp.get_context("fork").Pool(max(1, min(len(svs), os.cpu_count() or 1))) as pool:
-        return pool.map(_search_worker, [(sv, x, fs, n) for sv in svs])
-
-
-def check_search(got, sv, ref, ambiguous, x, fs, n, what):
-    """The rules of tests/test_gpu_parity.py::test_detector_against_reference_golden.  got: (doppler, code_phase, strength,
-    carrier phase); ref: (doppler, code_phase, strength, carrier phase) of the float64 search."""
-    doppler, code_phase, strength, phase = got
-    if ref[2] > o.DETECTION_THRESHOLD:  # detected satellites: everything must agree
-        assert (doppler, code_phase) == (ref[0], ref[1]), what
-        assert abs(strength - ref[2]) <= 1e-4 * ref[2], what
-        d = abs(phase - ref[3])
-        assert min(d, 2 * np.pi - d) <= 1e-4, what
-    elif (doppler, code_phase) == (ref[0], ref[1]):
-        assert abs(strength - ref[2]) <= 1e-4 * ref[2], what
-    else:  # noise only: another answer only where the float64 search itself sits on a branch point
-        assert ambiguous, what
-        prof = o.integrate(o.NON_COHERENT, x, fs, n, doppler, o.replica(sv, n))
-        assert abs(o.peak_strength(prof) - strength) <= 1e-4 * strength, what
-
-
 @pytest.mark.parametrize("s", RATES)
-def test_on_device_search_against_oracle(s):
+def test_on_device_search_against_oracle(engines, s):
     """gb200_detect at M = 3 == acquire_sv (acquisition.py:70-152): two planted satellites, one at code phase n - 1, and
     one absent."""
     n, fs = rate(s)
     svs = [14, 27, 20]
     planted = [(14, 2345.0, n - 1, 0.9, 0.2), (27, -4150.0, mid_branch_lag(s), 2.2, 0.2)]
     x = o.synth_iq(600 + s, n, 3, fs, planted)
-    eng = engine_for(s)
+    eng = engines(1023 * s)
     eng.upload_iq(x)
     got = eng.detect([sv - 1 for sv in svs], 3)
     refs = oracle_searches(svs, x, fs, n)
@@ -350,12 +270,6 @@ def test_on_device_search_against_oracle(s):
     # the best of ~220 noise-only cells can reach just above the threshold (3.1 - 3.4 at some rates): the absent satellite
     # is checked by the rules above whichever side of it it lands on
     assert refs[2][0].strength < min(refs[0][0].strength, refs[1][0].strength)
-
-
-class Attrs:
-    def __init__(self, fs, n):
-        self.samples_per_second = fs
-        self.samples_per_prn_transmission = n
 
 
 @pytest.mark.parametrize("s", [5, 12])
@@ -374,35 +288,12 @@ def test_detector_against_reference_golden_at_other_rates(native_lib, s):
     codes = generate_replica_prn_signals()
     det = GpsSatelliteDetector({sid: GpsSatellite(sid, code, s) for sid, code in codes.items()})
     ids = [GpsSatelliteId(int(sv)) for sv in z[f"{key}__svs"]]
-    attrs = Attrs(fs, n)
-    found = det.detect_satellites_in_antenna_data(ids, x, attrs)
-    assert [r.satellite_id.id for r in found] == [int(sv) for sv in z[f"{key}__detected"]]
-    many = det._acquire_many(ids, x, attrs)
-    for r, row in zip(many, z[f"{key}__results"]):
-        sv = int(row[0])
-        ambiguous = False
-        if (r.doppler_shift, r.prn_phase_shift) != (int(row[1]), int(row[3])):
-            trace = []
-            o.acquire_sv(sv, x, fs, n, trace)
-            ambiguous = o.search_is_ambiguous(trace, MAG_TOL)
-        check_search((r.doppler_shift, r.prn_phase_shift, r.correlation_strength, r.carrier_wave_phase_shift), sv,
-                     (int(row[1]), int(row[3]), row[4], row[2]), ambiguous, x, fs, n, (s, sv))
-    for a, b in zip(many, det._acquire_many_stepwise(ids, x, attrs)):
-        if (a.doppler_shift, a.prn_phase_shift) != (b.doppler_shift, b.prn_phase_shift):
-            sv = a.satellite_id.id
-            assert b.correlation_strength <= 3, sv  # detected satellites: never
-            trace = []
-            o.acquire_sv(sv, x, fs, n, trace)
-            assert o.search_is_ambiguous(trace, MAG_TOL), sv
-            continue
-        assert abs(a.correlation_strength - b.correlation_strength) <= 1e-5 * b.correlation_strength
-        d = abs(a.carrier_wave_phase_shift - b.carrier_wave_phase_shift)
-        assert min(d, 2 * np.pi - d) <= 1e-4 or b.correlation_strength <= 3
+    check_detector_golden(det, ids, x, Attrs(fs, n), z[f"{key}__detected"], z[f"{key}__results"], fs, n, f"S={s}")
 
 
 # ---- 8. generic replica ---------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("s", [5, 16])
-def test_generic_replica_profiles(s):
+def test_generic_replica_profiles(engines, s):
     """correlation_profile_replica with a random complex replica, M = 2, both kinds, against o.integrate."""
     from gypsum_b200 import _native
 
@@ -410,7 +301,7 @@ def test_generic_replica_profiles(s):
     x = o.synth_iq(700 + s, n, 2, fs, [(9, -1250.0, n - 1, 0.7, 0.3)])
     rep = (np.random.default_rng(s).standard_normal(n) + 1j * np.random.default_rng(100 + s).standard_normal(n))
     rep = rep.astype(np.complex64)
-    eng = engine_for(s)
+    eng = engines(1023 * s)
     eng.upload_iq(x)
     nc = eng.correlation_profile_replica(rep, 1500.0, 2, _native.NON_COHERENT)
     co = eng.correlation_profile_replica(rep, 1500.0, 2, _native.COHERENT)
@@ -421,7 +312,7 @@ def test_generic_replica_profiles(s):
 
 
 # ---- 9. odd N: milliseconds that start 8 but not 16 bytes into a buffer ------------------------------------------------
-def test_odd_n_ring_windows_and_graph_replayed_host_grid(native_lib):
+def test_odd_n_ring_windows_and_graph_replayed_host_grid(engines):
     """At 5.115 Msps N is odd.  Grids and searches over a device-ring window bound at an odd slot and at an even slot,
     and acquire_grid_host (eager, captured, replayed), are bit-identical to upload_iq + acquire_grid / detect on the same
     samples."""
@@ -431,7 +322,7 @@ def test_odd_n_ring_windows_and_graph_replayed_host_grid(native_lib):
     svs = np.array([13, 24, 2], dtype=np.int32)
     dop = np.arange(-3000.0, 3001.0, 1000.0)
     x = o.synth_iq(800, n, 5, fs, [(14, 2000.0, n - 1, 0.9, 0.2), (25, -1000.0, 2557, 0.3, 0.2)])
-    eng = engine_for(5)
+    eng = engines(n)
 
     def run():
         return (eng.acquire_grid(3, 1, svs, dop), eng.acquire_grid(1, 3, svs, dop), eng.detect(svs, 3))
@@ -466,13 +357,13 @@ def test_odd_n_ring_windows_and_graph_replayed_host_grid(native_lib):
 
 # ---- 10. all-zero input ---------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("s", RATES)
-def test_all_zero_input(s):
+def test_all_zero_input(engines, s):
     """Every profile value ties at 0: peak 0, argmax 0, count N, sum 0 through the M = 1 grid, the M = 2 grid and a
     coherent list.  The fused kernel exists only at S = 2 and 4."""
     from gypsum_b200 import _native
 
     n, _ = rate(s)
-    eng = engine_for(s)
+    eng = engines(1023 * s)
     eng.upload_iq(np.zeros(2 * n, np.complex64))
     dop = np.array([-5000.0, 0.0, 2500.0])
     for rec in (eng.acquire_grid(1, 1, [0, 17, 31], dop), eng.acquire_grid(1, 2, [0, 17, 31], dop),

@@ -1,38 +1,34 @@
 """GPU tracking at every rate the engine acquires at other than 2.046 / 4.092 Msps: k_track_channels at S = 1, 3 and
 k_track_channels_wide at S = 5 .. 16 (tracker.cu), against the tracker oracle and the live reference's trajectories
-(tests/golden/tracker_fs1/fs8/fs16/fs16_long.npz).  Same tolerances as tests/test_gpu_tracker.py."""
-import os
-import subprocess
-import sys
-
+(tests/golden/tracker_fs1/fs8/fs16/fs16_long.npz).  Same bounds as tests/test_gpu_tracker.py
+(tests/tracker_support.py)."""
 import numpy as np
 import pytest
 
+from gpu_support import EngineCache, run_child
 from oracle import gypsum_oracle as o
 from oracle import tracker_oracle as t
+from tracker_support import assert_follows_reference, load_tracker_case, start_times
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
 RATES = [1, 3, 5, 6, 8, 10, 12, 16]
 N16, FS16 = 16368, 16368000
 
 _FIRST_RUN_SCRIPT = r"""
 import sys
-import numpy as np
-sys.path.insert(0, sys.argv[1])
+sys.path[:0] = [sys.argv[1], sys.argv[1] + "/tests"]
+from gpu_support import make_engine
 from gypsum_b200 import _native
-from oracle import gypsum_oracle as o
 from oracle import tracker_oracle as t
+from tracker_support import start_times
 
 for s in (1, 3, 5, 16):
     n, fs = 1023 * s, 1023000 * s
     x = t.synth_tracking_iq(7, n, 20, fs, [(12, 640.4, 0.0, 1501, 0.7, 0.004)])
-    eng = _native.Engine(fs, n)
-    eng.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
+    eng = make_engine(fs, n)
     eng.upload_iq(x)
     trk = _native.Tracker(eng, [11], [640.0], [0.0], [1501])
-    rec = trk.process(20, np.array([t.chunk_times(k, fs, n)[0] for k in range(20)]))[0]
+    rec = trk.process(20, start_times(20, fs, n))[0]
     tr = t.TrackerOracle(12, 640.0, 0.0, 1501, fs, n)
     want = [tr.step(x[k * n:(k + 1) * n], *t.chunk_times(k, fs, n))["symbol"] for k in range(20)]
     assert not rec["lost"].any() and list(rec["symbol"]) == want, s
@@ -45,37 +41,18 @@ print("rates ok")
 def test_first_run_of_the_new_instantiations_in_a_child_process(native_lib):
     """Runs first, in its own process, so that a fault in a never-exercised kernel cannot disturb the CUDA context of
     the tests below."""
-    proc = subprocess.run([sys.executable, "-c", _FIRST_RUN_SCRIPT, ROOT], capture_output=True, text=True, timeout=600)
-    assert proc.returncode == 0 and "rates ok" in proc.stdout, proc.stderr[-2000:]
+    run_child(_FIRST_RUN_SCRIPT, ok="rates ok")
 
 
-_ENGINES = {}
-
-
-def engine_for(s):
-    from gypsum_b200 import _native
-
-    if s not in _ENGINES:
-        e = _native.Engine(1023000 * s, 1023 * s)
-        e.set_replicas(np.stack([o.ca_code(sv) for sv in range(1, 33)]).astype(np.uint8))
-        _ENGINES[s] = e
-    return _ENGINES[s]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _close_engines():
-    yield
-    for e in _ENGINES.values():
-        e.close()
-    _ENGINES.clear()
-
-
-def times(n_ms, fs, n):
-    return np.array([t.chunk_times(k, fs, n)[0] for k in range(n_ms)])
+@pytest.fixture(scope="module")
+def engines(native_lib):
+    cache = EngineCache()
+    yield cache
+    cache.close()
 
 
 @pytest.mark.parametrize("s", RATES)
-def test_teacher_forced_correlators_at_every_rate(native_lib, s):
+def test_teacher_forced_correlators_at_every_rate(engines, s):
     """Each millisecond starts from the oracle's loop state: early / late / prompt outputs and the updated state."""
     from gypsum_b200 import _native
 
@@ -83,7 +60,7 @@ def test_teacher_forced_correlators_at_every_rate(native_lib, s):
     amp = 0.004 if s < 8 else 0.002
     x = t.synth_tracking_iq(100 + s, n, 60, fs, [(25, 1500.3, 0.0, 777, 0.3, amp)])
     tr = t.TrackerOracle(25, 1500.0, 0.0, 777, fs, n)
-    eng = engine_for(s)
+    eng = engines(n)
     trk = _native.Tracker(eng, [24], [1500.0], [0.0], [777])
     for k in range(60):
         a, b = t.chunk_times(k, fs, n)
@@ -103,34 +80,19 @@ def test_teacher_forced_correlators_at_every_rate(native_lib, s):
     trk.close()
 
 
-def load_case(name):
-    z = np.load(os.path.join(GOLDEN, f"tracker_{name}.npz"))
-    ch = z["channel"]
-    ch = (int(ch[0]), ch[1], ch[2], int(ch[3]), ch[4], ch[5])
-    n, fs = int(z["n"]), int(z["fs"])
-    x = t.synth_tracking_iq(int(z["seed"]), n, int(z["n_ms"]), fs, [ch], float(z["sigma"]))
-    return z, ch, x, n, fs
-
-
 @pytest.mark.parametrize("name", ["fs1", "fs8", "fs16", "fs16_long"])
-def test_free_running_matches_reference_at_other_rates(native_lib, name):
+def test_free_running_matches_reference_at_other_rates(engines, name):
     from gypsum_b200 import _native
-    from test_gpu_tracker import assert_symbols_and_code_phase_follow_reference
 
-    z, ch, x, n, fs = load_case(name)
+    z, ch, x, n, fs = load_tracker_case(name)
     init, rows = z["init"], z["rows"]
     n_ms = len(rows)
-    eng = engine_for(n // 1023)
+    eng = engines(n)
     trk = _native.Tracker(eng, [ch[0] - 1], [init[0]], [init[1]], [int(init[2])])
     eng.upload_iq(x)
-    rec = trk.process(n_ms, times(n_ms, fs, n))[0]
+    rec = trk.process(n_ms, start_times(n_ms, fs, n))[0]
     trk.close()
-    assert not rec["lost"].any()
-    assert_symbols_and_code_phase_follow_reference(rec, rows)
-    assert np.abs(rec["doppler"] - rows[:, 6]).max() <= 5e-3
-    d = np.abs(rec["carrier_phase"] - rows[:, 7])
-    assert np.minimum(d, 2 * np.pi - d).max() <= 2e-3
-    assert np.abs(rec["doppler_hist"] - rows[:, 12]).max() <= 5e-3
+    assert_follows_reference(rec, rows, histories=True)
     assert np.array_equal(rec["doppler"] != rec["doppler_hist"], rows[:, 6] != rows[:, 12])
     if name == "fs16":  # sigma 0.01: the reference reaches is_locked(); the device decides the same milliseconds
         tr = t.TrackerOracle(ch[0], init[0], init[1], int(init[2]), fs, n)
@@ -141,21 +103,21 @@ def test_free_running_matches_reference_at_other_rates(native_lib, name):
         assert n_ms > 6000 and rec["locked"].sum() == 0
 
 
-def test_bank_and_profile_at_16368_ksps(native_lib):
+def test_bank_and_profile_at_16368_ksps(engines):
     """Several channels over one stream == each channel alone; |prompt profile| matches the oracle."""
     from gypsum_b200 import _native
 
     chans = [(25, 1500.3, 0.0, 777, 0.3, 0.002), (7, -2212.7, 0.0, 100, 1.0, 0.002), (31, 3000.2, 0.0, 2045, 2.0, 0.002)]
     init = [(24, 1500.0, 0.0, 777), (6, -2210.0, 0.5, 100), (30, 3000.0, 0.0, 2045)]
     x = t.synth_tracking_iq(21, N16, 40, FS16, chans)
-    eng = engine_for(16)
+    eng = engines(N16)
     eng.upload_iq(x)
     bank = _native.Tracker(eng, *[list(v) for v in zip(*init)])
-    rec, prof = bank.process(40, times(40, FS16, N16), want_profiles=True)
+    rec, prof = bank.process(40, start_times(40, FS16, N16), want_profiles=True)
     bank.close()
     for c in range(3):
         one = _native.Tracker(eng, *[[v] for v in init[c]])
-        r1 = one.process(40, times(40, FS16, N16))[0]
+        r1 = one.process(40, start_times(40, FS16, N16))[0]
         one.close()
         for k in ("doppler", "carrier_phase", "peak_re", "code_phase", "symbol"):
             assert np.array_equal(rec[c][k], r1[k]), (c, k)

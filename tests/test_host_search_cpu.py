@@ -7,6 +7,7 @@ import os
 
 import numpy as np
 
+from gpu_support import Attrs
 from gypsum_b200 import _native
 from oracle import gypsum_oracle as o
 
@@ -51,10 +52,6 @@ class OracleEngine:
         return o.integrate(which, self.x[: n_ms * self.n], self.fs, self.n, float(dop), np.asarray(replica, dtype=complex))
 
 
-class Attrs:
-    samples_per_second, samples_per_prn_transmission = 2046000, 2046
-
-
 def test_pass_by_pass_search_reproduces_the_reference_detector(monkeypatch):
     from gypsum_b200 import utils
     from gypsum_b200.acquisition import GpsSatelliteDetector, doppler_search_bins
@@ -71,7 +68,7 @@ def test_pass_by_pass_search_reproduces_the_reference_detector(monkeypatch):
     det = GpsSatelliteDetector({sid: GpsSatellite(sid, code, 2) for sid, code in codes.items()})
     rows = {int(r[0]): r for r in z["results"]}
     ids = [GpsSatelliteId(sv) for sv in (25, 1, 3)]  # two planted satellites and a noise-only one
-    got = det._acquire_many_stepwise(ids, x, Attrs)
+    got = det._acquire_many_stepwise(ids, x, Attrs(2046000, 2046))
     # ten non-coherent passes of (20 | 28) bins per satellite + one coherent call
     assert [c[1] for c in eng.calls] == [_native.NON_COHERENT] * 10 + [_native.COHERENT]
     assert sum(c[0] for c in eng.calls[:10]) == 3 * 222
@@ -85,7 +82,7 @@ def test_pass_by_pass_search_reproduces_the_reference_detector(monkeypatch):
     # acquisition.py:163-167: int() truncates toward zero and the upper end is excluded
     assert list(doppler_search_bins(0.0, 7000.0))[:2] == [-7000, -6300] and len(doppler_search_bins(0.0, 7000.0)) == 20
     assert list(doppler_search_bins(-3258.0, 13.671875)) == list(range(-3271, -3244, 1))
-    best = det.get_best_doppler_shift_estimation(0.0, 7000.0, x, Attrs, GpsSatelliteId(25))
+    best = det.get_best_doppler_shift_estimation(0.0, 7000.0, x, Attrs(2046000, 2046), GpsSatelliteId(25))
     assert best.sample_offset_of_correlation_peak == int(best.non_coherent_correlation_profile.argmax()) == 777
     assert best.doppler_shift in doppler_search_bins(0.0, 7000.0)
 
@@ -105,8 +102,7 @@ def test_drop_in_utils_wrappers_argument_handling(monkeypatch):
     ent = {"engine": eng, "codes": {}, "table": []}
     monkeypatch.setattr(utils.POOL, "get", lambda fs_, n_, device=0: ent)
 
-    class A:
-        samples_per_second, samples_per_prn_transmission = fs, n
+    A = Attrs(fs, n)
 
     x = o.synth_iq(3, n, 3, fs, [(9, 1250.0, 1001, 0.4, 0.3)])
     rep = o.replica(9, n)

@@ -7,6 +7,7 @@ import os
 import numpy as np
 import pytest
 
+from gpu_support import Attrs
 from gypsum_b200 import _native
 from oracle import tracker_oracle as t
 
@@ -76,10 +77,6 @@ class StandInPool:
         return (rec, prof) if want_profiles else rec
 
 
-class Attrs:
-    samples_per_second, samples_per_prn_transmission = FS, N
-
-
 class Chunk:
     def __init__(self, k, x):
         self.start_time, self.end_time = t.chunk_times(k, FS, N)
@@ -109,7 +106,7 @@ def _add_tracker(world, sv, init, profiles=True):
     params = trk_mod.GpsSatelliteTrackingParameters(
         satellite=GpsSatellite(GpsSatelliteId(sv), codes[GpsSatelliteId(sv)], 2), current_doppler_shift=init[0],
         current_carrier_wave_phase_shift=init[1], current_prn_code_phase_shift=int(init[2]), doppler_shifts=[])
-    return trk_mod.GpsSatelliteTracker(params, Attrs, keep_correlation_profiles=profiles), params
+    return trk_mod.GpsSatelliteTracker(params, Attrs(FS, N), keep_correlation_profiles=profiles), params
 
 
 def _tracker(monkeypatch, sv, init):

@@ -2,46 +2,29 @@
 product's scalar loop code (gypsum_b200/csrc/tracker_core.cuh, run by the lane emulator) teacher-forced with
 the oracle's correlator outputs."""
 import ctypes
-import os
 
 import numpy as np
 import pytest
 
 from oracle import tracker_oracle as t
+from tracker_support import load_tracker_case, oracle_row
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
-N, FS = 2046, 2046000
 TRACK_REC = np.dtype([("doppler", "<f8"), ("carrier_phase", "<f8"), ("error", "<f8"), ("disc", "<f8"), ("phase_acc", "<f8"),
                       ("doppler_hist", "<f8"), ("carrier_phase_hist", "<f8"), ("peak_re", "<f4"), ("peak_im", "<f4"), ("strength", "<f4"), ("early_re", "<f4"), ("early_im", "<f4"),
                       ("late_re", "<f4"), ("late_im", "<f4"), ("code_phase", "<i4"), ("symbol", "<i4"), ("locked", "<i4"),
                       ("lost", "<i4"), ("peak_offset", "<i4"), ("pad0", "<i4"), ("pad1", "<i4")])
 
 
-def load_case(name):
-    z = np.load(os.path.join(GOLDEN, f"tracker_{name}.npz"))
-    ch = z["channel"]
-    ch = (int(ch[0]), ch[1], ch[2], int(ch[3]), ch[4], ch[5])
-    x = t.synth_tracking_iq(int(z["seed"]), N, int(z["n_ms"]), FS, [ch], float(z["sigma"]))
-    return z, ch, x
-
-
 @pytest.mark.parametrize("name,limit", [("short", 700), ("long", 1200), ("fs4", 500), ("adjust", 6100)])
 def test_oracle_tracker_bit_exact_with_reference(name, limit):
     """fs4: 4.092 Msps, where the reference keeps its hard-wired 2046 (tracker.py:301-303, :319; SURVEY F12)."""
-    z, ch, x = load_case(name)
+    z, ch, x, n, fs = load_tracker_case(name)
     init = z["init"]
-    N, FS = (int(z["n"]), int(z["fs"])) if "n" in z.files else (2046, 2046000)
-    if N != 2046:
-        x = t.synth_tracking_iq(int(z["seed"]), N, int(z["n_ms"]), FS, [ch], float(z["sigma"]))
-    tr = t.TrackerOracle(ch[0], init[0], init[1], int(init[2]), FS, N)
+    tr = t.TrackerOracle(ch[0], init[0], init[1], int(init[2]), fs, n)
     for k in range(min(limit, len(z["rows"]))):
-        a, b = t.chunk_times(k, FS, N)
-        r = tr.step(x[k * N:(k + 1) * N], a, b)
-        mine = np.array([r["peak"].real, r["peak"].imag, r["strength"], r["symbol"], r["error"], r["disc"], r["doppler"],
-                         r["carrier_phase"], r["code_phase"], r["start"], r["end"], tr.phase, r["doppler_hist"],
-                         r["carrier_phase_hist"]], dtype=np.float64)
-        assert np.array_equal(mine, z["rows"][k]), k
+        a, b = t.chunk_times(k, fs, n)
+        r = tr.step(x[k * n:(k + 1) * n], a, b)
+        assert np.array_equal(oracle_row(tr, r), z["rows"][k]), k
     if name == "adjust":  # the 6-second nudge fired: histories hold the value before it, current_* the value after
         assert z["rows"][6000, 6] - z["rows"][6000, 12] == 5.0 and z["rows"][6000, 7] != z["rows"][6000, 13]
 
@@ -51,9 +34,9 @@ def test_scalar_loop_teacher_forced(emu_lib, name):
     """track_update (DLL, PLL, is_locked with sliding sums, 6-s constellation check) fed the oracle's per-ms E/L/peak
     reproduces the reference's Doppler / phase / code-phase / lock-loss trajectory."""
     assert TRACK_REC.itemsize == 112
-    z, ch, x = load_case(name)
+    z, ch, x, n, fs = load_tracker_case(name)
     init = z["init"]
-    tr = t.TrackerOracle(ch[0], init[0], init[1], int(init[2]), FS, N)
+    tr = t.TrackerOracle(ch[0], init[0], init[1], int(init[2]), fs, n)
     st = ctypes.create_string_buffer(emu_lib.emu_track_state_size())
     emu_lib.emu_track_init.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_double, ctypes.c_int]
     emu_lib.emu_track_update.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_int, ctypes.c_double,
@@ -64,15 +47,15 @@ def test_scalar_loop_teacher_forced(emu_lib, name):
     lost_at = -1
     locked_ref = locked_mine = 0
     for k in range(int(z["n_ms"])):
-        a, b = t.chunk_times(k, FS, N)
+        a, b = t.chunk_times(k, fs, n)
         raised = False
         try:
-            r = tr.step(x[k * N:(k + 1) * N], a, b)
+            r = tr.step(x[k * n:(k + 1) * n], a, b)
         except t.LostLock as exc:
             r, raised = exc.args[0], True
         elp = np.array([r["early"].real, r["early"].imag, r["late"].real, r["late"].imag, r["peak"].real, r["peak"].imag],
                        dtype=np.float32)
-        emu_lib.emu_track_update(st, elp.ctypes.data, np.float32(r["strength"]), r["peak_offset"], a, float(FS), rec.ctypes.data)
+        emu_lib.emu_track_update(st, elp.ctypes.data, np.float32(r["strength"]), r["peak_offset"], a, float(fs), rec.ctypes.data)
         if raised:  # tracker.py:378: the scalar loop must flag the same millisecond
             assert rec["lost"][0] == 1
             lost_at = k
