@@ -1,5 +1,7 @@
 """What the acquisition test modules share: the tolerances of DESIGN.md section 6, the float64 oracle's grids and searches
 spread over the host's cores (fork pool), and the rules that hold the device's records and searches to them."""
+import functools
+import math
 import multiprocessing as mp
 import os
 
@@ -44,10 +46,73 @@ def oracle_grid(x, fs, n, svs, dop, kind=o.NON_COHERENT):
     return peak, arg, total, count
 
 
-def check_grid(rec, x, fs, n, svs, dop, what, kind=o.NON_COHERENT):
+@functools.lru_cache(maxsize=None)
+def _replica_spectrum(sv, n):
+    return np.conj(np.fft.fft(o.replica(sv, n)))
+
+
+def _vector_cols(x, fs, n, svs, dop, kind, probe):
+    uniq = sorted(set(svs))
+    rows = [uniq.index(sv) for sv in svs]
+    rep = np.stack([_replica_spectrum(sv, n) for sv in uniq])
+    shape = (len(svs), len(dop))
+    peak, arg, total, count = (np.zeros(shape), np.zeros(shape, np.int64), np.zeros(shape), np.zeros(shape, np.int64))
+    val = np.zeros(shape, complex)
+    cols = {}  # equal Doppler entries (bit for bit) share one profile
+    for b, f in enumerate(dop):
+        cols.setdefault(np.float64(f).tobytes(), []).append(b)
+    for bs in cols.values():
+        f = dop[bs[0]]
+        acc = np.zeros((len(uniq), n), dtype=complex if kind == o.COHERENT else np.float64)
+        for i in range(len(x) // n):  # o.integrate's arithmetic, every SV of the column at once
+            t = (np.arange(n) / fs) + ((i * n) / fs)
+            carrier = np.exp(-1j * math.tau * f * t)
+            c = np.fft.ifft(np.fft.fft(x[i * n:(i + 1) * n] * carrier)[None, :] * rep, axis=-1)
+            if kind == o.COHERENT:
+                acc += c
+            else:
+                acc += np.abs(c)
+        mag = np.abs(acc) if kind == o.COHERENT else acc
+        mx = mag.max(axis=1)
+        for b in bs:
+            peak[:, b], arg[:, b], total[:, b] = mx[rows], mag.argmax(axis=1)[rows], mag.sum(axis=1)[rows]
+            count[:, b] = np.count_nonzero(mag == mx[:, None], axis=1)[rows]
+            if probe is not None:
+                val[:, b] = acc[rows, np.asarray(probe)[:, b]]
+    return peak, arg, total, count, val
+
+
+def _vector_worker(args):
+    return _vector_cols(*args)
+
+
+def vector_grid(x, fs, n, svs, dop, kind=o.NON_COHERENT, probe=None):
+    """o.grid_cells restated for speed, same float64 arithmetic: per (Doppler, ms) one wiped-off forward FFT, its products
+    with conj(FFT(replica)) of every SV at once and one batched inverse FFT; repeated SVs and bit-equal Doppler entries are
+    computed once.  Returns (peak, argmax, sum, count, probe values), each [len(svs), len(dop)]: probe values are the
+    coherent (complex) or non-coherent profile at the lag probe[a, b], zeros without probe.  Large grids are spread over
+    the host's cores (fork pool) by Doppler column."""
+    dop = np.asarray(dop, dtype=np.float64)
+    work = len(set(svs)) * dop.size * len(x)
+    procs = max(1, min(dop.size, os.cpu_count() or 1, work // (1 << 24)))
+    if procs == 1:
+        return _vector_cols(x, fs, n, list(svs), dop, kind, probe)
+    parts = [np.arange(i, dop.size, procs) for i in range(procs)]
+    with _pool(procs) as pool:
+        res = pool.map(_vector_worker, [(x, fs, n, list(svs), dop[p], kind,
+                                         None if probe is None else np.asarray(probe)[:, p]) for p in parts])
+    out = [np.zeros((len(svs), dop.size), a.dtype) for a in res[0]]
+    for p, r in zip(parts, res):
+        for o_, a in zip(out, r):
+            o_[:, p] = a
+    return tuple(out)
+
+
+def check_grid(rec, x, fs, n, svs, dop, what, kind=o.NON_COHERENT, ref=None):
     """Every record of a (SV x Doppler) grid against the oracle: peak, sum and strength within the tolerance, count exact,
-    argmax exact bar near-ties proved on the float64 profile.  Returns the number of such proofs."""
-    peak, arg, total, count = oracle_grid(x, fs, n, svs, dop, kind)
+    argmax exact bar near-ties proved on the float64 profile.  ref: the oracle's (peak, argmax, sum, count) of the grid
+    when the caller has them (vector_grid), else o.grid_cells runs here.  Returns the number of near-tie proofs."""
+    peak, arg, total, count = ref if ref is not None else oracle_grid(x, fs, n, svs, dop, kind)
     assert rec.shape == peak.shape
     assert np.abs(rec["peak"] - peak).max() <= MAG_TOL * peak.max(), what
     assert np.abs(rec["sum"] - total).max() <= MAG_TOL * total.max(), what
