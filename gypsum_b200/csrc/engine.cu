@@ -1358,7 +1358,12 @@ static int tracker_launch(gb200_tracker* t, int n_sel, const int32_t* sel, int n
     if (n_ms < 1 || !start_times) GB_FAIL(e, GB200_EINVAL, "need at least one whole millisecond of samples");
     GB_TRY(check_iq(e, n_ms));
     GB_TRY(check_samples(e, n_ms));
-    if (reinterpret_cast<uintptr_t>(e->iq) % 16 != 0) GB_FAIL(e, GB200_EINVAL, "IQ buffer must be 16-byte aligned for tracking");
+    // k_track_channels stages the chunks of an even S with 16-byte cp.async; at odd S, N is odd, every other millisecond of
+    // a stream starts 8 bytes past a 16-byte boundary, and both tracking kernels read it in 8-byte pieces (a device ring's
+    // odd slots are such addresses)
+    const uintptr_t iq_align = e->s % 2 == 0 ? 16 : 8;
+    if (reinterpret_cast<uintptr_t>(e->iq) % iq_align != 0)
+        GB_FAIL(e, GB200_EINVAL, "IQ buffer must be %d-byte aligned for tracking at S = %d", static_cast<int>(iq_align), e->s);
     if (sel) {
         for (int i = 0; i < n_sel; ++i) {
             GB_TRY(check_channel(t, sel[i]));

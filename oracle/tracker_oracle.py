@@ -115,13 +115,14 @@ class TrackerOracle:
         return out
 
 
-def synth_tracking_iq(seed: int, n: int, n_ms: int, fs: int, channels, sigma: float = 0.02) -> np.ndarray:
+def synth_tracking_iq(seed: int, n: int, n_ms: int, fs: int, channels, sigma: float = 0.02, t0: float = 0.0) -> np.ndarray:
     """SURVEY.md 8d / F11: noise sigma per sample plus, per channel (sv, doppler_hz, doppler_rate_hz_s, code_phase,
-    carrier_phase, amplitude), amplitude * code * data-bit (20 ms, random) * exp(j(2 pi (f t + rate t^2/2) + phi))."""
+    carrier_phase, amplitude), amplitude * code * data-bit (20 ms, random) * exp(j(2 pi (f t + rate t^2/2) + phi)), the
+    first sample at stream time t0."""
     rng = np.random.default_rng(seed)
     total = n * n_ms
     x = (rng.standard_normal(total) + 1j * rng.standard_normal(total)) * (sigma / math.sqrt(2.0))
-    t = np.arange(total) / fs
+    t = np.arange(total) / fs + t0
     for sv, f, rate, tau_s, phi, amp in channels:
         code = np.tile(np.roll(replica(sv, n).real, tau_s), n_ms)
         bits = rng.integers(0, 2, size=n_ms // 20 + 2) * 2 - 1

@@ -10,7 +10,7 @@ import pytest
 from gpu_support import Attrs, make_engine, run_child
 from oracle import gypsum_oracle as o
 from oracle import tracker_oracle as t
-from tracker_support import assert_follows_reference, load_tracker_case, start_times
+from tracker_support import assert_follows_reference, assert_ms_matches_oracle, load_tracker_case, start_times
 
 pytestmark = pytest.mark.gpu
 N, FS = 2046, 2046000
@@ -27,25 +27,16 @@ def test_teacher_forced_correlators(engine):
     """Each millisecond starts from the oracle's loop state: early / late / prompt outputs and the updated state."""
     from gypsum_b200 import _native
 
-    z, ch, x, _, _ = load_tracker_case("short")
+    z, ch, x, _, _, tt = load_tracker_case("short")
     init = z["init"]
     tr = t.TrackerOracle(ch[0], init[0], init[1], int(init[2]), FS, N)
     trk = _native.Tracker(engine, [ch[0] - 1], [init[0]], [init[1]], [int(init[2])])
     for k in range(300):
-        a, b = t.chunk_times(k, FS, N)
+        a, b = tt[k]
         trk.set_state(0, tr.doppler, tr.carrier_phase, float(tr.phase), tr.code_phase)
         engine.upload_iq(x[k * N:(k + 1) * N])
         rec = trk.process(1, [a])[0, 0]
-        r = tr.step(x[k * N:(k + 1) * N], a, b)
-        scale = abs(r["peak"])
-        assert abs(complex(rec["peak_re"], rec["peak_im"]) - r["peak"]) <= 1e-5 * scale, k
-        assert abs(complex(rec["early_re"], rec["early_im"]) - r["early"]) <= 1e-5 * scale, k
-        assert abs(complex(rec["late_re"], rec["late_im"]) - r["late"]) <= 1e-5 * scale, k
-        assert abs(rec["strength"] - r["strength"]) <= 1e-4 * r["strength"], k
-        assert rec["peak_offset"] == r["peak_offset"] and rec["symbol"] == r["symbol"], k
-        assert rec["code_phase"] == r["code_phase"], k
-        assert abs(rec["disc"] - r["disc"]) <= 1e-4 * max(1.0, abs(r["disc"])), k
-        assert abs(rec["error"] - r["error"]) <= 1e-4 * max(1.0, abs(r["error"])), k
+        assert_ms_matches_oracle(rec, tr.step(x[k * N:(k + 1) * N], a, b), k)
     trk.close()
 
 
@@ -54,12 +45,12 @@ def test_free_running_matches_reference(engine, name):
     """One launch over the whole recording: the reference's pseudosymbol stream, Doppler and phase trajectories."""
     from gypsum_b200 import _native
 
-    z, ch, x, _, _ = load_tracker_case(name)
+    z, ch, x, _, _, tt = load_tracker_case(name)
     init, rows = z["init"], z["rows"]
     n_ms = len(rows)
     trk = _native.Tracker(engine, [ch[0] - 1], [init[0]], [init[1]], [int(init[2])])
     engine.upload_iq(x)
-    rec = trk.process(n_ms, start_times(n_ms, FS, N))[0]
+    rec = trk.process(n_ms, tt[:n_ms, 0])[0]
     trk.close()
     # histories (tracker.py:352-353) carry the value BEFORE the 6-second adjustment of :380-387 (recorded columns 12, 13)
     assert_follows_reference(rec, rows, histories=True)
@@ -73,12 +64,12 @@ def test_free_running_matches_reference(engine, name):
 def test_noise_channel_loses_lock_at_the_six_second_check(engine):
     from gypsum_b200 import _native
 
-    z, ch, x, _, _ = load_tracker_case("noise")
+    z, ch, x, _, _, tt = load_tracker_case("noise")
     init = z["init"]
     n_ms = int(z["n_ms"])
     trk = _native.Tracker(engine, [ch[0] - 1], [init[0]], [init[1]], [int(init[2])])
     engine.upload_iq(x)
-    rec = trk.process(n_ms, start_times(n_ms, FS, N))[0]
+    rec = trk.process(n_ms, tt[:, 0])[0]
     assert int(np.flatnonzero(rec["lost"] == 1)[0]) == int(z["lost_at"]) == 6000
     assert (rec["lost"][6001:] == 2).all() and trk.get_state(0)["lost"] == 1
     trk.close()
@@ -117,7 +108,7 @@ def test_drop_in_tracker_class(engine):
     from gypsum_b200.satellite import GpsSatellite
     from gypsum_b200.tracker import (GpsSatelliteTracker, GpsSatelliteTrackingParameters, NavigationBitPseudosymbol)
 
-    z, ch, x, _, _ = load_tracker_case("short")
+    z, ch, x, _, _, _ = load_tracker_case("short")
     init, rows = z["init"], z["rows"]
     codes = generate_replica_prn_signals()
     sat = GpsSatellite(GpsSatelliteId(ch[0]), codes[GpsSatelliteId(ch[0])], 2)
@@ -173,14 +164,14 @@ import sys
 sys.path[:0] = [sys.argv[1], sys.argv[1] + "/tests"]
 from gpu_support import make_engine
 from gypsum_b200 import _native
-from tracker_support import assert_follows_reference, load_tracker_case, start_times
+from tracker_support import assert_follows_reference, load_tracker_case
 
-z, ch, x, n, fs = load_tracker_case("fs4")
+z, ch, x, n, fs, tt = load_tracker_case("fs4")
 init, rows = z["init"], z["rows"]
 eng = make_engine(fs, n)
 eng.upload_iq(x)
 trk = _native.Tracker(eng, [ch[0] - 1], [init[0]], [init[1]], [int(init[2])])
-rec = trk.process(len(rows), start_times(len(rows), fs, n))[0]
+rec = trk.process(len(rows), tt[:len(rows), 0])[0]
 assert_follows_reference(rec, rows)
 print("fs4 ok")
 """

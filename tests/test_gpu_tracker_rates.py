@@ -5,10 +5,10 @@ k_track_channels_wide at S = 5 .. 16 (tracker.cu), against the tracker oracle an
 import numpy as np
 import pytest
 
-from gpu_support import EngineCache, run_child
+from gpu_support import Attrs, EngineCache, run_child
 from oracle import gypsum_oracle as o
 from oracle import tracker_oracle as t
-from tracker_support import assert_follows_reference, load_tracker_case, start_times
+from tracker_support import assert_follows_reference, assert_ms_matches_oracle, load_tracker_case, start_times
 
 pytestmark = pytest.mark.gpu
 RATES = [1, 3, 5, 6, 8, 10, 12, 16]
@@ -51,32 +51,78 @@ def engines(native_lib):
     cache.close()
 
 
-@pytest.mark.parametrize("s", RATES)
-def test_teacher_forced_correlators_at_every_rate(engines, s):
-    """Each millisecond starts from the oracle's loop state: early / late / prompt outputs and the updated state."""
+def _code_phase_geometry(s):
+    """(name, code phase) of every edge of the early / prompt / late lags at S = s: phases 0 and N - 1, where p -+ 1 wraps;
+    one phase on every polyphase branch p mod S; phases of N and above at S = 1; and the negative and >= 2046 phases that
+    int() of an overshooting DLL accumulator gives (tracker.py:298-303)."""
+    n = 1023 * s
+    cases = [("zero", 0), ("one", 1), ("n-2", n - 2), ("n-1", n - 1)]
+    cases += [(f"branch{r}", s * ((311 + 97 * r) % 1023) + r) for r in range(s)]
+    cases += [("p2045", 2045)] + ([(f"p{p}", p) for p in (1023, 1024, 1535, 2044)] if s == 1 else [])
+    cases += [("minus1", -1), ("minus2", -2), ("p2046", 2046), ("p2047", 2047)]
+    seen, out = set(), []
+    for name, p in cases:
+        if p not in seen:
+            seen.add(p)
+            out.append(pytest.param(s, name, p, id=f"{s}-{name}"))
+    return out
+
+
+def _assert_named_edge(s, name, p):
+    n = 1023 * s
+    if name == "zero":
+        assert p % n == 0  # early lag wraps to N - 1
+    elif name == "n-1":
+        assert p % n == n - 1  # late lag wraps to 0
+    elif name.startswith("branch"):
+        assert p % s == int(name[6:]) and 0 <= p < n  # prompt on branch r, E / L on its neighbours
+    elif name.startswith("minus"):
+        assert p < 0
+    elif name in ("p2046", "p2047"):
+        assert p >= 2046
+    elif s == 1 and name.startswith("p"):
+        assert p >= n  # past N at 1.023 Msps: np.roll is modular
+
+
+GEOMETRY = [c for s in [1, 2, 3, 4, 5, 6, 8, 10, 12, 16] for c in _code_phase_geometry(s)]
+
+
+@pytest.mark.parametrize("s,name,p", GEOMETRY)
+def test_teacher_forced_correlators_at_every_rate(engines, s, name, p):
+    """Each millisecond starts from the oracle's loop state with code phase p and the DLL accumulator the reference's
+    int() and % 2046 leave with it: early / late / prompt outputs, the updated state and |prompt profile|.  The signal
+    sits at p, p - 1 and p + 1, so the prompt, the early or the late tap is the peak: the last two at an amplitude
+    that makes the planted lag the peak in every millisecond, the first at the one the golden rates use (at the prompt,
+    |E| and |L| are nearly equal and their difference must stay above float32 rounding)."""
     from gypsum_b200 import _native
 
+    _assert_named_edge(s, name, p)
     n, fs = 1023 * s, 1023000 * s
-    amp = 0.004 if s < 8 else 0.002
-    x = t.synth_tracking_iq(100 + s, n, 60, fs, [(25, 1500.3, 0.0, 777, 0.3, amp)])
-    tr = t.TrackerOracle(25, 1500.0, 0.0, 777, fs, n)
+    phase = p + 0.3 if p >= 0 else p - 0.3
+    acc = phase % 2046  # int(phase) == p
+    assert int(phase) == p
     eng = engines(n)
-    trk = _native.Tracker(eng, [24], [1500.0], [0.0], [777])
-    for k in range(60):
-        a, b = t.chunk_times(k, fs, n)
-        trk.set_state(0, tr.doppler, tr.carrier_phase, float(tr.phase), tr.code_phase)
-        eng.upload_iq(x[k * n:(k + 1) * n])
-        rec = trk.process(1, [a])[0, 0]
-        r = tr.step(x[k * n:(k + 1) * n], a, b)
-        scale = abs(r["peak"])
-        assert abs(complex(rec["peak_re"], rec["peak_im"]) - r["peak"]) <= 1e-5 * scale, k
-        assert abs(complex(rec["early_re"], rec["early_im"]) - r["early"]) <= 1e-5 * scale, k
-        assert abs(complex(rec["late_re"], rec["late_im"]) - r["late"]) <= 1e-5 * scale, k
-        assert abs(rec["strength"] - r["strength"]) <= 1e-4 * r["strength"], k
-        assert rec["peak_offset"] == r["peak_offset"] and rec["symbol"] == r["symbol"], k
-        assert rec["code_phase"] == r["code_phase"], k
-        assert abs(rec["disc"] - r["disc"]) <= 1e-4 * max(1.0, abs(r["disc"])), k
-        assert abs(rec["error"] - r["error"]) <= 1e-4 * max(1.0, abs(r["error"])), k
+    trk = _native.Tracker(eng, [24], [1500.0], [0.0], [p])
+    tr = t.TrackerOracle(25, 1500.0, 0.0, p, fs, n)
+    for d in (0, -1, 1):
+        amp = 0.01 if d else (0.004 if s < 8 else 0.002)
+        x = t.synth_tracking_iq(100 + s + d, n, 4, fs, [(25, 1500.3, 0.0, p + d, 0.3, amp)])
+        for k in range(4):
+            a, b = t.chunk_times(k, fs, n)
+            tr.code_phase, tr.phase = p, acc
+            trk.set_state(0, tr.doppler, tr.carrier_phase, acc, p)
+            xk = x[k * n:(k + 1) * n]
+            eng.upload_iq(xk)
+            rec, prof = trk.process(1, [a], want_profiles=True)
+            y = xk * np.exp(-1j * (2 * np.pi * tr.doppler * (tr.t1ms + a) + tr.carrier_phase))
+            ref = np.abs(o.correlate_1ms(y, np.roll(tr.prn, p)))
+            r = tr.step(xk, a, b)
+            assert_ms_matches_oracle(rec[0, 0], r, (d, k))
+            if d:  # the early (d = -1) or late tap is the peak, at rolled index N - 1 or 1
+                assert r["peak_offset"] == d % n, (d, k)
+                tap = r["early"] if d < 0 else r["late"]
+                assert abs(abs(tap) - abs(r["peak"])) <= 1e-9 * abs(r["peak"]), (d, k)
+            assert np.abs(prof[0, 0] - ref).max() <= 1e-5 * ref.max(), (d, k)
     trk.close()
 
 
@@ -84,19 +130,19 @@ def test_teacher_forced_correlators_at_every_rate(engines, s):
 def test_free_running_matches_reference_at_other_rates(engines, name):
     from gypsum_b200 import _native
 
-    z, ch, x, n, fs = load_tracker_case(name)
+    z, ch, x, n, fs, tt = load_tracker_case(name)
     init, rows = z["init"], z["rows"]
     n_ms = len(rows)
     eng = engines(n)
     trk = _native.Tracker(eng, [ch[0] - 1], [init[0]], [init[1]], [int(init[2])])
     eng.upload_iq(x)
-    rec = trk.process(n_ms, start_times(n_ms, fs, n))[0]
+    rec = trk.process(n_ms, tt[:n_ms, 0])[0]
     trk.close()
     assert_follows_reference(rec, rows, histories=True)
     assert np.array_equal(rec["doppler"] != rec["doppler_hist"], rows[:, 6] != rows[:, 12])
     if name == "fs16":  # sigma 0.01: the reference reaches is_locked(); the device decides the same milliseconds
         tr = t.TrackerOracle(ch[0], init[0], init[1], int(init[2]), fs, n)
-        want = np.array([tr.step(x[k * n:(k + 1) * n], *t.chunk_times(k, fs, n))["locked"] for k in range(n_ms)])
+        want = np.array([tr.step(x[k * n:(k + 1) * n], *tt[k])["locked"] for k in range(n_ms)])
         assert want.sum() > 0 and rec["locked"].sum() > 0
         assert np.count_nonzero(rec["locked"].astype(bool) != want) <= n_ms // 200
     if name == "fs16_long":  # sigma 0.02: never locked (I-pole variance ~ sigma^2 N / 2 > 2); the 6-s check passes
@@ -175,9 +221,10 @@ def test_drop_in_pool_with_undo_equals_bank_and_bits_at_16368_ksps(native_lib):
         trks[c].close()
 
 
-def test_receiver_flow_at_16368_ksps(tmp_path, native_lib):
-    """file provider -> DeviceSampleRing -> detector -> trackers -> pseudosymbols, step for step against the oracle
-    flow (acquisition and tracking).  Planted code phases stay below 2046, the only ones the reference can keep."""
+def _receiver_flow(tmp_path, s, n_ms=60):
+    """file provider -> DeviceSampleRing (10 ms) -> detector on the full window -> one drop-in tracker per detected
+    satellite, each fed the newest ring slot from the first full window on (the first tracker call is at slot 9).
+    Returns the IQ, {sv: acquisition result}, {sv: pseudosymbols} and the satellites."""
     from gypsum_b200.acquisition import GpsSatelliteDetector
     from gypsum_b200.antenna_sample_provider import (AntennaSampleProviderBackedByFile, DeviceSampleRing, InputFileInfo,
                                                      NoMoreSamplesError)
@@ -185,12 +232,12 @@ def test_receiver_flow_at_16368_ksps(tmp_path, native_lib):
     from gypsum_b200.satellite import GpsSatellite
     from gypsum_b200.tracker import GpsSatelliteTracker, GpsSatelliteTrackingParameters
 
-    n_ms = 60
+    n, fs = 1023 * s, 1023000 * s
     planted = [(25, 1500.3, 0.0, 777, 0.3, 0.004), (7, -2212.7, 0.0, 1900, 1.0, 0.004)]
-    x = t.synth_tracking_iq(44, N16, n_ms + 1, FS16, planted)
+    x = t.synth_tracking_iq(44, n, n_ms + 1, fs, planted)
     path = tmp_path / "recording"
     x.view(np.float32).tofile(path)
-    provider = AntennaSampleProviderBackedByFile(InputFileInfo(path, FS16))
+    provider = AntennaSampleProviderBackedByFile(InputFileInfo(path, fs))
     attrs = provider.get_attributes()
     codes = generate_replica_prn_signals()
     satellites = {sid: GpsSatellite(sid, code, attrs.samples_per_prn_transmission // 1023) for sid, code in codes.items()}
@@ -216,12 +263,56 @@ def test_receiver_flow_at_16368_ksps(tmp_path, native_lib):
             symbols[sv].append(trk.process_samples(chunk).pseudosymbol.as_val())
         k += 1
     assert k == n_ms and sorted(trackers) == [7, 25]  # detector first (acquisition), then the trackers
+    for trk in trackers.values():
+        trk.close()
+    ring.native.close()
+    return x, acq, symbols, satellites
+
+
+def test_receiver_flow_at_16368_ksps(tmp_path, native_lib):
+    """file provider -> DeviceSampleRing -> detector -> trackers -> pseudosymbols, step for step against the oracle
+    flow (acquisition and tracking).  Planted code phases stay below 2046, the only ones the reference can keep."""
+    n_ms = 60
+    x, acq, symbols, _ = _receiver_flow(tmp_path, 16, n_ms)
     first = x[: 10 * N16]
-    for sv, trk in trackers.items():
+    for sv in acq:
         ref = o.acquire_sv(sv, first, FS16, N16)
         assert (ref.doppler, ref.code_phase) == (acq[sv].doppler_shift, acq[sv].prn_phase_shift), sv
         tr = t.TrackerOracle(sv, ref.doppler, ref.carrier_phase, ref.code_phase, FS16, N16)
         want = [tr.step(x[ms * N16:(ms + 1) * N16], *t.chunk_times(ms, FS16, N16))["symbol"] for ms in range(9, n_ms)]
         assert symbols[sv] == want, sv
-        trk.close()
-    ring.native.close()
+
+
+@pytest.mark.parametrize("s", [1, 3, 5])
+def test_receiver_flow_reads_odd_ring_slots_at_odd_n(tmp_path, native_lib, s):
+    """The flow above where N = 1023 S is odd: every other slot of the 10-ms ring starts 8 bytes past a 16-byte boundary,
+    and the trackers read slots 9, 0, 1, ... in turn.  Each tracker's pseudosymbols and final Doppler == a TrackerBank
+    seeded with the same acquisition and fed the same milliseconds by upload, bit for bit; and == the float64 oracle
+    tracker from that acquisition, bar symbols where the oracle's in-phase prompt is float32 noise around zero.  The
+    acquisition equals the oracle's in code phase; a different Doppler bin must be proved a near-tie (its non-coherent
+    peak within 1e-5 of the oracle bin's on the oracle's own float64 profiles), as the acquisition tests do."""
+    from gypsum_b200.gps_ca_prn_codes import GpsSatelliteId
+    from gypsum_b200.tracker import TrackerBank
+
+    n_ms = 60
+    n, fs = 1023 * s, 1023000 * s
+    x, acq, symbols, satellites = _receiver_flow(tmp_path, s, n_ms)
+    first = x[: 10 * n]
+    tt = np.array([t.chunk_times(ms, fs, n) for ms in range(9, n_ms)])
+    for sv, r in acq.items():
+        ref = o.acquire_sv(sv, first, fs, n)
+        assert r.prn_phase_shift == ref.code_phase, sv
+        if r.doppler_shift != ref.doppler:
+            prn = o.replica(sv, n)
+            here = o.integrate(o.NON_COHERENT, first, fs, n, r.doppler_shift, prn).max()
+            there = o.integrate(o.NON_COHERENT, first, fs, n, ref.doppler, prn).max()
+            assert here >= there * (1 - 1e-5), (sv, r.doppler_shift, ref.doppler)
+        seed = (r.doppler_shift, r.carrier_wave_phase_shift, r.prn_phase_shift)
+        bank = TrackerBank([(satellites[GpsSatelliteId(sv)], *seed)], Attrs(fs, n))
+        rec = bank.process(x[9 * n:n_ms * n], tt[:, 0])[0]
+        assert symbols[sv] == list(rec["symbol"]), sv
+        tr = t.TrackerOracle(sv, *seed, fs, n)
+        got = [tr.step(x[ms * n:(ms + 1) * n], *tt[ms - 9]) for ms in range(9, n_ms)]
+        scale = max(abs(g["peak"].real) for g in got)
+        for k, g in enumerate(got):
+            assert symbols[sv][k] == g["symbol"] or abs(g["peak"].real) <= 1e-4 * scale, (sv, k)

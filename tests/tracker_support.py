@@ -10,14 +10,21 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def load_tracker_case(name):
-    """(golden file, channel, IQ, n, fs) of tracker_<name>.npz, the IQ re-synthesised from the recorded seed.  A file
-    that records no n / fs is at 2.046 Msps."""
+    """(golden file, channel, IQ, n, fs, times) of tracker_<name>.npz, the IQ re-synthesised from the recorded seed and
+    times[k] = (start, end) of millisecond k.  A file that records no n / fs is at 2.046 Msps; one that records no start
+    times starts at 0 without gaps.  A file that records them (a late join, a gap, long stream times) has its samples
+    synthesised from the first start time on."""
     z = np.load(os.path.join(GOLDEN, f"tracker_{name}.npz"))
     ch = z["channel"]
     ch = (int(ch[0]), ch[1], ch[2], int(ch[3]), ch[4], ch[5])
     n, fs = (int(z["n"]), int(z["fs"])) if "n" in z.files else (2046, 2046000)
-    x = t.synth_tracking_iq(int(z["seed"]), n, int(z["n_ms"]), fs, [ch], float(z["sigma"]))
-    return z, ch, x, n, fs
+    n_ms = int(z["n_ms"])
+    if "start_times" in z.files:
+        times = np.stack([z["start_times"], z["end_times"]], axis=1)
+    else:
+        times = np.array([t.chunk_times(k, fs, n) for k in range(n_ms)])
+    x = t.synth_tracking_iq(int(z["seed"]), n, n_ms, fs, [ch], float(z["sigma"]), t0=float(times[0, 0]))
+    return z, ch, x, n, fs, times
 
 
 def start_times(n_ms, fs, n):
@@ -30,6 +37,21 @@ def oracle_row(tr, r):
     return np.array([r["peak"].real, r["peak"].imag, r["strength"], r["symbol"], r["error"], r["disc"], r["doppler"],
                      r["carrier_phase"], r["code_phase"], r["start"], r["end"], tr.phase, r["doppler_hist"],
                      r["carrier_phase_hist"]], dtype=np.float64)
+
+
+def assert_ms_matches_oracle(rec, r, k):
+    """One teacher-forced millisecond: device record rec against the oracle's step result r from the same state.
+    Correlator outputs within 1e-5 of the prompt peak's magnitude (float32 against float64), strength, disc and error
+    within 1e-4, peak offset, symbol and code phase exact."""
+    scale = abs(r["peak"])
+    assert abs(complex(rec["peak_re"], rec["peak_im"]) - r["peak"]) <= 1e-5 * scale, k
+    assert abs(complex(rec["early_re"], rec["early_im"]) - r["early"]) <= 1e-5 * scale, k
+    assert abs(complex(rec["late_re"], rec["late_im"]) - r["late"]) <= 1e-5 * scale, k
+    assert abs(rec["strength"] - r["strength"]) <= 1e-4 * r["strength"], k
+    assert rec["peak_offset"] == r["peak_offset"] and rec["symbol"] == r["symbol"], k
+    assert rec["code_phase"] == r["code_phase"], k
+    assert abs(rec["disc"] - r["disc"]) <= 1e-4 * max(1.0, abs(r["disc"])), k
+    assert abs(rec["error"] - r["error"]) <= 1e-4 * max(1.0, abs(r["error"])), k
 
 
 def _assert_phase_close(got, want, tol):

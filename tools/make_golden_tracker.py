@@ -23,10 +23,14 @@ OUT = os.path.join(ROOT, "tests", "golden")
 N, FS = 2046, 2046000
 
 
-def run(name, seed, n_ms, channel, init, sigma=0.02, N=N, FS=FS):
+def run(name, seed, n_ms, channel, init, sigma=0.02, N=N, FS=FS, ms_of=None):
+    """ms_of(k): the stream millisecond whose timestamps chunk k carries (default k).  A case with ms_of records its
+    start / end times, and its samples are synthesised from the first chunk's start time on (a later gap in the times
+    is a gap in the timestamps only)."""
     codes = generate_replica_prn_signals()
     sv = channel[0]
-    x = t.synth_tracking_iq(seed, N, n_ms, FS, [channel], sigma)
+    times = [t.chunk_times(k if ms_of is None else ms_of(k), FS, N) for k in range(n_ms)]
+    x = t.synth_tracking_iq(seed, N, n_ms, FS, [channel], sigma, t0=times[0][0])
     # prn_as_complex is lru-cached per satellite id (satellite.py:20-21): a cached replica of another rate would collide
     GpsSatellite.prn_as_complex.fget.cache_clear()
     sat = GpsSatellite(GpsSatelliteId(sv), codes[GpsSatelliteId(sv)], N // 1023)
@@ -36,7 +40,7 @@ def run(name, seed, n_ms, channel, init, sigma=0.02, N=N, FS=FS):
     trk = GpsSatelliteTracker(params, SampleProviderAttributes(FS, N))
     rows, lost_at = [], -1
     for k in range(n_ms):
-        t0, t1 = t.chunk_times(k, FS, N)
+        t0, t1 = times[k]
         try:
             ps = trk.process_samples(AntennaSampleChunk(t0, t1, x[k * N:(k + 1) * N]))
         except LostSatelliteLockError:
@@ -50,10 +54,12 @@ def run(name, seed, n_ms, channel, init, sigma=0.02, N=N, FS=FS):
                      # what the reference APPENDS to its histories (tracker.py:352-353): the values before the 6-second
                      # constellation adjustment of :370-387, which only the current_* fields above include
                      params.doppler_shifts[-1], params.carrier_wave_phases[-1]])
+    extra = {} if ms_of is None else {"start_times": np.array(times, dtype=np.float64)[:, 0],
+                                      "end_times": np.array(times, dtype=np.float64)[:, 1]}
     np.savez_compressed(os.path.join(OUT, f"tracker_{name}.npz"), seed=np.int64(seed), n_ms=np.int64(n_ms),
                         channel=np.array(channel, dtype=np.float64), init=np.array(init, dtype=np.float64),
                         sigma=np.float64(sigma), rows=np.array(rows, dtype=np.float64), lost_at=np.int64(lost_at),
-                        n=np.int64(N), fs=np.int64(FS))
+                        n=np.int64(N), fs=np.int64(FS), **extra)
     r = np.array(rows)
     print(name, "ms", len(rows), "lost_at", lost_at, "final doppler", r[-1, 6], "symbols +/-", (r[:, 3] > 0).sum(), (r[:, 3] < 0).sum())
 
@@ -78,6 +84,23 @@ CASES = {
     # ... and never at sigma = 0.02; this one crosses the 6-second constellation check
     "fs16_long": lambda: run("fs16_long", 34, 6100, (12, 640.4, 0.0, 1501, 0.7, 0.001), (640.0, 0.0, 1501), N=16368,
                              FS=16368000),
+    # Channels that join late, and stream times far from 0.  The 6-second check compares a chunk's start time with the
+    # time of the last check, which starts at 0 (tracker.py:221-222, :370-374).
+    # joins at 5.5 s: the 6.0-s check sees the 501 peaks since the join and the -+5 Hz / +-pi/2 nudge fires
+    "join55": lambda: run("join55", 21, 700, (9, 432.1, 0.0, 300, 0.4, 0.0016), (430.0, 0.0, 300), ms_of=lambda k: 5500 + k),
+    # joins at exactly 6.0 s: the check runs on the first millisecond (one peak: nothing to do), then at 12.0 s (nudge)
+    "join6": lambda: run("join6", 21, 6100, (9, 432.1, 0.0, 300, 0.4, 0.0016), (430.0, 0.0, 300), ms_of=lambda k: 6000 + k),
+    # no signal, joins at 5.75 s: the 6.0-s check on 251 peaks loses it
+    "join575_noise": lambda: run("join575_noise", 13, 300, (3, 800.0, 0.0, 5, 0.0, 0.0), (800.0, 0.0, 5),
+                                 ms_of=lambda k: 5750 + k),
+    # a 7-s gap in the start times after 600 ms: the check fires on the first millisecond after it (nudge)
+    "gap": lambda: run("gap", 23, 1200, (9, 432.1, 0.0, 300, 0.4, 0.003), (430.0, 0.0, 300),
+                       ms_of=lambda k: k if k < 600 else k + 7000),
+    # stream times near one hour and one day: checks at the join (one peak) and 6 s later (nothing to do)
+    "hour": lambda: run("hour", 24, 6100, (25, 1500.3, 0.0, 777, 0.3, 0.004), (1500.0, 0.0, 777),
+                        ms_of=lambda k: 3599500 + k),
+    "day": lambda: run("day", 25, 6100, (25, 1500.3, 0.0, 777, 0.3, 0.004), (1500.0, 0.0, 777),
+                       ms_of=lambda k: 86399500 + k),
 }
 
 if __name__ == "__main__":
