@@ -87,6 +87,8 @@ SYMBOLS = {
     "gb200_tracker_receiver_state": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_int32), _P]),
     "gb200_tracker_fix_repairs": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "gb200_tracker_set_fix_solver": (C.c_int, [_P, C.c_int]),
+    "gb200_tracker_velocity_fixes": (C.c_int, [_P, _P, _P, _P]),
+    "gb200_tracker_velocity_fixes_device": (C.c_int, [_P, _P, _P, _P]),
     "gb200_tracker_chain_sizes": (C.c_int, [_P, _P]),
     "gb200_set_fused": (C.c_int, [_P, C.c_int]),
     "gb200_launch_count": (C.c_int, [_P, C.POINTER(C.c_int64)]),
@@ -663,6 +665,22 @@ class Tracker:
         self._engine._check(self._lib.gb200_tracker_position_fixes_device(self._h, _ptr(rx), _P(out_device_ptr)),
                             "gb200_tracker_position_fixes_device")
 
+    def velocity_fixes(self, doppler_device_ptr=None, fixes_device_ptr=None) -> np.ndarray:
+        """VELOCITY_DTYPE [n_ms]: velocity, clock drift, geodetic position and DOP of every millisecond of the last
+        parse_subframes call with a solved position fix (gb200_tracker_velocity_fixes).  doppler_device_ptr: a device
+        float64 [n_channels, n_ms] Doppler in Hz, or None for the tracking records of the process call behind that parse
+        call; fixes_device_ptr: the fix records on the device, or None for those the last position_fixes call kept."""
+        out = np.empty(self._chain_sizes()[2], dtype=VELOCITY_DTYPE)
+        self._engine._check(self._lib.gb200_tracker_velocity_fixes(self._h, _P(doppler_device_ptr), _P(fixes_device_ptr),
+                                                                   _ptr(out)), "gb200_tracker_velocity_fixes")
+        return out
+
+    def velocity_fixes_device(self, out_device_ptr: int, doppler_device_ptr=None, fixes_device_ptr=None) -> None:
+        """Enqueue only: n_ms VELOCITY_DTYPE records to device memory."""
+        self._engine._check(self._lib.gb200_tracker_velocity_fixes_device(self._h, _P(doppler_device_ptr),
+                                                                          _P(fixes_device_ptr), _P(out_device_ptr)),
+                            "gb200_tracker_velocity_fixes_device")
+
     def receiver_state(self) -> dict:
         """After the last fix call: slide (receiver_clock_slide, None before any), stopped, order: the channels in
         the world model's order, and repaired: the fixes the serial chain recomputed where the parallel passes' chain
@@ -727,6 +745,13 @@ FIX_DTYPE = np.dtype([  # gb200_position_fix
 assert FIX_DTYPE.itemsize == 112
 FIX_NONE, FIX_SOLVED, FIX_RAISED, FIX_STOPPED = 0, 1, 2, 3  # FIX_DTYPE["status"]
 FIX_SOLVERS = {"reference": 0, "least_squares": 1}  # GB200_FIX_SOLVER_*
+VELOCITY_DTYPE = np.dtype([  # gb200_velocity_fix
+    ("receiver_timestamp", "<f8"), ("vx", "<f8"), ("vy", "<f8"), ("vz", "<f8"), ("clock_drift", "<f8"),
+    ("latitude_deg", "<f8"), ("longitude_deg", "<f8"), ("height", "<f8"), ("gdop", "<f8"), ("pdop", "<f8"),
+    ("hdop", "<f8"), ("vdop", "<f8"), ("tdop", "<f8"), ("residual_rms", "<f8"), ("status", "<i4"), ("n_rows", "<i4"),
+    ("reserved", "<i4", (2,))])
+assert VELOCITY_DTYPE.itemsize == 128
+VEL_NONE, VEL_SOLVED, VEL_UNSOLVABLE = 0, 1, 2  # VELOCITY_DTYPE["status"]
 
 
 def subframe_event_capacity(n_bits: int) -> int:

@@ -17,6 +17,7 @@
 #include "bits_core.cuh"
 #include "kernels.cuh"
 #include "fix_core.cuh"
+#include "velocity_core.cuh"
 #include "nav_core.cuh"
 #include "orbit_core.cuh"
 
@@ -172,9 +173,13 @@ struct TrackerChain {
     Output orbit;      // the change tables of the last parse call: stride and n_ms (0 = no parse call yet)
     bool fix_pending = false;  // the last parse call's fixes are not computed yet
     bool fix_gap = false;      // a parse call's fixes were skipped after the first fix call: for the tracker's lifetime
+    bool parse_records = false;  // the last parse call came from the records still in d_out (their Dopplers)
 
     // the records are about to be rewritten: nothing behind them is on the chain any more; pending bits stay pending
-    void process_begin() { records.n_ms = bits.n_ms = subframes.n_ms = 0; }
+    void process_begin() {
+        records.n_ms = bits.n_ms = subframes.n_ms = 0;
+        parse_records = false;
+    }
     void processed(int n_ms) { records.n_ms = n_ms; }  // whole-bank calls only
     void integrated(const int* counts, int nc, int stride, bool own_records) {
         bits = {{counts, counts + nc}, stride, own_records ? records.n_ms : 0, true};
@@ -187,6 +192,7 @@ struct TrackerChain {
     // fixing_began: the receiver state exists (a fix call has run)
     void parsed(int n_ms, int change_stride, bool own_subframes, bool fixing_began) {
         if (own_subframes) subframes.pending = false;
+        parse_records = own_subframes;
         orbit.n_ms = n_ms;
         orbit.stride = change_stride;
         if (fixing_began && fix_pending) fix_gap = true;
@@ -246,7 +252,12 @@ struct gb200_tracker {
         DevBuf<FixRecord> d_fixes;
         PinnedBuf<double> h_rx;
         PinnedBuf<FixRecord> h_fixes;
+        bool kept = false;  // d_fixes holds the last fix call's records (gb200_tracker_position_fixes, not _device)
     } fix;
+    struct {  // velocity.cu
+        DevBuf<VelocityRecord> d_out;
+        PinnedBuf<VelocityRecord> h_out;
+    } vel;
 };
 // A pipelined stream of grid batches: slot k's host->device copy, compute and device->host copy run on three streams.
 struct gb200_grid_stream {
@@ -299,6 +310,13 @@ static_assert(sizeof(gb200_position_fix) == sizeof(FixRecord) &&
                   offsetof(gb200_position_fix, status) == offsetof(FixRecord, status) &&
                   offsetof(gb200_position_fix, channel) == offsetof(FixRecord, channel),
               "ABI position fix and device fix must match");
+static_assert(sizeof(gb200_velocity_fix) == sizeof(VelocityRecord) &&
+                  offsetof(gb200_velocity_fix, residual_rms) == offsetof(VelocityRecord, residual_rms) &&
+                  offsetof(gb200_velocity_fix, status) == offsetof(VelocityRecord, status) &&
+                  offsetof(gb200_velocity_fix, n_rows) == offsetof(VelocityRecord, n_rows),
+              "ABI velocity fix and device velocity fix must match");
+static_assert(offsetof(TrackMsRecord, doppler) == 0 && sizeof(TrackMsRecord) % sizeof(double) == 0,
+              "the velocity fix reads the tracking records' Doppler with a stride in doubles");
 static_assert(offsetof(gb200_subframe_event, words) == offsetof(SubframeEvent, words) &&
                   offsetof(gb200_subframe_event, kind) == offsetof(SubframeEvent, kind) &&
                   offsetof(gb200_subframe_event, parity_ok) == offsetof(SubframeEvent, parity_ok),
@@ -1855,7 +1873,9 @@ int gb200_tracker_position_fixes_device(gb200_tracker* t, const double* receiver
     if (!t) return GB200_EINVAL;
     if (!out_device) GB_FAIL(t->e, GB200_EINVAL, "null output");
     GB_CUDA(t->e, cudaSetDevice(t->e->device));
-    return fixes_launch(t, receiver_timestamps_host, static_cast<FixRecord*>(out_device));
+    GB_TRY(fixes_launch(t, receiver_timestamps_host, static_cast<FixRecord*>(out_device)));
+    t->fix.kept = false;
+    return GB200_OK;
 }
 
 int gb200_tracker_position_fixes(gb200_tracker* t, const double* receiver_timestamps_host, gb200_position_fix* out_host) {
@@ -1867,7 +1887,67 @@ int gb200_tracker_position_fixes(gb200_tracker* t, const double* receiver_timest
     const size_t n = static_cast<size_t>(t->chain.orbit.n_ms);
     if (n) GB_CUDA(e, s.d_fixes.ensure(n));
     GB_TRY(fixes_launch(t, receiver_timestamps_host, s.d_fixes.p));
+    s.kept = true;
     return download(e, reinterpret_cast<FixRecord*>(out_host), s.d_fixes.p, n, s.h_fixes);
+}
+
+// The velocity fixes of the last parse call (velocity.cu), enqueued into out_dev.  Reads what the fix call left on the
+// device and changes nothing.
+static int velocity_launch(gb200_tracker* t, const double* doppler_dev, const void* fixes_dev, VelocityRecord* out_dev) {
+    gb200_engine* e = t->e;
+    const int n_ms = t->chain.orbit.n_ms;
+    if (!n_ms) GB_FAIL(e, GB200_ESTATE, "no gb200_tracker_parse_subframes call yet");
+    if (t->chain.fix_pending)
+        GB_FAIL(e, GB200_ESTATE, "the position fixes of the last parse call are not computed yet (call gb200_tracker_position_fixes)");
+    if (!fixes_dev && !t->fix.kept)
+        GB_FAIL(e, GB200_ESTATE, "the last fix call wrote its records to caller memory (gb200_tracker_position_fixes_device): "
+                                 "pass that buffer as fixes_device");
+    if (!doppler_dev && !t->chain.parse_records)
+        GB_FAIL(e, GB200_ESTATE, "the tracking records behind the last parse call are not on the device (it was fed a "
+                                 "caller's events, or a later process call replaced them): pass doppler_device");
+    VelocityArgs a{};
+    a.fixes = fixes_dev ? static_cast<const FixRecord*>(fixes_dev) : t->fix.d_fixes.p;
+    a.obs = t->orbit.d_obs.p;
+    a.changes = t->orbit.d_changes.p;
+    a.change_counts = t->orbit.d_change_counts.p;
+    a.change_stride = t->chain.orbit.stride;
+    if (doppler_dev) {
+        a.doppler = doppler_dev;
+        a.doppler_channel_stride = n_ms;
+        a.doppler_ms_stride = 1;
+    } else {  // TrackMsRecord::doppler of [channel][n_ms] records
+        constexpr int kRecordDoubles = sizeof(TrackMsRecord) / sizeof(double);
+        a.doppler = &t->d_out.p[0].doppler;
+        a.doppler_channel_stride = static_cast<long long>(kRecordDoubles) * n_ms;
+        a.doppler_ms_stride = kRecordDoubles;
+    }
+    a.order = t->fix.order.p;
+    a.bank = t->fix.bank.p;
+    a.out = out_dev;
+    a.n_ms = n_ms;
+    GB_LAUNCH(e, -1, launch_velocity_fixes(a, e->stream));
+    return GB200_OK;
+}
+
+int gb200_tracker_velocity_fixes_device(gb200_tracker* t, const double* doppler_device, const void* fixes_device,
+                                        void* out_device) {
+    if (!t) return GB200_EINVAL;
+    if (!out_device) GB_FAIL(t->e, GB200_EINVAL, "null output");
+    GB_CUDA(t->e, cudaSetDevice(t->e->device));
+    return velocity_launch(t, doppler_device, fixes_device, static_cast<VelocityRecord*>(out_device));
+}
+
+int gb200_tracker_velocity_fixes(gb200_tracker* t, const double* doppler_device, const void* fixes_device,
+                                 gb200_velocity_fix* out_host) {
+    if (!t) return GB200_EINVAL;
+    gb200_engine* e = t->e;
+    auto& s = t->vel;
+    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
+    GB_CUDA(e, cudaSetDevice(e->device));
+    const size_t n = static_cast<size_t>(t->chain.orbit.n_ms);
+    if (n) GB_CUDA(e, s.d_out.ensure(n));
+    GB_TRY(velocity_launch(t, doppler_device, fixes_device, s.d_out.p));
+    return download(e, reinterpret_cast<VelocityRecord*>(out_host), s.d_out.p, n, s.h_out);
 }
 
 int gb200_tracker_set_fix_solver(gb200_tracker* t, int solver) {

@@ -167,6 +167,24 @@ struct FixArgs {
 };
 cudaError_t launch_position_fixes(const FixArgs& a, cudaStream_t st);
 
+// velocity_fixes: velocity, clock drift, geodetic position and DOP of every solved fix (velocity.cu, velocity_core.cuh).
+struct VelocityRecord;
+struct VelocityArgs {
+    const FixRecord* fixes;             // [n_ms] the position fixes of the last parse call
+    const SvObservation* obs;           // [n_channels][n_ms] the observations the fix call computed
+    const OrbitSnap* changes;           // the last parse call's change tables, [n_channels][change_stride]
+    const int* change_counts;           // [n_channels]
+    int change_stride;
+    const double* doppler;              // channel c, millisecond m at c * doppler_channel_stride + m * doppler_ms_stride
+    long long doppler_channel_stride;   // (in doubles: a caller's [n_channels][n_ms] array or the tracking records)
+    int doppler_ms_stride;
+    const int* order;                   // [n_channels] the fix call's world-model order
+    const FixBank* bank;                // its n_touched
+    VelocityRecord* out;                // [n_ms]
+    int n_ms;
+};
+cudaError_t launch_velocity_fixes(const VelocityArgs& a, cudaStream_t st);
+
 // acquire_fused: one CTA per (PRN, Doppler) cell, the whole pipeline in one kernel (fused.cu).
 struct FusedArgs {
     const float2* iq;       // [M*N] one block

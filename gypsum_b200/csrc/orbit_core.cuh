@@ -337,6 +337,59 @@ GB_HD inline void orbit_position(const double* p, double tow, double& x, double&
     z = o_mul(yp, sin(ik));
 }
 
+// The time derivative of orbit_position at the same tow, in the same frame (Omega's rate includes -omega_e; no Sagnac
+// term, as the position fix has none), and of orbit_time_of_week's clock correction dsv: the satellite's ECEF velocity
+// (m/s) and clock drift (s/s).  Ek is the same seven-iteration value, and Ek' = n / (1 - e cos Ek) that of Kepler's
+// equation.  The drift differentiates the reference's own dsv expression: af1 + 2 af2^2 (t - toc) + F e sqrtA cos(Ek) Ek'.
+// The af2^2 is the reference's pow(af2 * (t - toc), 2) (world_model.py:686), where IS-GPS-200 has af2 (t - toc)^2; t is
+// taken as tow, which differs from the reference's uncorrected t by dsv (< 1 ms).  Like dsv, the relativistic term takes
+// Ek at tow - toe without the week wrap.
+GB_HD inline void orbit_velocity(const double* p, double tow, double& vx, double& vy, double& vz, double& drift) {
+    const double tk0 = o_sub(tow, p[kToe]);
+    double tk = tk0;
+    if (tk > 302400.0) tk = o_sub(tk, 604800.0);
+    else if (tk < -302400.0) tk = o_add(tk, 604800.0);
+    const double e = p[kEccentricity];
+    const double n = orbit_mean_motion(p);
+    const double ek = orbit_eccentric_anomaly(p, n, tk);
+    const double se = sin(ek), ce = cos(ek);
+    const double den = o_sub(1.0, o_mul(e, ce));
+    const double ekd = n / den;
+    const double sq = sqrt(o_sub(1.0, o_mul(e, e)));
+    const double vk = atan2(o_mul(sq, se), o_sub(ce, e));
+    const double vkd = o_mul(sq, ekd) / den;  // d(vk)/dt
+    const double phi = o_add(vk, p[kArgumentOfPerigee]);
+    const double s2 = sin(o_mul(2.0, phi)), c2 = cos(o_mul(2.0, phi));
+    const double duk = o_add(o_mul(p[kCus], s2), o_mul(p[kCuc], c2));
+    const double drk = o_add(o_mul(p[kCrs], s2), o_mul(p[kCrc], c2));
+    const double dik = o_add(o_mul(p[kCis], s2), o_mul(p[kCic], c2));
+    const double w2 = o_mul(2.0, vkd);
+    const double uk = o_add(phi, duk);
+    const double ukd = o_add(vkd, o_mul(w2, o_sub(o_mul(p[kCus], c2), o_mul(p[kCuc], s2))));
+    const double rk = o_add(o_mul(p[kSemiMajorAxis], o_sub(1.0, o_mul(e, ce))), drk);
+    const double rkd = o_add(o_mul(o_mul(o_mul(p[kSemiMajorAxis], e), se), ekd), o_mul(w2, o_sub(o_mul(p[kCrs], c2), o_mul(p[kCrc], s2))));
+    const double ik = o_add(o_add(p[kInclination], o_mul(p[kRateOfInclination], tk)), dik);
+    const double ikd = o_add(p[kRateOfInclination], o_mul(w2, o_sub(o_mul(p[kCis], c2), o_mul(p[kCic], s2))));
+    const double cu = cos(uk), su = sin(uk);
+    const double xp = o_mul(rk, cu), yp = o_mul(rk, su);
+    const double xpd = o_sub(o_mul(rkd, cu), o_mul(o_mul(rk, ukd), su));
+    const double ypd = o_add(o_mul(rkd, su), o_mul(o_mul(rk, ukd), cu));
+    const double omd = o_sub(p[kRateOfRightAscension], kEarthRotationRate);
+    const double om = o_sub(o_add(p[kLongitudeOfAscendingNode], o_mul(omd, tk)), o_mul(kEarthRotationRate, p[kToe]));
+    const double so = sin(om), co = cos(om), ci = cos(ik), si = sin(ik);
+    const double x = o_sub(o_mul(xp, co), o_mul(o_mul(yp, ci), so));
+    const double y = o_add(o_mul(xp, so), o_mul(o_mul(yp, ci), co));
+    const double yi = o_mul(o_mul(yp, si), ikd);  // d(cos ik)/dt = -sin(ik) ik'
+    vx = o_sub(o_add(o_sub(o_mul(xpd, co), o_mul(o_mul(ypd, ci), so)), o_mul(yi, so)), o_mul(y, omd));
+    vy = o_add(o_sub(o_add(o_mul(xpd, so), o_mul(o_mul(ypd, ci), co)), o_mul(yi, co)), o_mul(x, omd));
+    vz = o_add(o_mul(ypd, si), o_mul(o_mul(yp, ci), ikd));
+    const double tc = o_sub(tow, p[kToc]);
+    const double ec = tk == tk0 ? ek : orbit_eccentric_anomaly(p, n, tk0);
+    const double cc = tk == tk0 ? ce : cos(ec);
+    const double rel = o_mul(o_mul(o_mul(o_mul(kRelativisticF, e), p[kSqrtA]), cc), n / o_sub(1.0, o_mul(e, cc)));
+    drift = o_add(o_add(p[kAf1], o_mul(o_mul(2.0, o_mul(p[kAf2], p[kAf2])), tc)), rel);
+}
+
 // What the world model knows about one satellite at the end of millisecond m (>= s.ms, with no change in between).
 GB_HD inline void orbit_observe(const OrbitSnap& s, int m, SvObservation& o) {
     const long long count = orbit_count_at(s, m);

@@ -398,6 +398,15 @@ class TrackerBank:
         gypsum_b200.world_model.solution_from_fix turns a status-1 record into a ReceiverSolution."""
         return self.native.position_fixes(start_times)
 
+    def velocity_fixes(self) -> np.ndarray:
+        """_native.VELOCITY_DTYPE [ms] over the milliseconds of the last parse_subframes call, after position_fixes: the
+        receiver's ECEF velocity (m/s) and clock drift (s/s) from the channels' tracker Dopplers of the last `process`
+        call, solved by least squares over the rows of each solved fix, with the fix's WGS-84 latitude, longitude and
+        height and the GDOP / PDOP / HDOP / VDOP / TDOP of its geometry (DESIGN.md §8d).  status 1: solved (residual_rms
+        with more than four rows); 0: no solved fix at that millisecond; 2: rank-deficient rows or a non-finite input,
+        where only the geodetic position is set."""
+        return self.native.velocity_fixes()
+
 
 # OrbitalParameterType (world_model.py:151-199), in order
 ORBITAL_PARAMETER_NAMES = (

@@ -421,6 +421,46 @@ int gb200_tracker_receiver_state(gb200_tracker* t, double* slide, int32_t* stopp
  * differed in any bit from the slide the fix before them left.  A receiver-clock jump inside a segment (a gap in the
  * sample stream) is an input that makes the check fail. */
 int gb200_tracker_fix_repairs(gb200_tracker* t, int64_t* n);
+
+/* The receiver's velocity and clock drift, geodetic position and dilution of precision at one millisecond with a
+ * solved position fix (128 bytes; DESIGN.md §8d).  The rows are the fix's: channel[0..3] of a four-row fix, every
+ * ready channel in world-model order for a least-squares fix of more.  Row i is -u_i . v + c drift = rho'_i - u_i . v_sv,i
+ * + c drift_sv,i, u_i the line of sight from the fix position to the satellite, rho'_i = -(c / 1575.42 MHz) * Doppler_i
+ * the measured range rate and v_sv, drift_sv the satellite's velocity and clock drift from its ephemeris; solved by least
+ * squares in the fix's frame (ECEF, no Sagnac term).  DOP is (G^T G)^-1 of the rows G_i = [-u_i, 1] in east/north/up
+ * at the geodetic position.  status:
+ *   0  no solved position fix at this millisecond: every number is NaN
+ *   1  solved: residual_rms is set with more than four rows (NaN with four)
+ *   2  not solvable (rank < 4, or a non-finite input in a row): velocity, drift and DOP are NaN; latitude, longitude
+ *      and height are set
+ * Values that are not set are NaN. */
+typedef struct gb200_velocity_fix {
+    double receiver_timestamp; /* the fix's                                                                           */
+    double vx, vy, vz;         /* receiver ECEF velocity, m/s                                                         */
+    double clock_drift;        /* receiver clock drift, s/s                                                           */
+    double latitude_deg, longitude_deg, height; /* WGS-84 geodetic position of the fix, degrees and metres            */
+    double gdop, pdop, hdop, vdop, tdop;
+    double residual_rms;       /* RMS of the range-rate residuals, m/s                                                */
+    int32_t status;
+    int32_t n_rows;            /* the rows solved over (the fix's n_ready)                                            */
+    int32_t reserved[2];
+} gb200_velocity_fix;
+typedef char gb200_velocity_fix_is_128_bytes[sizeof(gb200_velocity_fix) == 128 ? 1 : -1]; /* C99 static assert */
+
+/* One record per millisecond of the last gb200_tracker_parse_subframes call, from its position fixes.
+ * doppler_device: [n_channels][n_ms] float64 Doppler in Hz on the device, or NULL for the `doppler` field of the
+ * tracking records of the gb200_tracker_process call that fed that parse call through the chain.  fixes_device: the
+ * n_ms gb200_position_fix records of that parse call on the device, or NULL for those the last
+ * gb200_tracker_position_fixes call kept.  The rows of a least-squares fix come from the world-model order the last fix
+ * call left.  A pure function of its inputs: the tracker's state does not change.  GB200_ESTATE if there has been no
+ * parse call, if its fixes are not computed yet, if doppler_device is NULL and that parse call was not fed by the
+ * chain or a later process call replaced its records, or if fixes_device is NULL and the last fix call wrote to caller
+ * memory (gb200_tracker_position_fixes_device: pass that buffer).  The _device variant only enqueues (out_device: n_ms
+ * records). */
+int gb200_tracker_velocity_fixes(gb200_tracker* t, const double* doppler_device, const void* fixes_device,
+                                 gb200_velocity_fix* out_host);
+int gb200_tracker_velocity_fixes_device(gb200_tracker* t, const double* doppler_device, const void* fixes_device,
+                                        void* out_device);
 /* The sizes of what the chain holds, for sizing the outputs of the calls that read it: out[0] = bit events per
  * channel the last gb200_tracker_integrate_bits call kept (its max_events), out[1] = subframe events per channel the
  * last gb200_tracker_decode_subframes call kept (its max_events), out[2] = n_ms of the last

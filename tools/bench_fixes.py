@@ -13,7 +13,11 @@ line then also reports the repaired fixes and the cost of each.
 --channels N tracks and fixes N channels (4 to 12) on the same schedule, so every fixing millisecond has N ready;
 --solver least_squares fixes them by least squares (gb200_tracker_set_fix_solver).  The reference mode raises at the
 first fix with more than four channels.
-usage (GPU box): python tools/bench_fixes.py [--reps 5] [--jump -0.2 [--jump-ms 1000]] [--channels 8 --solver least_squares]"""
+
+--velocity also times gb200_tracker_velocity_fixes_device right after each fix call, on the fix records that call wrote
+and the tracking records' Dopplers, and reports its median and its kernel next to the fix call's.
+usage (GPU box): python tools/bench_fixes.py [--reps 5] [--jump -0.2 [--jump-ms 1000]] [--channels 8 --solver least_squares]
+                 [--velocity]"""
 import argparse
 import json
 import os
@@ -59,6 +63,7 @@ def main():
     ap.add_argument("--jump-ms", type=int, default=1000, help="the millisecond the jump lands on")
     ap.add_argument("--channels", type=int, default=4, choices=range(4, len(SVS) + 1), metavar="N")
     ap.add_argument("--solver", default="reference", choices=sorted(_native.FIX_SOLVERS))
+    ap.add_argument("--velocity", action="store_true", help="also time the velocity call after each fix call")
     args = ap.parse_args()
     n_ch = args.channels
     eng = _native.Engine(FS, N)
@@ -89,8 +94,10 @@ def main():
     counts = np.full(n_ch, N_SUB, dtype=np.int32)
     drop = np.full(n_ch, -1, dtype=np.int32)
     out = torch.empty(N_MS * _native.FIX_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+    vout = torch.empty(N_MS * _native.VELOCITY_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+    rec_doubles = _native.TRACK_DTYPE.itemsize // 8  # the Doppler is the record's first field
 
-    track_ms, fix_ms, kernel_ms, repaired = [], [], {}, []
+    track_ms, fix_ms, vel_ms, kernel_ms, repaired = [], [], [], {}, []
     for rep in range(args.reps + 1):
         trk = _native.Tracker(eng, list(range(n_ch)), [c[1] for c in chans], [0.0] * n_ch, [c[3] for c in chans])
         trk.set_fix_solver(args.solver)
@@ -100,17 +107,23 @@ def main():
         if prof:
             prof.__enter__()
         df, _ = timed(stream, lambda: trk.position_fixes_device(fix_times, out.data_ptr()))
+        if args.velocity:
+            with torch.cuda.stream(stream):
+                dop = rec.view(torch.float64).view(n_ch, N_MS, rec_doubles)[:, :, 0].contiguous()
+            dv, _ = timed(stream, lambda: trk.velocity_fixes_device(vout.data_ptr(), dop.data_ptr(), out.data_ptr()))
         if prof:
             prof.__exit__(None, None, None)
             for k in prof.key_averages():
                 for name in ("k_sv_observations", "k_fix_plan", "k_fix_pass<1>", "k_fix_pass<2>", "k_fix_repair",
                              "k_fix_finish", "k_fix_plan_lsq", "k_fix_pass_lsq<1>", "k_fix_pass_lsq<2>",
-                             "k_fix_repair_lsq"):
+                             "k_fix_repair_lsq", "k_velocity_fixes"):
                     if name + "(" in k.key or k.key.endswith(name):
                         kernel_ms[name] = getattr(k, "device_time_total", getattr(k, "cuda_time_total", 0.0)) / 1e3
         if rep:  # the first round allocates
             track_ms.append(dt)
             fix_ms.append(df)
+            if args.velocity:
+                vel_ms.append(dv)
         repaired.append(trk.receiver_state()["repaired"])
         trk.close()
     f = out.cpu().numpy().view(_native.FIX_DTYPE)
@@ -119,6 +132,12 @@ def main():
     if args.jump:
         jump = {"jump_s": args.jump, "jump_ms": args.jump_ms, "repaired_fixes": repaired[-1],
                 "repair_kernel_us_per_fix": kernel_ms.get("k_fix_repair_lsq" if args.solver == "least_squares" else "k_fix_repair", 0.0) * 1e3 / max(1, repaired[-1])}
+    vel = {}
+    if args.velocity:
+        v = vout.cpu().numpy().view(_native.VELOCITY_DTYPE)
+        vel = {"velocity_call_ms_median": float(np.median(vel_ms)), "velocity_call_ms": vel_ms,
+               "velocity_fraction_of_fix": float(np.median(vel_ms) / np.median(fix_ms)),
+               "velocity_status_counts": [int(c) for c in np.bincount(v["status"], minlength=3)]}
     print(json.dumps({
         "workload": f"position_fixes_device: {n_ch} channels x {N_MS} ms after the parse call, {args.solver} solver",
         "gpu": dev.name, "power_limit": power_limit(),
@@ -127,7 +146,7 @@ def main():
         "tracking_launch_ms_median": float(np.median(track_ms)),
         "fix_fraction_of_tracking": float(np.median(fix_ms) / np.median(track_ms)),
         "fixes": int((f["status"] == _native.FIX_SOLVED).sum()),
-        "status_counts": [int(v) for v in np.bincount(f["status"], minlength=4)], **jump}), flush=True)
+        "status_counts": [int(v) for v in np.bincount(f["status"], minlength=4)], **jump, **vel}), flush=True)
     eng.close()
 
 

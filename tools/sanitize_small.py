@@ -43,6 +43,7 @@ for n, m in ((2046, 2), (4092, 1)):
         assert t.observations().shape == (2, 12)
         assert t.position_fixes(ts).shape == (12,)  # plan, both passes and finish of the position fix
         assert t.receiver_state()["slide"] is None
+        assert t.velocity_fixes().shape == (12,)  # the velocity fix on the tracking records' Dopplers
         # subframe decoding over caller bit events: full warp preamble scan, phase, drain, a reset and a re-sync
         import torch
 
@@ -68,6 +69,24 @@ for n, m in ((2046, 2), (4092, 1)):
         t.decode_subframes()
         t.parse_subframes()
         assert t.position_fixes(ts).shape == (12,)
+        t.close()
+        # the velocity fix on solved fixes: the first call of a recorded fix timeline, with caller Dopplers
+        from oracle import fix_oracle as fx
+
+        rx, chans = fx.golden_calls(np.load(os.path.join(ROOT, "tests", "golden", "fix.npz")), "realistic")[0]
+        stride = max(len(ev) for ev, _ in chans)
+        host = np.zeros((4, stride), dtype=_native.SUBFRAME_DTYPE)
+        ems = np.zeros((4, stride), dtype=np.int32)
+        for c, (events, _) in enumerate(chans):
+            for j, (kind, w, te, ms) in enumerate(events):
+                host[c, j]["kind"], host[c, j]["words"], host[c, j]["trailing_edge_receiver_timestamp"] = kind, w, te
+                ems[c, j] = ms
+        t = _native.Tracker(eng, [0, 1, 2, 3], [0.0] * 4, [0.0] * 4, [0] * 4)
+        evd = torch.from_numpy(host.view(np.uint8).reshape(4, -1)).cuda()
+        t.parse_subframes(evd.data_ptr(), [len(ev) for ev, _ in chans], stride, ems, [d for _, d in chans], len(rx))
+        t.position_fixes(rx)
+        dopd = torch.full((4, len(rx)), 1234.5, dtype=torch.float64, device="cuda")
+        assert (t.velocity_fixes(dopd.data_ptr())["status"] == 1).any()
         t.close()
         # pipelined batch stream: three streams, pageable staging
         gs = _native.GridStream(eng, 2, 1, [24, 0, 5], dop, _native.NON_COHERENT, depth=2)
