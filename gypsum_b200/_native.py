@@ -89,6 +89,7 @@ SYMBOLS = {
     "gb200_tracker_set_fix_solver": (C.c_int, [_P, C.c_int]),
     "gb200_tracker_velocity_fixes": (C.c_int, [_P, _P, _P, _P]),
     "gb200_tracker_velocity_fixes_device": (C.c_int, [_P, _P, _P, _P]),
+    "gb200_tracker_signal_windows": (C.c_int, [_P, C.c_int, _P, C.c_int32, _P, _P, C.c_int32, _P]),
     "gb200_tracker_chain_sizes": (C.c_int, [_P, _P]),
     "gb200_set_fused": (C.c_int, [_P, C.c_int]),
     "gb200_launch_count": (C.c_int, [_P, C.POINTER(C.c_int64)]),
@@ -681,6 +682,22 @@ class Tracker:
                                                                           _P(fixes_device_ptr), _P(out_device_ptr)),
                             "gb200_tracker_velocity_fixes_device")
 
+    def signal_windows(self, n_ms: int, start_times, window_ms: int, records_device_ptr: int | None = None,
+                       max_windows: int | None = None) -> list:
+        """Carrier-to-noise density and phase-lock indicator of every channel over windows of window_ms consecutive
+        milliseconds of its tracking records (gb200_tracker_signal_windows): records in device memory, by default the
+        ones the last `process` call left there.  Each channel's open window carries into the next call; window_ms is
+        fixed by the first call.  Returns one SIGNAL_DTYPE array per channel.  max_windows (default: the most one call
+        touches) caps the windows kept per channel; RuntimeError if a channel produced more."""
+        ts = np.ascontiguousarray(start_times, dtype=np.float64)
+        if ts.shape != (n_ms,):
+            raise ValueError("start_times must hold one timestamp per millisecond")
+        # the window the last call left open, then one every window_ms: at most n_ms // window_ms + 2 (valid W only)
+        cap = int(n_ms) // max(int(window_ms), 1) + 2 if max_windows is None else int(max_windows)
+        records = None if records_device_ptr is None else _P(records_device_ptr)
+        return self._per_channel("gb200_tracker_signal_windows", SIGNAL_DTYPE, cap, "signal window",
+                                 int(n_ms), _ptr(ts), int(window_ms), records)
+
     def receiver_state(self) -> dict:
         """After the last fix call: slide (receiver_clock_slide, None before any), stopped, order: the channels in
         the world model's order, and repaired: the fixes the serial chain recomputed where the parallel passes' chain
@@ -752,6 +769,12 @@ VELOCITY_DTYPE = np.dtype([  # gb200_velocity_fix
     ("reserved", "<i4", (2,))])
 assert VELOCITY_DTYPE.itemsize == 128
 VEL_NONE, VEL_SOLVED, VEL_UNSOLVABLE = 0, 1, 2  # VELOCITY_DTYPE["status"]
+SIGNAL_DTYPE = np.dtype([  # gb200_signal_window
+    ("receiver_timestamp", "<f8"), ("cn0_dbhz", "<f8"), ("prompt_power", "<f8"), ("noise_power", "<f8"),
+    ("pll_lock", "<f8"), ("first_ms", "<i8"), ("ms_index", "<i4"), ("n_ms", "<i4"), ("locked_ms", "<i4"),
+    ("status", "<i4")])
+assert SIGNAL_DTYPE.itemsize == 64
+SIGNAL_NONE, SIGNAL_FOUND, SIGNAL_NOISE = 0, 1, 2  # SIGNAL_DTYPE["status"]
 
 
 def subframe_event_capacity(n_bits: int) -> int:

@@ -18,6 +18,7 @@
 #include "kernels.cuh"
 #include "fix_core.cuh"
 #include "velocity_core.cuh"
+#include "signal_core.cuh"
 #include "nav_core.cuh"
 #include "orbit_core.cuh"
 
@@ -258,6 +259,17 @@ struct gb200_tracker {
         DevBuf<VelocityRecord> d_out;
         PinnedBuf<VelocityRecord> h_out;
     } vel;
+    struct {  // signal.cu
+        int window_ms = 0;  // W, fixed by the first call (0 = no call yet)
+        double floor_dbhz = 0.0;  // signal_noise_floor_dbhz(N), from the first call on
+        DevBuf<SignalState> states, carried;
+        DevBuf<SignalWindow> d_out;
+        DevBuf<int> d_stop, d_counts;
+        DevBuf<double> d_times;
+        PinnedBuf<SignalWindow> h_out;
+        PinnedBuf<int> h_counts;
+        PinnedBuf<double> h_times;
+    } sig;
 };
 // A pipelined stream of grid batches: slot k's host->device copy, compute and device->host copy run on three streams.
 struct gb200_grid_stream {
@@ -315,6 +327,11 @@ static_assert(sizeof(gb200_velocity_fix) == sizeof(VelocityRecord) &&
                   offsetof(gb200_velocity_fix, status) == offsetof(VelocityRecord, status) &&
                   offsetof(gb200_velocity_fix, n_rows) == offsetof(VelocityRecord, n_rows),
               "ABI velocity fix and device velocity fix must match");
+static_assert(sizeof(gb200_signal_window) == sizeof(SignalWindow) &&
+                  offsetof(gb200_signal_window, first_ms) == offsetof(SignalWindow, first_ms) &&
+                  offsetof(gb200_signal_window, ms_index) == offsetof(SignalWindow, ms_index) &&
+                  offsetof(gb200_signal_window, status) == offsetof(SignalWindow, status),
+              "ABI signal window and device signal window must match");
 static_assert(offsetof(TrackMsRecord, doppler) == 0 && sizeof(TrackMsRecord) % sizeof(double) == 0,
               "the velocity fix reads the tracking records' Doppler with a stride in doubles");
 static_assert(offsetof(gb200_subframe_event, words) == offsetof(SubframeEvent, words) &&
@@ -1609,6 +1626,54 @@ int gb200_tracker_integrate_bits(gb200_tracker* t, int n_ms, const double* start
     }));
     t->chain.integrated(s.h_counts.p, nc, max_events, !records_device);
     return GB200_OK;
+}
+
+int gb200_tracker_signal_windows(gb200_tracker* t, int n_ms, const double* start_times, int32_t window_ms,
+                                 const void* records_device, gb200_signal_window* out_host, int32_t max_windows,
+                                 int32_t* counts_host) {
+    if (!t) return GB200_EINVAL;
+    gb200_engine* e = t->e;
+    auto& s = t->sig;
+    const int nc = t->n_channels, chain_ms = t->chain.records.n_ms;
+    if (n_ms < 1 || !start_times) GB_FAIL(e, GB200_EINVAL, "need at least one millisecond and its start times");
+    if (!out_host || !counts_host || max_windows < 1) GB_FAIL(e, GB200_EINVAL, "null / empty window buffer");
+    if (window_ms < kSignalMinMs || window_ms > kSignalMaxMs)
+        GB_FAIL(e, GB200_EINVAL, "window_ms must be between %d and %d, not %d", kSignalMinMs, kSignalMaxMs, window_ms);
+    if (s.window_ms && window_ms != s.window_ms)
+        GB_FAIL(e, GB200_ESTATE, "the open windows were formed with window_ms = %d, not %d", s.window_ms, window_ms);
+    if (!records_device && chain_ms != n_ms)
+        GB_FAIL(e, GB200_ESTATE, "no records of %d ms on the device (last gb200_tracker_process call held %d)", n_ms, chain_ms);
+    GB_CUDA(e, cudaSetDevice(e->device));
+    GB_CUDA(e, cudaStreamSynchronize(e->stream));  // pinned staging may still be in flight
+    GB_TRY(ensure_state(e, s.states, nc, [](SignalState& st) { signal_state_init(st); }));
+    if (!s.window_ms) s.floor_dbhz = signal_noise_floor_dbhz(e->N);
+    s.window_ms = window_ms;
+    const size_t nw = static_cast<size_t>(nc) * max_windows;
+    GB_CUDA(e, s.carried.ensure(nc));
+    GB_CUDA(e, s.d_stop.ensure(nc));
+    GB_CUDA(e, s.d_counts.ensure(nc));
+    GB_CUDA(e, s.h_counts.ensure(nc));
+    GB_CUDA(e, s.d_out.ensure(nw));
+    GB_CUDA(e, s.d_times.ensure(n_ms));
+    GB_TRY(upload(e, s.d_times.p, start_times, n_ms, s.h_times));
+    SignalArgs a{};
+    a.records = records_device ? static_cast<const TrackMsRecord*>(records_device) : t->d_out.p;
+    a.start_times = s.d_times.p;
+    a.states = s.states.p;
+    a.carried = s.carried.p;
+    a.stop = s.d_stop.p;
+    a.out = s.d_out.p;
+    a.counts = s.d_counts.p;
+    a.floor_dbhz = s.floor_dbhz;
+    a.n_ms = n_ms;
+    a.n_channels = nc;
+    a.window_ms = window_ms;
+    a.max_windows = max_windows;
+    GB_LAUNCH(e, -1, launch_signal_windows(a, e->stream));
+    e->launches++;  // the stop scan and the windows
+    return fetch_output(e, nc, s.d_counts, s.h_counts, counts_host, [&]() -> int {
+        return download(e, reinterpret_cast<SignalWindow*>(out_host), s.d_out.p, nw, s.h_out);
+    });
 }
 
 int gb200_tracker_bit_state(gb200_tracker* t, int channel, int64_t out[8]) {

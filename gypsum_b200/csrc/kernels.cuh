@@ -185,6 +185,22 @@ struct VelocityArgs {
 };
 cudaError_t launch_velocity_fixes(const VelocityArgs& a, cudaStream_t st);
 
+// signal_windows: C/N0 and phase-lock windows of every channel's tracking records (signal.cu, signal_core.cuh).
+struct SignalState;
+struct SignalWindow;
+struct SignalArgs {
+    const TrackMsRecord* records;  // [n_channels][n_ms] as written by k_track_channels
+    const double* start_times;     // [n_ms] chunk start timestamps
+    SignalState* states;           // [n_channels] carried from call to call
+    SignalState* carried;          // [n_channels] scratch: the states as the call found them
+    int* stop;                     // [n_channels] scratch: the channel's first lost record in the call (>= n_ms: none)
+    SignalWindow* out;             // [n_channels][max_windows]
+    int* counts;                   // [n_channels] windows produced (may exceed max_windows: truncated)
+    double floor_dbhz;             // signal_noise_floor_dbhz(N)
+    int n_ms, n_channels, window_ms, max_windows;
+};
+cudaError_t launch_signal_windows(const SignalArgs& a, cudaStream_t st);
+
 // acquire_fused: one CTA per (PRN, Doppler) cell, the whole pipeline in one kernel (fused.cu).
 struct FusedArgs {
     const float2* iq;       // [M*N] one block

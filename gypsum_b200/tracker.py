@@ -407,6 +407,25 @@ class TrackerBank:
         where only the geodetic position is set."""
         return self.native.velocity_fixes()
 
+    def signal_quality(self, start_times, window_ms: int = 1000) -> list:
+        """Each channel's carrier-to-noise density (dB-Hz) and phase-lock indicator over windows of window_ms consecutive
+        milliseconds of the tracking records the last `process` / `process_ring` call left on the device (DESIGN.md
+        §8e).  One estimator per channel, kept across calls: a window a call leaves open carries into the next, and
+        window_ms is fixed by the first call.  A channel stops at its first lost record.  Returns one
+        _native.SIGNAL_DTYPE array per channel; status 1: a signal (cn0_dbhz at least 1 dB above
+        cn0_noise_floor_dbhz), 2: nothing distinguishable from noise, 0: a stop cut the window below 20 ms.  Reads the
+        chain without changing it: integrate_bits and the calls after it give the same results with or without it."""
+        return self.native.signal_windows(len(start_times), start_times, window_ms)
+
+
+def cn0_noise_floor_dbhz(samples_per_ms: int) -> float:
+    """What the C/N0 estimate of TrackerBank.signal_quality reads for noise alone at this many samples per
+    millisecond: 10 log10((H_N - 1) / 1 ms), H_N the N-th harmonic number (38.57 dB-Hz at 2046, 39.68 at 16368)."""
+    h = 0.0
+    for k in range(1, int(samples_per_ms) + 1):
+        h += 1.0 / k
+    return 10.0 * math.log10((h - 1.0) / 1e-3)
+
 
 # OrbitalParameterType (world_model.py:151-199), in order
 ORBITAL_PARAMETER_NAMES = (

@@ -461,6 +461,44 @@ int gb200_tracker_velocity_fixes(gb200_tracker* t, const double* doppler_device,
                                  gb200_velocity_fix* out_host);
 int gb200_tracker_velocity_fixes_device(gb200_tracker* t, const double* doppler_device, const void* fixes_device,
                                         void* out_device);
+/* The carrier-to-noise density and phase-lock indicator of one tracking channel over one window of W consecutive
+ * milliseconds of its tracking records (64 bytes; DESIGN.md §8e).  With P_k the record's prompt (peak_re, peak_im) and
+ * s_k its strength, over the window's n records
+ *     M2 = sum |P_k|^2 / n,  Pn = (4/pi) sum (|P_k| / s_k)^2 / n,  C/N0 = 10 log10((M2 - Pn) / (Pn * 1 ms)),
+ *     PLI = (sum I^2 - sum Q^2) / (sum I^2 + sum Q^2).
+ * For noise alone the estimate sits at the floor 10 log10((H_N - 1) / 1 ms), H_N = sum_{k=1..N} 1/k, N the samples per
+ * millisecond (38.57 dB-Hz at N = 2046).  status:
+ *   0  not estimated: a stop cut the window below 20 records, or a sum is not finite; cn0_dbhz is NaN
+ *   1  a signal: cn0_dbhz >= floor + 1 dB
+ *   2  nothing distinguishable from noise: cn0_dbhz < floor + 1 dB, or NaN when M2 <= Pn */
+typedef struct gb200_signal_window {
+    double receiver_timestamp; /* chunk start time of the window's first millisecond                                */
+    double cn0_dbhz;           /* C/N0, dB-Hz                                                                        */
+    double prompt_power;       /* M2                                                                                 */
+    double noise_power;        /* Pn                                                                                 */
+    double pll_lock;           /* PLI, -1..1                                                                         */
+    int64_t first_ms;          /* the window's first record, counted from the first one this channel's estimator consumed */
+    int32_t ms_index;          /* millisecond of this call holding the window's last counted record, -1 = an earlier call */
+    int32_t n_ms;              /* records in the window: W, or fewer when a stop cut it                              */
+    int32_t locked_ms;         /* of them with `locked` set                                                          */
+    int32_t status;
+} gb200_signal_window;
+typedef char gb200_signal_window_is_64_bytes[sizeof(gb200_signal_window) == 64 ? 1 : -1]; /* C99 static assert */
+
+/* The windows every channel closes over n_ms millisecond records in device memory: records_device ([channel][n_ms]
+ * gb200_track_record), or NULL for the records of the last whole-bank gb200_tracker_process call (GB200_ESTATE unless
+ * that call held n_ms).  start_times[n_ms]: the chunk start times.  Each channel keeps one estimator across calls:
+ * windows are W = window_ms consecutive milliseconds of its records (20 <= W <= 60000), and the window a call leaves
+ * open carries into the next call.  Each window's sums run in millisecond order, so the same stream split into calls of
+ * any sizes gives byte-identical windows apart from ms_index.  W is fixed by the tracker's first call: another W later
+ * is GB200_ESTATE.  A channel stops at its first record with `lost` set, which is not counted: its open window is
+ * emitted at once if it holds a record, and the channel emits nothing afterwards, even after gb200_tracker_set_state.
+ * Reads the chain and changes none of it.  out_host: [channel][max_windows]; counts_host: [channel] windows produced
+ * (> max_windows: truncated). */
+int gb200_tracker_signal_windows(gb200_tracker* t, int n_ms, const double* start_times, int32_t window_ms,
+                                 const void* records_device, gb200_signal_window* out_host, int32_t max_windows,
+                                 int32_t* counts_host);
+
 /* The sizes of what the chain holds, for sizing the outputs of the calls that read it: out[0] = bit events per
  * channel the last gb200_tracker_integrate_bits call kept (its max_events), out[1] = subframe events per channel the
  * last gb200_tracker_decode_subframes call kept (its max_events), out[2] = n_ms of the last

@@ -44,6 +44,9 @@ for n, m in ((2046, 2), (4092, 1)):
         assert t.position_fixes(ts).shape == (12,)  # plan, both passes and finish of the position fix
         assert t.receiver_state()["slide"] is None
         assert t.velocity_fixes().shape == (12,)  # the velocity fix on the tracking records' Dopplers
+        # C/N0 windows on the chain's records: a window left open by the first call and closed by the second
+        assert [len(w) for w in t.signal_windows(12, ts, 20)] == [0, 0]
+        assert [len(w) for w in t.signal_windows(12, ts, 20)] == [1, 1]
         # subframe decoding over caller bit events: full warp preamble scan, phase, drain, a reset and a re-sync
         import torch
 
