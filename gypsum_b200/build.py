@@ -8,7 +8,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgypsum_b200.so")
-SOURCES = ["kernels.cu", "tracker.cu", "bits.cu", "nav.cu", "orbit.cu", "fix.cu", "velocity.cu", "signal.cu", "fused.cu", "engine.cu"]
+SOURCES = ["kernels.cu", "tracker.cu", "bits.cu", "nav.cu", "orbit.cu", "fix.cu", "velocity.cu", "signal.cu", "fused.cu", "engine.cu", "receiver.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared", "-cudart", "static",

@@ -1,4 +1,4 @@
-// Kernel argument blocks and launch wrappers (implemented in kernels.cu, used by engine.cu).
+// Kernel argument blocks and launch wrappers (implemented in kernels.cu, used by engine.cu and receiver.cu).
 #pragma once
 #include "gb_common.cuh"
 #include "tracker_core.cuh"
