@@ -11,7 +11,7 @@ import pytest
 
 import fix_lsq_oracle as lo
 from fix_support import (BIAS_S, MANY_BIAS_S, MANY_POS_M, MANY_SLIDE_ULPS, POS_M, SLIDE_ULPS, fix_emulator, parse_events,
-                         run_calls)
+                         ready_rows, run_calls, scripted_timeline)
 from gpu_support import make_engine
 from oracle import fix_oracle as fx
 from oracle import nav_oracle as nav
@@ -35,40 +35,6 @@ def engine(native_lib):
 @pytest.fixture(scope="module")
 def lsq_emu():
     return fix_emulator()
-
-
-def scripted_timeline():
-    """Six channels with their own planted ephemerides and the same TOW counts, in two calls (the layout of
-    fx.golden_calls), built as tools/make_golden_fix.py builds its timelines:
-      call 0  subframes 1-3 on all six at ms 100 / 200 / 300: six ready from 300; channel 4 loses lock at 600 and
-              channel 5 at 700 (6 -> 5 -> 4 inside the segment); subframe 4 on channels 0-3 at 900 resets the slide
-      call 1  subframe 5 on all six at ms 200: channels 4 and 5 return, six ready again; a receiver-clock jump of
-              -0.2 s at ms 600 inside that segment, so the chain check misses and the repair solves six rows"""
-    rng = np.random.default_rng(2031)
-    svs = (2, 6, 11, 17, 24, 29)
-    words = [[orb.words_of(sf) for sf in orb.ephemeris_subframes(orb.realistic_ephemeris(rng, sv), 5, tow0=50000,
-                                                                  seed=100 + c)] for c, sv in enumerate(svs)]
-    sched = [[[(0, 100), (1, 200), (2, 300), (3, 900)], [(4, 200)]] for _ in range(4)]
-    sched += [[[(0, 100), (1, 200), (2, 300)], [(4, 200)]] for _ in range(2)]
-    drops = [[-1, -1, -1, -1, 600, 700], [-1] * 6]
-    calls_ms, jumps = [1500, 1200], [(1, 600, -0.2)]
-    out, t0 = [], 0.0
-    for c, n_ms in enumerate(calls_ms):
-        def offset(m, c=c):
-            return sum(j for jc, jm, j in jumps if (jc, jm) <= (c, m))
-
-        rx = np.array([t0 + 0.001 * m + offset(m) for m in range(n_ms)])
-        chans = [([(nav.KIND_SUBFRAME, words[ch][k], round(t0 + 0.001 * m - 0.0003 * ch + offset(m), 7), m)
-                   for k, m in sched[ch][c]], drops[c][ch]) for ch in range(len(svs))]
-        out.append((rx, chans))
-        t0 += 0.001 * n_ms
-    return out
-
-
-def _rows(obs, order, m):
-    """The ready rows (flags 2 and 4) of millisecond m in the world model's order, from the device's observations."""
-    return [(obs[ch, m]["tow"], obs[ch, m]["x"], obs[ch, m]["y"], obs[ch, m]["z"]) for ch in order
-            if (obs[ch, m]["flags"] & 6) == 6]
 
 
 def _check(calls, got_calls, ref_calls, lsq_emu):
@@ -101,7 +67,7 @@ def _check(calls, got_calls, ref_calls, lsq_emu):
             assert worst[1] <= bias_s and worst[2] <= pos_m, worst
         assert np.isnan(got["x"][got["status"] != fx.FIX_SOLVED]).all()
         # the model of the passes on the device's own observations: every record bit for bit, and the repair count
-        rows = {m: _rows(obs, state["order"], m) for m in fixing}
+        rows = {m: ready_rows(obs, state["order"], m) for m in fixing}
         assert all(len(rows[m]) == want[m]["n_ready"] for m in fixing)
         model = lo.device_passes(lsq_emu, want, rows, rcv.resets, carried)
         carried = model["slide"]

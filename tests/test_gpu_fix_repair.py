@@ -8,7 +8,7 @@ import os
 import numpy as np
 import pytest
 
-from fix_support import BIAS_S, POS_M, fix_emulator, rows_at, run_golden, slide_tol
+from fix_support import ChainCheck, fix_emulator, rows_at, run_golden, slide_tol
 from gpu_support import make_engine
 from oracle import fix_oracle as fx
 
@@ -35,47 +35,24 @@ def fix_emu():
 def test_repair_on_the_device(engine, fix_emu, name):
     """Against the recording and the oracle: status, ready count and rows exact; slides and round-0 pseudoranges within
     4 ulp, clock bias within 1e-14 s, position within 2e-6 m.  Against the model of the passes on the device's own
-    observations: every record bit for bit and receiver_state()["repaired"] after every call.  Every solved record is
-    the host core's fix from its own slide_in; a fix that does not start a segment starts from the slide the fix
-    before it left, exactly where the repair ran and within 4 ulp elsewhere; slide, order and stopped are the
-    oracle's."""
+    observations (fix_support.ChainCheck): every record bit for bit, and after every call receiver_state()'s slide the
+    model's carried slide exactly, its order and stop the oracle's and its repair count the model's.  Every solved
+    record is the host core's fix from its own slide_in; a fix that does not start a segment starts from the slide the
+    fix before it left, exactly where the repair ran and within 4 ulp elsewhere; the last slide is the oracle's within
+    4 ulp."""
     z, calls, out = run_golden(engine, GOLDEN, name)
     rcv = fx.ReceiverOracle(len(calls[0][1]))
-    carried, repaired, worst = None, 0, [0.0, 0.0, 0.0]
+    check = ChainCheck(fix_emu)
     for c, ((rx, chans), (got, obs, state)) in enumerate(zip(calls, out)):
         want = rcv.call(chans, rx)
         rec = fx.golden_fix_rows(z, name, c)
         assert np.array_equal(got["status"], rec[:, 3].astype(int))
-        assert np.array_equal(got["n_ready"], want["n_ready"]) and np.array_equal(got["channel"], want["channel"])
+        # the oracle's status, rows and numbers, the model of the passes bit for bit and receiver_state()
+        model = check(want, rcv.resets, rcv.order, rcv.stopped, got, obs, state, what=c)
         fixing = np.flatnonzero(np.isin(want["status"], [fx.FIX_SOLVED, fx.FIX_RAISED]))
-        solved = np.flatnonzero(want["status"] == fx.FIX_SOLVED)
-        for k in ("slide_in", "slide_out"):
-            d = np.abs(got[k][fixing] - want[k][fixing])
-            assert (d <= slide_tol(want[k][fixing])).all(), k
-            worst[0] = max([worst[0], *d])
-        if len(solved):
-            d = np.abs(got["pseudorange"][solved] - want["pseudorange"][solved]).max(axis=1)
-            assert (d <= slide_tol(want["slide_in"][solved])).all()
-            worst[1] = max(worst[1], float(np.abs(got["clock_bias"][solved] - want["clock_bias"][solved]).max()))
-            worst[2] = max([worst[2], *(float(np.abs(got[k][solved] - want[k][solved]).max()) for k in "xyz")])
-        assert worst[1] <= BIAS_S and worst[2] <= POS_M, worst
-        assert np.isnan(got["x"][got["status"] != fx.FIX_SOLVED]).all()
-        # the model of the passes, on the rows the device observed
-        rows = {m: rows_at(obs, want[m]["channel"], m) for m in fixing if want[m]["n_ready"] == 4}
-        model = fx.device_passes(fix_emu, want, rows, rcv.resets, carried)
-        carried = model["slide"]
-        assert sorted(model["out"]) == list(fixing)
-        for m in fixing:  # the numbers (slides, solution, pseudoranges) of a solved record; the slides of a raise
-            p = model["out"][m]
-            assert p["status"] == got[m]["status"] and p["slide_in"] == got[m]["slide_in"], m
-            assert p["slide_out"] == got[m]["slide_out"], m
-            if m in solved:
-                assert p.tobytes()[:88] == got[m].tobytes()[:88], m
-        for m in solved:
-            host = fix_emu(rows[m], got[m]["receiver_timestamp"], got[m]["slide_in"])
+        for m in np.flatnonzero(want["status"] == fx.FIX_SOLVED):
+            host = fix_emu(rows_at(obs, want[m]["channel"], m), got[m]["receiver_timestamp"], got[m]["slide_in"])
             assert host.tobytes()[:88] == got[m].tobytes()[:88] and host["status"] == got[m]["status"], m
-        repaired += len(model["repaired"])
-        assert state["repaired"] == repaired, (c, state["repaired"], repaired)
         # the chain relation
         for a, b in zip(fixing[:-1], fixing[1:]):
             if b in rcv.resets or any(r in rcv.resets for r in range(a + 1, b)):
@@ -92,7 +69,8 @@ def test_repair_on_the_device(engine, fix_emu, name):
         assert abs(st["slide"] - rcv.slide) <= slide_tol(rcv.slide)
     if name in GAPS:
         assert out[0][2]["repaired"] > 0
-    print(f"{name}: worst slide / pseudorange {worst[0]:.3g} s, clock bias {worst[1]:.3g} s, position {worst[2]:.3g} m")
+    print(f"{name}: worst slide {check.worst[0]:.3g} ulp, clock bias {check.worst[1]:.3g} s, position "
+          f"{check.worst[2]:.3g} m")
 
 
 def test_carried_slide_needs_no_repair(engine):
