@@ -27,11 +27,13 @@ __global__ void __launch_bounds__(kBitWarps * 32) k_integrate_bits(const BitArgs
         if (k < a.n_ms) {
             sym = rec[k].symbol;
             lost = rec[k].lost;
-            // tracker.py:319-325: the symbol is stamped with the chunk times delayed by the code phase
+            // tracker.py:319-325: the symbol is stamped with the chunk times delayed by the code phase.  The sums are
+            // rounded on their own, as the reference rounds them: a multiply-add fused into one rounding would move
+            // some stamps by an ulp.
             const double delay = (static_cast<double>(rec[k].code_phase) / 2046.0) * 0.001;
             t0 = a.start_times[k];
-            ts = t0 + delay;
-            te = a.end_times[k] + delay;
+            ts = __dadd_rn(t0, delay);
+            te = __dadd_rn(a.end_times[k], delay);
         }
         const int m = min(32, a.n_ms - k0);
         for (int j = 0; j < m; ++j) {

@@ -1,5 +1,6 @@
 // Host build of the subframe decoder's state machine (gypsum_b200/csrc/nav_core.cuh) with its scalar preamble scan,
-// for tests/test_nav_decoder_cpu.py.  Built with nvcc for the host only; no device code runs.
+// for tests/test_nav_decoder_cpu.py and tests/test_nav_edges_cpu.py.  Built with nvcc for the host only; no device
+// code runs.
 #include <cstddef>
 #include <cstring>
 
@@ -21,6 +22,28 @@ int nav_emu_run(NavState* st, int n, const int* bits, const double* t0, const do
     NavQueue q{st->val, st->known, st->qstart, st->qend};
     int n_out = 0;
     for (int k = 0; k < n; ++k) nav_step(st->h, q, bits[k], t0[k], t1[k], k, out, max_events, n_out);
+    return n_out;
+}
+// nav_emu_run that also records, for every bit k, what nav_push chose and the queue the search saw:
+// trace[4k .. 4k+3] = scan kind (NavPush), qhead and qlen after the push, phase after the bit (-1 = None)
+int nav_emu_trace(NavState* st, int n, const int* bits, const double* t0, const double* t1, SubframeEvent* out,
+                  int max_events, int* trace) {
+    NavQueue q{st->val, st->known, st->qstart, st->qend};
+    int n_out = 0;
+    for (int k = 0; k < n; ++k) {
+        const int n_at_bit = n_out;
+        const int scan = nav_push(st->h, q, bits[k], t0[k], t1[k]);
+        trace[4 * k] = scan;
+        trace[4 * k + 1] = st->h.qhead;
+        trace[4 * k + 2] = st->h.qlen;
+        int up = -1, inv = -1;
+        if (scan == kNavFullScan) {
+            up = nav_first_pair(q, st->h.qhead, st->h.qlen, kPreambleUp);
+            if (up < 0) inv = nav_first_pair(q, st->h.qhead, st->h.qlen, kPreambleInv);
+        }
+        nav_finish(st->h, q, scan, up, inv, k, out, max_events, n_out, n_at_bit);
+        trace[4 * k + 3] = st->h.phase;
+    }
     return n_out;
 }
 void nav_emu_summary(const NavState* st, long long* out /*[6]*/) {
