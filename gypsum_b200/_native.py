@@ -87,6 +87,7 @@ SYMBOLS = {
     "gb200_tracker_receiver_state": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_int32), _P]),
     "gb200_tracker_fix_repairs": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "gb200_tracker_set_fix_solver": (C.c_int, [_P, C.c_int]),
+    "gb200_tracker_set_code_phase_mode": (C.c_int, [_P, C.c_int]),
     "gb200_tracker_velocity_fixes": (C.c_int, [_P, _P, _P, _P]),
     "gb200_tracker_velocity_fixes_device": (C.c_int, [_P, _P, _P, _P]),
     "gb200_tracker_signal_windows": (C.c_int, [_P, C.c_int, _P, C.c_int32, _P, _P, C.c_int32, _P]),
@@ -660,6 +661,17 @@ class Tracker:
         self._engine._check(self._lib.gb200_tracker_set_fix_solver(self._h, FIX_SOLVERS[solver]),
                             "gb200_tracker_set_fix_solver")
 
+    def set_code_phase_mode(self, mode: str) -> None:
+        """How the channels count code phase (gb200_tracker_set_code_phase_mode): "reference" (the default) wraps the DLL
+        accumulator at 2046 and delays each pseudosymbol by code phase / 2046 ms at every rate, as the reference does;
+        "samples" wraps at the engine's samples per millisecond N and delays by code phase / N ms, so that every code
+        phase in [0, N) stays tracked.  Only before the first tracking or bit-integration call (RuntimeError after it);
+        ValueError for another name."""
+        if mode not in CODE_PHASE_MODES:
+            raise ValueError(f"code-phase mode must be one of {sorted(CODE_PHASE_MODES)}, not {mode!r}")
+        self._engine._check(self._lib.gb200_tracker_set_code_phase_mode(self._h, CODE_PHASE_MODES[mode]),
+                            "gb200_tracker_set_code_phase_mode")
+
     def position_fixes_device(self, receiver_timestamps, out_device_ptr: int) -> None:
         """Enqueue only: n_ms FIX_DTYPE records to device memory."""
         rx = self._fix_times(receiver_timestamps)
@@ -762,6 +774,8 @@ FIX_DTYPE = np.dtype([  # gb200_position_fix
 assert FIX_DTYPE.itemsize == 112
 FIX_NONE, FIX_SOLVED, FIX_RAISED, FIX_STOPPED = 0, 1, 2, 3  # FIX_DTYPE["status"]
 FIX_SOLVERS = {"reference": 0, "least_squares": 1}  # GB200_FIX_SOLVER_*
+CODE_PHASE_MODES = {"reference": 0, "samples": 1}  # GB200_CODE_PHASE_*
+REFERENCE_CODE_WRAP = 2046  # where the reference's DLL accumulator wraps at every rate (tracker.py:301-303, :319)
 VELOCITY_DTYPE = np.dtype([  # gb200_velocity_fix
     ("receiver_timestamp", "<f8"), ("vx", "<f8"), ("vy", "<f8"), ("vz", "<f8"), ("clock_drift", "<f8"),
     ("latitude_deg", "<f8"), ("longitude_deg", "<f8"), ("height", "<f8"), ("gdop", "<f8"), ("pdop", "<f8"),

@@ -30,7 +30,7 @@ __global__ void __launch_bounds__(kBitWarps * 32) k_integrate_bits(const BitArgs
             // tracker.py:319-325: the symbol is stamped with the chunk times delayed by the code phase.  The sums are
             // rounded on their own, as the reference rounds them: a multiply-add fused into one rounding would move
             // some stamps by an ulp.
-            const double delay = (static_cast<double>(rec[k].code_phase) / 2046.0) * 0.001;
+            const double delay = track_symbol_delay(rec[k].code_phase, a.code_wrap);
             t0 = a.start_times[k];
             ts = __dadd_rn(t0, delay);
             te = __dadd_rn(a.end_times[k], delay);

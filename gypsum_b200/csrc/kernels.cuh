@@ -94,6 +94,7 @@ struct TrackArgs {
     double t0_single;           // start time used when start_times is null (single-millisecond launches: no upload)
     const int* channel_idx;     // optional [n_channels]: CTA b runs channel channel_idx[b] (records still go to out[b]); null = b
     TrackState* shadow;         // optional [capacity]: every launched channel's state as it was BEFORE this launch (rollback)
+    double code_wrap;           // the DLL accumulator's modulus: kReferenceCodeWrap or N (tracker_core.cuh)
 };
 
 // integrate_bits: one warp per tracking channel (bits.cu, bits_core.cuh).
@@ -107,6 +108,7 @@ struct BitArgs {
     BitEvent* events;              // [n_channels][max_events]
     int* counts;                   // [n_channels] events produced (may exceed max_events: truncated)
     int n_ms, n_channels, max_events;
+    double code_wrap;              // the tracker's code-phase modulus: each symbol's delay is code_phase / code_wrap ms
 };
 
 // decode_subframes: one warp per channel over its bit events (nav.cu, nav_core.cuh).

@@ -78,6 +78,8 @@ struct gb200_tracker {
     PinnedBuf<double> h_times;
     PinnedBuf<float> h_prof;
     TrackerChain chain;
+    double code_wrap = kReferenceCodeWrap;  // gb200_tracker_set_code_phase_mode: the DLL's modulus and the symbol delay's
+    bool tracked = false;                   // a tracking or bit-integration launch has used code_wrap
     // Each later stage's per-channel state (created by its first call) and scratch.
     struct {  // bits.cu
         DevBuf<BitState> states;
@@ -143,6 +145,7 @@ static_assert(sizeof(gb200_sv_observation) == sizeof(SvObservation) &&
                   offsetof(gb200_sv_observation, prn_count) == offsetof(SvObservation, prn_count) &&
                   offsetof(gb200_sv_observation, flags) == offsetof(SvObservation, flags),
               "ABI observation and device observation must match");
+static_assert(GB200_CODE_PHASE_REFERENCE == 0 && GB200_CODE_PHASE_SAMPLES == 1, "code-phase modes are 0 and 1");
 static_assert(GB200_FIX_SOLVER_REFERENCE == kFixSolverReference && GB200_FIX_SOLVER_LEAST_SQUARES == kFixSolverLeastSquares,
               "ABI and device fix solvers must match");
 static_assert(sizeof(gb200_position_fix) == sizeof(FixRecord) &&
@@ -368,6 +371,8 @@ static int tracker_launch(gb200_tracker* t, int n_sel, const int32_t* sel, int n
     a.s = e->s;
     a.n_ms = n_ms;
     a.n_channels = sel ? n_sel : t->n_channels;
+    a.code_wrap = t->code_wrap;
+    t->tracked = true;
     GB_LAUNCH(e, -1, launch_track_channels(a, e->stream));
     for (int i = 0; i < a.n_channels; ++i) t->undo_ok[sel ? sel[i] : i] = keep_undo ? 1 : 0;
     return GB200_OK;
@@ -516,6 +521,8 @@ int gb200_tracker_integrate_bits(gb200_tracker* t, int n_ms, const double* start
     a.n_ms = n_ms;
     a.n_channels = nc;
     a.max_events = max_events;
+    a.code_wrap = t->code_wrap;
+    t->tracked = true;
     GB_LAUNCH(e, -1, launch_integrate_bits(a, e->stream));
     GB_TRY(fetch_output(e, nc, s.d_counts, s.h_counts, counts_host, [&]() -> int {
         return download(e, reinterpret_cast<BitEvent*>(events_host), s.d_events.p, ne, s.h_events);
@@ -901,6 +908,16 @@ int gb200_tracker_set_fix_solver(gb200_tracker* t, int solver) {
     // the receiver's stop and slide so far came from the mode they were computed in
     if (t->fix.bank.p) GB_FAIL(t->e, GB200_ESTATE, "the fix solver cannot change after the tracker's first fix call");
     t->fix.solver = solver;
+    return GB200_OK;
+}
+
+int gb200_tracker_set_code_phase_mode(gb200_tracker* t, int mode) {
+    if (!t) return GB200_EINVAL;
+    if (mode != GB200_CODE_PHASE_REFERENCE && mode != GB200_CODE_PHASE_SAMPLES)
+        GB_FAIL(t->e, GB200_EINVAL, "unknown code-phase mode %d", mode);
+    // the channels' accumulators and the integrators' queued stamps already hold the modulus they were computed with
+    if (t->tracked) GB_FAIL(t->e, GB200_ESTATE, "the code-phase mode cannot change after the tracker's first tracking call");
+    t->code_wrap = mode == GB200_CODE_PHASE_SAMPLES ? static_cast<double>(t->e->N) : kReferenceCodeWrap;
     return GB200_OK;
 }
 

@@ -51,7 +51,7 @@ __device__ __forceinline__ void track_prologue(const TrackArgs& a, int ch, Track
         dst[i] = v;
         if (shd) shd[i] = v;
     }
-    if (tid == 0) *tc = track_consts(a.fs);
+    if (tid == 0) *tc = track_consts(a.fs, a.code_wrap);
     rtab[tid] = tid ? 1.0 / static_cast<double>(tid) : 0.0;  // kTrackThreads == 256 entries
 }
 __device__ __forceinline__ void store_state(const TrackState* st, TrackState* gst, int tid) {

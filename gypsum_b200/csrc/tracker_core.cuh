@@ -106,13 +106,21 @@ GB_HD inline bool track_rot_ok_fast(double mr, double mi) {
     return q >= 0 ? q != 0 : track_rot_ok(mr, mi);
 }
 
+// Where the DLL accumulator wraps.  The reference hard-wires 2046 at every rate (tracker.py:301-303, :319; SURVEY F12);
+// the tracker's "samples" code-phase mode wraps at N, the stream's samples per millisecond, so that every code phase in
+// [0, N) stays on the signal.  At N = 2046 the two are the same computation.
+constexpr double kReferenceCodeWrap = 2046.0;
+
 // What _calculate_loop_filter_alpha_and_beta (tracker.py:228-244; lru-cached there as well) returns for the two loop
 // bandwidths the tracker ever uses: [0] = 3 Hz (locked), [1] = 6 Hz (pull-in).  Same expressions, same evaluation order.
+// wrap: the DLL accumulator's modulus (kReferenceCodeWrap or N).
 struct TrackConsts {
     double alpha[2], beta[2];
+    double wrap;
 };
-GB_HD inline TrackConsts track_consts(double fs) {
+GB_HD inline TrackConsts track_consts(double fs, double wrap = kReferenceCodeWrap) {
     TrackConsts c;
+    c.wrap = wrap;
     const double ts = 1.0 / fs;
     for (int i = 0; i < 2; ++i) {
         const double bw = i == 0 ? 3.0 : 6.0;
@@ -275,6 +283,13 @@ GB_HD inline bool track_constellation(const TrackState& st, double& circularity,
     return true;
 }
 
+// tracker.py:319: a pseudosymbol is stamped with its chunk's start and end times delayed by code_phase / wrap ms, the
+// delay rounded on its own and added to each time with its own rounding (the device adds with __dadd_rn, so that no
+// multiply-add fused into one rounding moves a stamp by an ulp).  Division by a runtime 2046.0 rounds as by the literal.
+GB_HD GB_INLINE double track_symbol_delay(int code_phase, double wrap) {
+    return (static_cast<double>(code_phase) / wrap) * 0.001;
+}
+
 // The scalar part of GpsSatelliteTracker.process_samples for one millisecond.  E, L, peak come from the
 // correlators (float32); everything after is float64.
 GB_HD inline void track_update(TrackState& st, float2 E, float2 L, float2 peak, float strength, int peak_offset,
@@ -284,7 +299,7 @@ GB_HD inline void track_update(TrackState& st, float2 E, float2 L, float2 peak, 
     const double disc = ((er * er + ei * ei) - (lr * lr + li * li)) / 2.0;
     st.phase_acc += disc * 0.002;
     st.code_phase = static_cast<int>(st.phase_acc);  // int(): truncation toward zero
-    st.phase_acc = pymod_near(st.phase_acc, 2046.0);  // hard-wired 2046 in the reference (SURVEY F12)
+    st.phase_acc = pymod_near(st.phase_acc, tc.wrap);  // 2046 in the reference at every rate (SURVEY F12), or N
     // --- histories, tracker.py:346 ---
     const double pre = peak.x, pim = peak.y;
     track_push_peak(st, pre, pim);

@@ -2,8 +2,8 @@
 pseudosymbol types, same names / fields / exception (tracker.py:33-110, :117-155, :206-389).
 
 `GpsSatelliteTracker.process_samples(chunk)` keeps the reference's one-millisecond-per-call contract; the trackers of
-one engine share a channel pool, so a chunk handed to N trackers in turn costs one GPU round trip, not N
-(`_ChannelPool`).  `TrackerBank` is the throughput interface: many channels x many milliseconds in one persistent-kernel
+one engine and code-phase mode share a channel pool, so a chunk handed to N trackers in turn costs one GPU round trip,
+not N (`_ChannelPool`).  `TrackerBank` is the throughput interface: many channels x many milliseconds in one persistent-kernel
 launch.  The correlators, loop filters, lock heuristics and the 6-second constellation check
 all run on the device (gypsum_b200/csrc/tracker.cu, tracker_core.cuh); this module only mirrors the host-visible
 state and histories the rest of gypsum reads.
@@ -151,10 +151,11 @@ def _apply_record(params: GpsSatelliteTrackingParameters, rec: tuple, profile=No
     params._last_is_locked = bool(rec[_LOCKED])
 
 
-def _pseudosymbol(rec, start_time: float, end_time: float) -> EmittedPseudosymbol:
+def _pseudosymbol(rec, start_time: float, end_time: float, wrap: int = _native.REFERENCE_CODE_WRAP) -> EmittedPseudosymbol:
+    """tracker.py:319-325: the chunk's times delayed by code_phase / wrap ms (track_symbol_delay in tracker_core.cuh)."""
     if not isinstance(rec, tuple):
         rec = rec.item()
-    delay = (rec[_CODE_PHASE] / 2046) * ONE_MILLISECOND  # tracker.py:319
+    delay = (rec[_CODE_PHASE] / wrap) * ONE_MILLISECOND
     return EmittedPseudosymbol(
         start_of_pseudosymbol=start_time + delay, end_of_pseudosymbol=end_time + delay,
         pseudosymbol=NavigationBitPseudosymbol.from_val(rec[_SYMBOL]), cursor_at_emit_time=0)
@@ -168,7 +169,8 @@ def _chunk_key(chunk) -> tuple:
 
 
 class _ChannelPool:
-    """Every GpsSatelliteTracker of one engine is a channel slot of ONE native pool (gb200_tracker_create_pool).
+    """Every GpsSatelliteTracker of one engine and code-phase mode is a channel slot of ONE native pool
+    (gb200_tracker_create_pool).
 
     The receiver hands the same chunk to every tracked satellite in turn (receiver.py:103-106, :237-257).  When the first
     tracker is asked about a chunk, all channels of the pool advance through it in one launch (one upload, one kernel, one
@@ -179,9 +181,13 @@ class _ChannelPool:
 
     CAPACITY = 64  # 32 GPS PRNs; room for re-acquisitions that overlap a dropped tracker's lifetime
 
-    def __init__(self, ent):
+    def __init__(self, ent, code_phase: str, samples_per_ms: int):
         self.engine = ent["engine"]
         self.native = _native.Tracker.pool(self.engine, self.CAPACITY)
+        self.code_wrap = _native.REFERENCE_CODE_WRAP  # what the pseudosymbol delay divides by
+        if code_phase != "reference":
+            self.native.set_code_phase_mode(code_phase)
+            self.code_wrap = samples_per_ms
         self.free = list(range(self.CAPACITY - 1, -1, -1))
         self.members: dict = {}   # channel -> weakref to its GpsSatelliteTracker
         self.ahead: dict = {}     # channel -> (chunk key, record, profile or None): computed, not yet asked for
@@ -244,16 +250,23 @@ class _ChannelPool:
         return rows[0], (None if prof is None else prof[0, 0])
 
 
-def _pool_of(ent) -> _ChannelPool:
-    pool = ent.get("tracker_pool")
-    if pool is None:
-        pool = ent["tracker_pool"] = _ChannelPool(ent)
-    return pool
+def _pool_of(ent, code_phase: str, samples_per_ms: int) -> _ChannelPool:
+    if code_phase not in _native.CODE_PHASE_MODES:
+        raise ValueError(f"code-phase mode must be one of {sorted(_native.CODE_PHASE_MODES)}, not {code_phase!r}")
+    pools = ent.setdefault("tracker_pools", {})
+    if code_phase not in pools:
+        pools[code_phase] = _ChannelPool(ent, code_phase, samples_per_ms)
+    return pools[code_phase]
 
 
 class GpsSatelliteTracker:
+    """tracker.py:206-389.  code_phase: "reference" (the default) counts code phase as the reference does, wrapping at
+    2046 at every rate; "samples" wraps at the stream's samples per millisecond, so that a satellite acquired at any code
+    phase stays tracked above 2.046 Msps (_native.Tracker.set_code_phase_mode).  The trackers of each mode batch within
+    their own pool: a chunk handed to trackers of both modes costs two launches."""
+
     def __init__(self, tracking_params: GpsSatelliteTrackingParameters, stream_attributes,
-                 keep_correlation_profiles: bool = True) -> None:
+                 keep_correlation_profiles: bool = True, code_phase: str = "reference") -> None:
         self.tracking_params = tracking_params
         self.stream_attributes = stream_attributes
         self.keep_correlation_profiles = keep_correlation_profiles
@@ -263,7 +276,7 @@ class GpsSatelliteTracker:
         self._ent = POOL.get(fs, n)
         self._eng = self._ent["engine"]
         idx = _replica_index(self._ent, tracking_params.satellite, n)
-        self._pool = _pool_of(self._ent)
+        self._pool = _pool_of(self._ent, code_phase, n)
         self._channel = self._pool.join(self, idx, tracking_params.current_doppler_shift,
                                         tracking_params.current_carrier_wave_phase_shift,
                                         tracking_params.current_prn_code_phase_shift)
@@ -315,16 +328,19 @@ class GpsSatelliteTracker:
         if rec[_LOST]:
             self._pool.stopped.add(self._channel)
             raise LostSatelliteLockError()  # tracker.py:378
-        return _pseudosymbol(rec, receiver_samples_chunk.start_time, receiver_samples_chunk.end_time)
+        return _pseudosymbol(rec, receiver_samples_chunk.start_time, receiver_samples_chunk.end_time, self._pool.code_wrap)
 
 
 class TrackerBank:
     """Throughput interface: `n` channels advance through a block of milliseconds in one persistent-kernel launch
     (BASELINE config 4).  channels: iterable of (satellite, doppler_hz, carrier_phase_rad, code_phase_samples).
     fix_solver: what position_fixes does with five or more ready satellites, "reference" (raise and stop, as the
-    reference receiver does) or "least_squares" (solve over all of them)."""
+    reference receiver does) or "least_squares" (solve over all of them).  code_phase: "reference" wraps the DLL at 2046
+    at every rate, as the reference does; "samples" wraps it at samples_per_ms, keeping every acquired code phase and
+    stamping each pseudosymbol with its true delay (_native.Tracker.set_code_phase_mode)."""
 
-    def __init__(self, channels, stream_attributes, device: int = 0, fix_solver: str = "reference"):
+    def __init__(self, channels, stream_attributes, device: int = 0, fix_solver: str = "reference",
+                 code_phase: str = "reference"):
         fs, n = int(stream_attributes.samples_per_second), int(stream_attributes.samples_per_prn_transmission)
         self.samples_per_ms = n
         self._ent = POOL.get(fs, n, device)
@@ -334,6 +350,7 @@ class TrackerBank:
         self.native = _native.Tracker(self.engine, idx, [c[1] for c in channels], [c[2] for c in channels],
                                       [c[3] for c in channels])
         self.native.set_fix_solver(fix_solver)
+        self.native.set_code_phase_mode(code_phase)
         self.n_channels = len(channels)
 
     def process(self, samples: np.ndarray, start_times, want_profiles: bool = False):

@@ -178,8 +178,9 @@ typedef struct gb200_track_record {
 
 /* satellite_signal_processing_pipeline.py:56-63: one channel per (replica row, Doppler, carrier phase, code
  * phase).  Works at every rate gb200_create accepts (samples_per_ms / 1023 in {1, 2, 3, 4, 5, 6, 8, 10, 12,
- * 16}).  Like the reference, the code-phase accumulator wraps at 2046 and the pseudosymbol delay is code phase /
- * 2046 ms at every rate (tracker.py:301-303,319): above 2.046 Msps only code phases below 2046 can be kept.     */
+ * 16}).  By default, like the reference, the code-phase accumulator wraps at 2046 and the pseudosymbol delay is code
+ * phase / 2046 ms at every rate (tracker.py:301-303,319): above 2.046 Msps only code phases below 2046 can be kept.
+ * gb200_tracker_set_code_phase_mode(GB200_CODE_PHASE_SAMPLES) keeps every code phase in [0, N) at every rate.     */
 int gb200_tracker_create(gb200_engine* e, int n_channels, const int32_t* prn_idx, const double* doppler_hz,
                          const double* carrier_phase, const int32_t* code_phase, gb200_tracker** out);
 int gb200_tracker_destroy(gb200_tracker* t);
@@ -410,6 +411,16 @@ int gb200_tracker_position_fixes_device(gb200_tracker* t, const double* receiver
 #define GB200_FIX_SOLVER_REFERENCE 0
 #define GB200_FIX_SOLVER_LEAST_SQUARES 1
 int gb200_tracker_set_fix_solver(gb200_tracker* t, int solver);
+/* How a tracker (bank or pool) counts code phase: GB200_CODE_PHASE_REFERENCE (the default) wraps the DLL accumulator at
+ * 2046 and delays each pseudosymbol by code phase / 2046 ms at every rate, as the reference does; GB200_CODE_PHASE_SAMPLES
+ * wraps it at N, the engine's samples per millisecond, and delays each pseudosymbol by code phase / N ms, so that a
+ * satellite acquired at any code phase in [0, N) stays tracked and its bits, subframes and fixes carry its true delay.
+ * The two are the same computation at 2.046 Msps.  Nothing else about the loop changes (DESIGN.md §7).  GB200_EINVAL
+ * for another value; GB200_ESTATE after the tracker's first gb200_tracker_process, _process_device, _process_channels
+ * or _integrate_bits call, whose accumulators and stamps used the mode in force. */
+#define GB200_CODE_PHASE_REFERENCE 0
+#define GB200_CODE_PHASE_SAMPLES 1
+int gb200_tracker_set_code_phase_mode(gb200_tracker* t, int mode);
 /* The receiver's state after the last fix call: the clock slide (NaN = None), whether it has stopped, and
  * order[n_channels]: the channels in world-model order, -1 after the last. */
 int gb200_tracker_receiver_state(gb200_tracker* t, double* slide, int32_t* stopped, int32_t* order);

@@ -1,6 +1,7 @@
 """Secondary measurements on one H100 (not the driver's bench line): BASELINE configs 2 (single block), 3, 5,
 the real 10-pass detector, and config 4 (tracking, at 2.046 and at 16.368 Msps).  Prints one JSON line per workload.
-usage: python tools/bench_configs.py [--quick]"""
+usage: python tools/bench_configs.py [--quick]
+       python tools/bench_configs.py --code-phase-modes R   config 4 only, both code-phase modes alternating, R rounds"""
 import json
 import os
 import sys
@@ -135,7 +136,15 @@ def detector_case():
                       "found": [[r.satellite_id.id, r.doppler_shift, r.prn_phase_shift] for r in found]}), flush=True)
 
 
-def tracker_case(n_ch, n_ms):
+def gpu_card():
+    """The card's name and power limit, read where the numbers are measured."""
+    import subprocess
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
+
+
+def tracker_case(n_ch, n_ms, code_phase="reference"):
     n, fs = 2046, 2046000
     eng = _native.Engine(fs, n)
     eng.set_replicas(CHIPS)
@@ -143,6 +152,7 @@ def tracker_case(n_ch, n_ms):
     base = to.synth_tracking_iq(5, n, 2000, fs, chans)
     x = np.tile(base, -(-n_ms // 2000))[: n_ms * n]  # periodic signal; noise repeats, which tracking does not care about
     trk = _native.Tracker(eng, [c[0] - 1 for c in chans], [c[1] for c in chans], [0.0] * n_ch, [c[3] for c in chans])
+    trk.set_code_phase_mode(code_phase)
     times = np.array([round(k * n / fs, 6) for k in range(n_ms)])
     xd = torch.from_numpy(x).cuda()
     eng.bind_iq_device(xd.data_ptr(), x.size)
@@ -157,11 +167,13 @@ def tracker_case(n_ch, n_ms):
     trk.integrate_bits(min(n_ms, 1000), times[:1000], ends[:1000], out.data_ptr())  # warm-up (allocations); state is reset below
     trk.close()
     trk = _native.Tracker(eng, [c[0] - 1 for c in chans], [c[1] for c in chans], [0.0] * n_ch, [c[3] for c in chans])
+    trk.set_code_phase_mode(code_phase)
     t0 = time.perf_counter()
     bits = trk.integrate_bits(n_ms, times, ends, out.data_ptr())
     dt_bits = time.perf_counter() - t0
     rec = out.cpu().numpy().view(_native.TRACK_DTYPE).reshape(n_ch, n_ms)
     print(json.dumps({"workload": f"config 4: {n_ch}-channel E/P/L tracking, {n_ms / 1000:.0f} s of IQ @ 2.046 Msps",
+                      "code_phase": code_phase,
                       "seconds": dt, "channel_ms_per_s": n_ch * n_ms / dt, "us_per_ms_per_channel_stream": dt / n_ms * 1e6,
                       "realtime_factor": (n_ms / 1000) / dt, "Msamples_per_s_stream": n_ms * n / dt / 1e6,
                       "locked_fraction_last_second": float(rec["locked"][:, -1000:].mean()),
@@ -172,7 +184,7 @@ def tracker_case(n_ch, n_ms):
     eng.close()
 
 
-def tracker_case_16368(n_ch, n_ms):
+def tracker_case_16368(n_ch, n_ms, code_phase="reference"):
     """Config 4 at 16.368 Msps (k_track_channels_wide<16>): device-resident IQ, a 1-s synthetic base repeated.  Planted code
     phases stay below 2046, the only ones the reference's tracker keeps at this rate.  The symbols of 3 channels over the
     first second are checked against the tracker oracle."""
@@ -192,9 +204,11 @@ def tracker_case_16368(n_ch, n_ms):
     out = torch.empty(n_ch * n_ms * _native.TRACK_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
     torch.cuda.synchronize()  # the stream and its buffers are ready before the engine's stream reads them
     trk = _native.Tracker(eng, *seeds)
+    trk.set_code_phase_mode(code_phase)
     trk.process_device(200, times[:200], out.data_ptr())  # warm-up
     trk.close()
     trk = _native.Tracker(eng, *seeds)
+    trk.set_code_phase_mode(code_phase)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     torch.cuda.synchronize()
     e0.record(st)
@@ -207,11 +221,11 @@ def tracker_case_16368(n_ch, n_ms):
     check_ms, mism = min(n_ms, base_ms), {}
     for i in (0, 13, 31):
         sv, f, _, cp = chans[i][:4]
-        tr = t.TrackerOracle(sv, f, 0.0, cp, fs, n)
+        tr = t.TrackerOracle(sv, f, 0.0, cp, fs, n)  # planted below 2046: both modes follow the same trajectory
         want = [tr.step(base[k * n:(k + 1) * n], *t.chunk_times(k, fs, n))["symbol"] for k in range(check_ms)]
         mism[sv] = int(np.count_nonzero(rec["symbol"][i, :check_ms] != np.array(want)))
     print(json.dumps({"workload": f"config 4 @ 16.368 Msps: {n_ch}-channel tracking, {n_ms / 1000:.0f} s of device-resident IQ",
-                      "kernel": "k_track_channels_wide<16>", "device_seconds": dt, "us_per_stream_ms": dt / n_ms * 1e6,
+                      "kernel": "k_track_channels_wide<16>", "code_phase": code_phase, "device_seconds": dt, "us_per_stream_ms": dt / n_ms * 1e6,
                       "realtime_factor": (n_ms / 1000) / dt, "channel_ms_per_s": n_ch * n_ms / dt,
                       "lost_channels": int((rec["lost"] > 0).any(axis=1).sum()),
                       "oracle_symbol_mismatches": {"ms": check_ms, "by_sv": mism},
@@ -220,7 +234,14 @@ def tracker_case_16368(n_ch, n_ms):
     eng.close()
 
 
-if __name__ == "__main__":
+if __name__ == "__main__" and "--code-phase-modes" in sys.argv:
+    rounds = int(sys.argv[sys.argv.index("--code-phase-modes") + 1])
+    print(json.dumps({"gpu": gpu_card()}), flush=True)
+    for _ in range(rounds):
+        for mode in ("reference", "samples"):
+            tracker_case(32, 5000 if quick else 60000, mode)
+            tracker_case_16368(32, 2000 if quick else 10000, mode)
+elif __name__ == "__main__":
     grid_case("config 2, one block", 2046, 1, 41, 1, 200)
     grid_case("config 2 x 32 blocks", 2046, 1, 41, 32, 50)
     grid_case("config 3: 32x41x10 ms @ 4.092 Msps", 4092, 10, 41, 1, 20)

@@ -169,5 +169,21 @@ pool.undo_channel(1)
 r2 = pool.process_channels([1], 1, [0.0])
 assert r1["symbol"][0, 0] == r2["symbol"][0, 0]
 pool.close()
+# the samples code-phase mode: a bank call with bits at a code phase past 2046, and a drop-in pool step
+xs = to.synth_tracking_iq(5, n, 20, fs, [(25, 1500.3, 0.0, 12345, 0.3, 0.002)])
+eng.upload_iq(xs)
+t = _native.Tracker(eng, [24, 6], [1500.0, -100.0], [0.0, 0.0], [12345, n - 1])
+t.set_code_phase_mode("samples")
+ts = [round(k * n / fs, 6) for k in range(20)]
+rec = t.process(20, ts)
+t.integrate_bits(20, ts, [round((k + 1) * n / fs, 6) for k in range(20)])
+assert (rec["code_phase"][0] >= 2046).all()
+t.close()
+pool = _native.Tracker.pool(eng, 2)
+pool.set_code_phase_mode("samples")
+pool.reset_channel(0, 24, 1500.0, 0.0, 12345)
+r1 = pool.process_channels([0], 1, [0.0], keep_undo=True)
+assert r1["code_phase"][0, 0] >= 2046
+pool.close()
 eng.close()
 print("sanitize_small ok")
