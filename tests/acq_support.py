@@ -4,6 +4,7 @@ import functools
 import math
 import multiprocessing as mp
 import os
+import warnings
 
 import numpy as np
 
@@ -167,6 +168,102 @@ def check_search(got, sv, ref, ambiguous, x, fs, n, what):
         assert ambiguous, what
         prof = o.integrate(o.NON_COHERENT, x, fs, n, doppler, o.replica(sv, n))
         assert abs(o.peak_strength(prof) - strength) <= 1e-4 * strength, what
+
+
+def _traced_worker(args):
+    sv, x, fs, n = args
+    trace = []
+    with warnings.catch_warnings():  # all-zero input: numpy's mean of an empty slice, the strength NaN (utils.py:111-116)
+        warnings.simplefilter("ignore", RuntimeWarning)
+        r = o.acquire_sv(sv, x, fs, n, trace)
+    return r, trace, o.search_is_ambiguous(trace, MAG_TOL)
+
+
+def oracle_searches_traced(svs, x, fs, n):
+    """{sv: (o.acquire_sv result, its trace, whether it sits on a branch point)}, each distinct SV searched once, one
+    process each."""
+    uniq = sorted(set(int(sv) for sv in svs))
+    with _pool(len(uniq)) as pool:
+        return dict(zip(uniq, pool.map(_traced_worker, [(sv, x, fs, n) for sv in uniq])))
+
+
+# ---- the on-device search's plan (gb200_detect) and the oracle's trace ------------------------------------------------
+REFINE_MAX_BINS = 32  # kRefineMaxBins: (satellite, bin) slots per satellite and pass
+SPREADS = [7000.0 / 2 ** k for k in range(10)]  # acquisition.py:78-89: 7000 halved while >= 10
+DEFAULT_SPEC_BUDGET_MB = 512  # GB200_SPEC_BUDGET_MB when unset
+FUSED_RATES = (2, 4)  # fused_supports: the block-per-cell kernel, no spectra scratch and no groups
+
+
+def refine_slots(center, spread):
+    """k_refine_plan restated: Dopplers of a satellite's kRefineMaxBins slots, NaN past the bins of
+    range(int(c - s), int(c + s), int(s / 10)) (int() truncates toward zero)."""
+    lo, hi, step = int(center - spread), int(center + spread), int(spread / 10)
+    return [float(lo + b * step) if lo + b * step < hi else math.nan for b in range(REFINE_MAX_BINS)]
+
+
+def detect_plan(s, m, n_sv, sms, budget_mb=DEFAULT_SPEC_BUDGET_MB):
+    """gb200_detect's schedule at S = s, M = m for n_sv satellites on a card of `sms` SMs with a budget_mb MiB spectra
+    budget: the refinement passes' correlate slots per CTA, rsplit, cells per group (cpg), groups per satellite (gps),
+    satellites per spectra chunk, the chunks (first satellite, satellites) and each chunk's CTA count; the coherent pass's
+    rsplit and CTA count.  The fused kernel (S = 2, 4) runs every pass as one launch of a CTA per slot instead."""
+    slots = 12 if m == 1 else 8  # correlate_slots, non-coherent: one-warp kernel
+    n_cells = n_sv * REFINE_MAX_BINS
+    rsplit = 1 if n_cells >= 8 * sms * slots else math.gcd(s, slots)  # pick_rsplit
+    cpg = slots // rsplit
+    gps = -(-REFINE_MAX_BINS // cpg)
+    unit_bytes = m * s * 2 * 1024 * 8  # unit_floats2 float2s: one (block, Doppler) spectra unit
+    spc = min(max(1, (budget_mb << 20) // (unit_bytes * REFINE_MAX_BINS)), n_sv)
+    chunks = [(sv0, min(spc, n_sv - sv0)) for sv0 in range(0, n_sv, spc)]
+    crsplit = 1 if n_sv >= 8 * sms * 8 else math.gcd(s, 8)  # coherent pass: warp-pair kernel, 8 pairs
+    return dict(slots=slots, rsplit=rsplit, cpg=cpg, gps=gps, group_sizes=[min(cpg, REFINE_MAX_BINS - g * cpg)
+                for g in range(gps)], sv_per_chunk=spc, chunks=chunks, grids=[min(k * gps, sms) for _, k in chunks],
+                crsplit=crsplit, coherent_grid=min(n_sv, sms), fused=s in FUSED_RATES)
+
+
+def budget_for(s, m, n_sv, spc, sms, limit_mb=4096):
+    """The smallest whole-MiB budget (>= 1) whose plan has spc satellites per chunk, or None."""
+    for mb in range(1, limit_mb + 1):
+        got = detect_plan(s, m, n_sv, sms, mb)["sv_per_chunk"]
+        if got == spc:
+            return mb
+        if got > spc:
+            return None
+    return None
+
+
+def trace_passes(trace):
+    """[(centre, spread, chosen Doppler, strength)] of each pass of an o.acquire_sv trace."""
+    out, centre = [], 0.0
+    for spread, p in zip(SPREADS, trace):
+        out.append((centre, spread, p["chosen"], p["strength"]))
+        centre = p["chosen"]
+    return out
+
+
+def kept_pass(trace):
+    """1-based pass whose result the search keeps: the first pass, replaced only by a strictly greater strength (NaN
+    never replaces and is never replaced)."""
+    kept, best = 1, trace[0]["strength"]
+    for k, p in enumerate(trace[1:], 2):
+        if p["strength"] > best:
+            kept, best = k, p["strength"]
+    return kept
+
+
+def centre_outside(trace, limit=7000.0):
+    """Whether a pass of the search is centred beyond +-limit Hz."""
+    return any(abs(c) > limit for c, _, _, _ in trace_passes(trace))
+
+
+def truncation_differs(trace):
+    """Whether a pass's lower edge c - spread is a negative non-integer, where int() (toward zero) and floor differ."""
+    return any(c - s < 0 and c - s != math.floor(c - s) for c, s, _, _ in trace_passes(trace))
+
+
+def centre_crosses_zero(trace):
+    """Whether consecutive pass centres (pass 1's 0 excluded) lie on both sides of zero."""
+    cs = [c for c, _, _, _ in trace_passes(trace)[1:]] + [trace[-1]["chosen"]]
+    return any(a * b < 0 for a, b in zip(cs, cs[1:]))
 
 
 def _is_ambiguous(sv, x, fs, n):
