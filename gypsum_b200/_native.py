@@ -128,6 +128,15 @@ def _ptr(a: np.ndarray) -> int:
     return a.ctypes.data
 
 
+def _records_out(out: np.ndarray | None, shape: tuple) -> np.ndarray:
+    """A grid's record buffer: out, which must be a C-contiguous RECORD_DTYPE array of that shape, or a new one."""
+    if out is None:
+        return np.empty(shape, dtype=RECORD_DTYPE)
+    if out.dtype != RECORD_DTYPE or out.shape != shape or not out.flags["C_CONTIGUOUS"]:
+        raise ValueError("out must be a C-contiguous RECORD_DTYPE array of shape [n_blocks, n_prn, n_doppler]")
+    return out
+
+
 class Engine:
     """One engine per (device, sample rate).  Thin, exception-raising wrapper over the C ABI."""
 
@@ -225,10 +234,7 @@ class Engine:
         (e.g. a view of a torch pinned tensor) the records are DMA'd straight into it."""
         prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
         dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
-        if out is None:
-            out = np.empty((n_blocks, prn.size, dop.size), dtype=RECORD_DTYPE)
-        elif out.dtype != RECORD_DTYPE or out.shape != (n_blocks, prn.size, dop.size) or not out.flags["C_CONTIGUOUS"]:
-            raise ValueError("out must be a C-contiguous RECORD_DTYPE array of shape [n_blocks, n_prn, n_doppler]")
+        out = _records_out(out, (n_blocks, prn.size, dop.size))
         self._check(
             self._lib.gb200_acquire_grid(self._h, n_blocks, ms_per_block, _ptr(prn), prn.size, _ptr(dop), dop.size, kind,
                                          _ptr(out)),
@@ -245,18 +251,14 @@ class Engine:
         c = self._host_call_cache
         if c is not None and c[0] is prn_idx and c[1] is doppler_hz and c[2] is out:
             prn, dop, p_prn, p_dop, p_out = c[3:]
+            _records_out(out, (n_blocks, prn.size, dop.size))
         else:
             prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
             dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
-            if out is None:
-                out = np.empty((n_blocks, prn.size, dop.size), dtype=RECORD_DTYPE)
-                cacheable = False
-            else:
-                cacheable = prn is prn_idx and dop is doppler_hz  # no converted copies that could go stale
+            cacheable = out is not None and prn is prn_idx and dop is doppler_hz  # no converted copies that could go stale
+            out = _records_out(out, (n_blocks, prn.size, dop.size))
             p_prn, p_dop, p_out = _ptr(prn), _ptr(dop), _ptr(out)
             self._host_call_cache = (prn_idx, doppler_hz, out, prn, dop, p_prn, p_dop, p_out) if cacheable else None
-        if out.dtype != RECORD_DTYPE or out.shape != (n_blocks, prn.size, dop.size) or not out.flags["C_CONTIGUOUS"]:
-            raise ValueError("out must be a C-contiguous RECORD_DTYPE array of shape [n_blocks, n_prn, n_doppler]")
         if isinstance(iq, int):
             keep, ptr = None, iq
         elif isinstance(iq, np.integer):
@@ -377,10 +379,7 @@ class GridStream:
             if keep.size != self.samples_per_batch:
                 raise ValueError(f"a batch is {self.samples_per_batch} samples, got {keep.size}")
             ptr = _ptr(keep)
-        if out is None:
-            out = np.empty(self.shape, dtype=RECORD_DTYPE)
-        elif out.dtype != RECORD_DTYPE or out.shape != self.shape or not out.flags["C_CONTIGUOUS"]:
-            raise ValueError("out must be a C-contiguous RECORD_DTYPE array of shape [n_blocks, n_prn, n_doppler]")
+        out = _records_out(out, self.shape)
         self._engine.iq_tag = None  # the stream rebinds the engine's IQ to its own slot buffer
         self._engine._check(self._lib.gb200_grid_stream_submit(self._h, ptr, _ptr(out)), "gb200_grid_stream_submit")
         self._pending.append((keep, out))

@@ -13,7 +13,7 @@ import numpy as np
 
 from gypsum_b200 import _native
 from gypsum_b200.constants import ACQUISITION_INTEGRATED_CORRELATION_STRENGTH_DETECTION_THRESHOLD
-from gypsum_b200.utils import POOL, IntegrationType, _kind, chips_of_replica
+from gypsum_b200.utils import POOL, IntegrationType, _kind, chips_of_satellite
 
 _logger = logging.getLogger(__name__)
 
@@ -57,15 +57,7 @@ class GpsSatelliteDetector:
         key = (getattr(satellite_id, "id", satellite_id), n)
         c = self._chips_cache.get(key)
         if c is None:
-            sat = self.satellites_by_id[satellite_id]
-            code = getattr(getattr(sat, "prn_code", None), "inner", None)
-            if code is not None and n // 1023 == getattr(sat, "scale_factor", n // 1023):
-                c = np.ascontiguousarray(np.asarray(code) != 0, dtype=np.uint8)
-            else:
-                c, roll = chips_of_replica(sat.prn_as_complex, n)
-                if roll:
-                    raise ValueError("satellite replica must not be rolled")
-            self._chips_cache[key] = c
+            c = self._chips_cache[key] = chips_of_satellite(self.satellites_by_id[satellite_id], n)
         return c
 
     def _prepare(self, satellite_ids, antenna_data, stream_attributes):

@@ -48,10 +48,6 @@ namespace {
 
 thread_local std::string g_create_error;
 
-// L2 window of the one-warp correlate kernel: the fastest size for the benchmark's config-2 call and for config 3 on the
-// H100's 50 MB L2 (DESIGN.md §4, L2 windows).
-constexpr int kL2WindowMb = 16;
-
 int env_int(const char* name, int dflt) {
     const char* v = getenv(name);
     return (v && *v) ? atoi(v) : dflt;
@@ -103,20 +99,28 @@ CorrelateArgs correlate_args(const gb200_engine* e, int M, int kind, int rsplit,
     return ca;
 }
 
-// The fused-kernel arguments every launch sets (the kernel is configured on first use); the caller adds its cells.
-int fused_args(gb200_engine* e, int M, FusedArgs* fa) {
+// One fused block-per-cell launch (a CTA per cell, the whole pipeline in one kernel; configured on first use) over n_cells
+// cells, each with its Doppler, replica row and optional coherent probe index (probe may be null).
+int launch_fused(gb200_engine* e, int M, int kind, const double* doppler, const int* prn, const int* probe, CellRecord* records,
+                 int n_cells) {
     if (!e->fused_configured) {
         GB_CUDA(e, configure_fused_kernel());
         e->fused_configured = true;
     }
-    *fa = FusedArgs{};
-    fa->iq = e->iq;
-    fa->crep = e->crep.p;
-    fa->tw1 = e->tw1.p;
-    fa->tw2 = e->tw2.p;
-    fa->inv_fs = 1.0 / static_cast<double>(e->fs);
-    fa->N = e->N;
-    fa->M = M;
+    FusedArgs fa{};
+    fa.iq = e->iq;
+    fa.crep = e->crep.p;
+    fa.tw1 = e->tw1.p;
+    fa.tw2 = e->tw2.p;
+    fa.inv_fs = 1.0 / static_cast<double>(e->fs);
+    fa.N = e->N;
+    fa.M = M;
+    fa.doppler = doppler;
+    fa.prn = prn;
+    fa.probe = probe;
+    fa.records = records;
+    fa.n_cells = n_cells;
+    GB_LAUNCH(e, 1, launch_acquire_fused(fa, e->s, kind, e->stream));
     return GB200_OK;
 }
 
@@ -140,6 +144,19 @@ struct ListPlan {
     }
 };
 
+// The split pipeline over groups [g0, g0 + n_groups) of the plan written at dev: doppler_spectra of the n_units Dopplers at
+// dop (spectrum unit u holds dop[u]), then correlate_cells.  probe, gate and profile are optional (see CorrelateArgs).
+int run_list(gb200_engine* e, const ListPlan& plan, const int* dev, int g0, int n_groups, int M, int kind, int rsplit,
+             const double* dop, int n_units, CellRecord* records, const int* probe, const double* gate, float* profile) {
+    GB_TRY(run_spectra(e, e->iq, M, dop, n_units, n_units));
+    CorrelateArgs ca = correlate_args(e, M, kind, rsplit, records, profile);
+    plan.bind(ca, dev, g0, n_groups);
+    ca.cell_probe = probe;
+    ca.cell_gate = gate;
+    GB_LAUNCH(e, 1, launch_correlate(ca, std::min(n_groups, e->num_sms), e->stream));
+    return GB200_OK;
+}
+
 // Argument rules of the acquisition entry points, one function each (host.cuh has the ones the trackers share).
 int check_kind(gb200_engine* e, int kind) {
     if (kind != GB200_COHERENT && kind != GB200_NON_COHERENT) GB_FAIL(e, GB200_EINVAL, "Unexpected integration type");
@@ -158,38 +175,40 @@ int check_common(gb200_engine* e, int n_ms, int kind) {
     return check_iq(e, n_ms);
 }
 
+// Points the engine's IQ at the n samples at buf.
+void bind_iq(gb200_engine* e, const float2* buf, int64_t n) {
+    e->iq = buf;
+    e->iq_samples = n;
+}
+
 // Forgets the engine's IQ binding when it points into the n samples at buf, which are about to be freed.
 void unbind_iq(gb200_engine* e, const float2* buf, size_t n) {
-    if (e->iq >= buf && e->iq < buf + n) {
-        e->iq = nullptr;
-        e->iq_samples = 0;
-    }
+    if (e->iq >= buf && e->iq < buf + n) bind_iq(e, nullptr, 0);
 }
 
 // The grid's axes (PRN rows in d_ints, Doppler bins in d_doppler) are uploaded only when they changed -- or when a list-mode
 // call (gb200_acquire_cells / gb200_detect) has reused those device buffers since.
 int upload_grid_axes(gb200_engine* e, const int32_t* prn_idx, int P, const double* dop, int D) {
-    const bool same = e->grid_cache_valid && static_cast<int>(e->doppler_cache.size()) == D &&
-                      static_cast<int>(e->prn_cache.size()) == P &&
-                      memcmp(e->doppler_cache.data(), dop, sizeof(double) * D) == 0 &&
-                      memcmp(e->prn_cache.data(), prn_idx, sizeof(int) * P) == 0;
+    auto& c = e->grid_axes;
+    const bool same = c.valid && static_cast<int>(c.dop.size()) == D && static_cast<int>(c.prn.size()) == P &&
+                      memcmp(c.dop.data(), dop, sizeof(double) * D) == 0 && memcmp(c.prn.data(), prn_idx, sizeof(int) * P) == 0;
     if (same) return GB200_OK;
     GB_CUDA(e, cudaStreamSynchronize(e->stream));  // staging buffers may still be in flight
     GB_CUDA(e, e->d_doppler.ensure(D));
     GB_CUDA(e, e->d_ints.ensure(P));
     GB_TRY(upload(e, e->d_doppler.p, dop, D, e->h_doubles));
     GB_TRY(upload(e, e->d_ints.p, prn_idx, P, e->h_ints));
-    e->doppler_cache.assign(dop, dop + D);
-    e->prn_cache.assign(prn_idx, prn_idx + P);
-    e->grid_cache_valid = true;
+    c.dop.assign(dop, dop + D);
+    c.prn.assign(prn_idx, prn_idx + P);
+    c.valid = true;
     return GB200_OK;
 }
 
-// grid mode: all cells of n_blocks x prn list x doppler list; records written to rec_dev (device)
+// grid mode: all cells of n_blocks x prn list x doppler list; records written to rec_dev (device).  The caller has applied
+// check_grid.
 int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D, int kind,
              CellRecord* rec_dev) {
     GB_TRY(check_common(e, M, kind));
-    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     if (static_cast<int64_t>(n_blocks) * M * e->N > e->iq_samples)
         GB_FAIL(e, GB200_EINVAL, "grid needs %lld samples, %lld loaded", static_cast<long long>(n_blocks) * M * e->N,
                 static_cast<long long>(e->iq_samples));
@@ -220,10 +239,10 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
         ca.prn_idx = e->d_ints.p;
         const int grid = std::min(ca.n_groups, e->num_sms);
         // L2 windows of the one-warp kernel (see the kernel; the pair kernel walks the batch as one window): a batch whose
-        // spectra exceed L2 is walked in equal runs of units of about GB200_L2_WINDOW_MB (default kL2WindowMb; 0 = off), as
-        // long as a window still gives every CTA at least two groups (the kernel's round-robin of the extra groups keeps the
-        // CTAs together).
-        static const size_t win_bytes = static_cast<size_t>(std::max(0, env_int("GB200_L2_WINDOW_MB", kL2WindowMb))) << 20;
+        // spectra exceed L2 is walked in equal runs of units of about l2_window_bytes (0 = off), as long as a window still
+        // gives every CTA at least l2_window_min_groups groups (the kernel's round-robin of the extra groups keeps the CTAs
+        // together).
+        const size_t win_bytes = e->l2_window_bytes;
         const size_t batch_bytes = static_cast<size_t>(nbb) * per_block * sizeof(float2);
         if (win_bytes && batch_bytes > win_bytes + win_bytes / 2) {
             const long long n_win = static_cast<long long>((batch_bytes + win_bytes - 1) / win_bytes);
@@ -232,8 +251,8 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
             const long long q = grid / std::gcd(P, grid);
             const long long even = ((wc + q / 2) / q) * q;
             if (even > 0 && even * 4 >= wc * 3 && even * 4 <= wc * 5) wc = even;
-            static const int min_groups = env_int("GB200_L2_WINDOW_MIN_GROUPS", 2);
-            if (wc * P >= static_cast<long long>(min_groups) * grid && wc < chunks) ca.win_chunks = static_cast<int>(wc);
+            if (wc * P >= static_cast<long long>(e->l2_window_min_groups) * grid && wc < chunks)
+                ca.win_chunks = static_cast<int>(wc);
         }
         GB_LAUNCH(e, 1, launch_correlate(ca, grid, e->stream));
     }
@@ -247,7 +266,7 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
     if (n_cells < 1 || !prn_idx || !dop) GB_FAIL(e, GB200_EINVAL, "empty cell list");
     GB_TRY(check_samples(e, M));
     GB_TRY(check_prns(e, prn_idx, n_cells));
-    e->grid_cache_valid = false;  // d_ints / d_doppler are about to be overwritten
+    e->grid_axes.valid = false;  // d_ints / d_doppler are about to be overwritten
 
     bool use_fused = e->fused == 1;
     if (e->fused < 0 && fused_supports(e->s) && !profile_dev) {
@@ -260,9 +279,6 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
         use_fused = n_unique * 4 > n_cells || static_cast<long long>(n_cells) * M <= 8192;
     }
     if (use_fused && fused_supports(e->s) && !profile_dev) {
-        // one CTA per cell, whole pipeline in one kernel
-        FusedArgs fa;
-        GB_TRY(fused_args(e, M, &fa));
         GB_CUDA(e, cudaStreamSynchronize(e->stream));
         GB_CUDA(e, e->d_ints.ensure(static_cast<size_t>(n_cells) * 2));
         GB_CUDA(e, e->h_ints.ensure(static_cast<size_t>(n_cells) * 2));
@@ -273,13 +289,7 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
         }
         GB_CUDA(e, cudaMemcpyAsync(e->d_ints.p, e->h_ints.p, sizeof(int) * 2 * n_cells, cudaMemcpyHostToDevice, e->stream));
         GB_TRY(upload(e, e->d_doppler.p, dop, n_cells, e->h_doubles));
-        fa.doppler = e->d_doppler.p;
-        fa.prn = e->d_ints.p;
-        fa.probe = e->d_ints.p + n_cells;
-        fa.records = rec_dev;
-        fa.n_cells = n_cells;
-        GB_LAUNCH(e, 1, launch_acquire_fused(fa, e->s, kind, e->stream));
-        return GB200_OK;
+        return launch_fused(e, M, kind, e->d_doppler.p, e->d_ints.p, e->d_ints.p + n_cells, rec_dev, n_cells);
     }
 
     const int slots = correlate_slots(kind, M, profile_dev != nullptr);
@@ -337,16 +347,20 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
         plan.write(e->h_ints.p + n_cells);
         GB_CUDA(e, cudaMemcpyAsync(di, e->h_ints.p + n_cells, sizeof(int) * plan.size(), cudaMemcpyHostToDevice, e->stream));
         GB_TRY(upload(e, e->d_doppler.p, udop.data(), udop.size(), e->h_doubles));
-
-        const int nu = static_cast<int>(udop.size()), ng = static_cast<int>(plan.grp_prn.size());
-        GB_TRY(run_spectra(e, e->iq, M, e->d_doppler.p, nu, nu));
-
-        CorrelateArgs ca = correlate_args(e, M, kind, rsplit, rec_dev, profile_dev);
-        plan.bind(ca, di, 0, ng);
-        ca.cell_probe = e->d_ints.p;
-        GB_LAUNCH(e, 1, launch_correlate(ca, std::min(ng, e->num_sms), e->stream));
+        GB_TRY(run_list(e, plan, di, 0, static_cast<int>(plan.grp_prn.size()), M, kind, rsplit, e->d_doppler.p,
+                        static_cast<int>(udop.size()), rec_dev, e->d_ints.p, nullptr, profile_dev));
         c0 = c1;
     }
+    return GB200_OK;
+}
+
+// The grid's records into d_records, after check_grid; with best, then each (block, PRN) row's best bin into best
+// (acquisition.py:179-189 on the device).
+int grid_records(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D, int kind,
+                 BestRecord* best) {
+    GB_CUDA(e, e->d_records.ensure(static_cast<size_t>(n_blocks) * P * D));
+    GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p));
+    if (best) GB_LAUNCH(e, -1, launch_best_bins(n_blocks * P, D, e->N, e->d_records.p, e->d_doppler.p, best, e->stream));
     return GB200_OK;
 }
 
@@ -386,6 +400,10 @@ int gb200_create(int device, int fs, int n, gb200_engine** out) {
     // Spectra scratch per launch pair.  It does not have to stay in L2 (a launch writes and re-reads 21 MB per 16.368 Msps
     // block), and launches that carry more cells run the correlate kernel without cross-warp merges and with a shorter tail.
     e->spec_budget_bytes = static_cast<size_t>(env_int("GB200_SPEC_BUDGET_MB", 512)) << 20;
+    // L2 window of the one-warp correlate kernel: 16 MB is the fastest size for the benchmark's config-2 call and for config 3
+    // on the H100's 50 MB L2 (DESIGN.md §4, L2 windows).
+    e->l2_window_bytes = static_cast<size_t>(std::max(0, env_int("GB200_L2_WINDOW_MB", 16))) << 20;
+    e->l2_window_min_groups = env_int("GB200_L2_WINDOW_MIN_GROUPS", 2);
     auto fail = [&](cudaError_t c, const char* what) {
         g_create_error = std::string(what) + ": " + cudaGetErrorString(c);
         cudaGetLastError();
@@ -464,8 +482,7 @@ int gb200_upload_iq(gb200_engine* e, const float* iq_host, int64_t n_samples) {
     }
     GB_CUDA(e, cudaMemcpyAsync(e->iq_own.p, src, static_cast<size_t>(n_samples) * sizeof(float2), cudaMemcpyHostToDevice,
                                e->stream));
-    e->iq = e->iq_own.p;
-    e->iq_samples = n_samples;
+    bind_iq(e, e->iq_own.p, n_samples);
     return GB200_OK;
 }
 
@@ -474,8 +491,7 @@ int gb200_bind_iq_device(gb200_engine* e, const void* iq_device, int64_t n_sampl
     if (!iq_device || n_samples < 0) GB_FAIL(e, GB200_EINVAL, "bad IQ buffer");
     // the fused acquisition kernel stages the IQ with cp.async.bulk and the tracking kernel with 16-byte cp.async
     if (reinterpret_cast<uintptr_t>(iq_device) % 16 != 0) GB_FAIL(e, GB200_EINVAL, "IQ buffer must be 16-byte aligned");
-    e->iq = static_cast<const float2*>(iq_device);
-    e->iq_samples = n_samples;
+    bind_iq(e, static_cast<const float2*>(iq_device), n_samples);
     return GB200_OK;
 }
 
@@ -484,6 +500,8 @@ int gb200_acquire_grid_device(gb200_engine* e, int n_blocks, int M, const int32_
     if (!e) return GB200_EINVAL;
     if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
     GB_CUDA(e, cudaSetDevice(e->device));
+    GB_TRY(check_common(e, M, kind));
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     return run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, static_cast<CellRecord*>(out_device));
 }
 
@@ -493,25 +511,17 @@ int gb200_acquire_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_
     if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    const size_t n = static_cast<size_t>(n_blocks) * P * D;
-    GB_CUDA(e, e->d_records.ensure(n));
-    GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p));
-    return fetch_records(e, n, out_host);
+    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, kind, nullptr));
+    return fetch_records(e, static_cast<size_t>(n_blocks) * P * D, out_host);
 }
 
-// acquisition.py:179-189 per (block, prn) row on the device: the grid, then one reduction kernel over its records.
 int gb200_acquire_grid_best_device(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D,
                                    int kind, void* out_device) {
     if (!e) return GB200_EINVAL;
     if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    const size_t n = static_cast<size_t>(n_blocks) * P * D;
-    GB_CUDA(e, e->d_records.ensure(n));
-    GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p));
-    GB_LAUNCH(e, -1, launch_best_bins(n_blocks * P, D, e->N, e->d_records.p, e->d_doppler.p, static_cast<BestRecord*>(out_device),
-                                      e->stream));
-    return GB200_OK;
+    return grid_records(e, n_blocks, M, prn_idx, P, dop, D, kind, static_cast<BestRecord*>(out_device));
 }
 
 int gb200_acquire_grid_best(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D,
@@ -522,7 +532,7 @@ int gb200_acquire_grid_best(gb200_engine* e, int n_blocks, int M, const int32_t*
     GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     const size_t n = static_cast<size_t>(n_blocks) * P;
     GB_CUDA(e, e->d_best.ensure(n));
-    GB_TRY(gb200_acquire_grid_best_device(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_best.p));
+    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_best.p));
     return download(e, reinterpret_cast<BestRecord*>(out_host), e->d_best.p, n, e->h_best);
 }
 
@@ -552,8 +562,7 @@ int gb200_acquire_grid_host(gb200_engine* e, const float* iq_host, int n_blocks,
     const float2* h2d_src = reinterpret_cast<const float2*>(iq_host);
     const bool eager_src = n_iq * sizeof(float2) > (64u << 10) && is_pinned(iq_host);
     if (!eager_src) GB_CUDA(e, stage_in(e->h_iq, h2d_src, n_iq));
-    e->iq = e->iq_own.p;
-    e->iq_samples = static_cast<int64_t>(n_iq);
+    bind_iq(e, e->iq_own.p, static_cast<int64_t>(n_iq));
 
     // The captured kernels read the axes from d_doppler / d_ints and the replica spectra from crep: make sure those hold THIS
     // grid's axes now (a list-mode call may have reused them since the last replay; cheap when nothing changed), and treat a
@@ -685,8 +694,7 @@ int gb200_ring_bind_newest(gb200_ring* r, int n_ms) {
         GB_FAIL(e, GB200_EINVAL, "the ring holds %lld of at most %d ms; %d asked for",
                 static_cast<long long>(std::min<int64_t>(r->appended, r->capacity)), r->capacity, n_ms);
     const int first = static_cast<int>((r->appended - n_ms) % r->capacity);
-    e->iq = r->buf.p + static_cast<size_t>(first) * e->N;
-    e->iq_samples = static_cast<int64_t>(n_ms) * e->N;
+    bind_iq(e, r->buf.p + static_cast<size_t>(first) * e->N, static_cast<int64_t>(n_ms) * e->N);
     return GB200_OK;
 }
 
@@ -805,83 +813,62 @@ int gb200_detect(gb200_engine* e, int n_sv, const int32_t* prn_idx, int n_ms, gb
         coh.grp_prn.push_back(prn_idx[sv]);
     }
     const size_t n_plans = plan.size() + coh.size();
+    auto& r = e->search;
     GB_CUDA(e, cudaStreamSynchronize(e->stream));
-    GB_CUDA(e, e->r_ints.ensure(n_plans + n_sv));
-    GB_CUDA(e, e->rh_ints.ensure(n_plans + n_sv));
-    plan.write(e->rh_ints.p);
-    coh.write(e->rh_ints.p + plan.size());
-    int* di = e->r_ints.p;
-    GB_CUDA(e, cudaMemcpyAsync(di, e->rh_ints.p, sizeof(int) * n_plans, cudaMemcpyHostToDevice, e->stream));
+    GB_CUDA(e, r.d_ints.ensure(n_plans + n_sv));
+    GB_CUDA(e, r.h_ints.ensure(n_plans + n_sv));
+    plan.write(r.h_ints.p);
+    coh.write(r.h_ints.p + plan.size());
+    int* di = r.d_ints.p;
+    GB_CUDA(e, cudaMemcpyAsync(di, r.h_ints.p, sizeof(int) * n_plans, cudaMemcpyHostToDevice, e->stream));
     int* d_probe = di + n_plans;
 
-    GB_CUDA(e, e->r_state.ensure(n_sv));
-    GB_CUDA(e, e->r_doppler.ensure(static_cast<size_t>(n_cells) + n_sv));
-    GB_CUDA(e, e->r_records.ensure(static_cast<size_t>(n_cells) + n_sv));
-    GB_CUDA(e, e->r_results.ensure(n_sv));
+    GB_CUDA(e, r.state.ensure(n_sv));
+    GB_CUDA(e, r.d_doppler.ensure(static_cast<size_t>(n_cells) + n_sv));
+    GB_CUDA(e, r.d_records.ensure(static_cast<size_t>(n_cells) + n_sv));
+    GB_CUDA(e, r.d_results.ensure(n_sv));
     GB_CUDA(e, e->spec.ensure(unit * std::max(sv_per_chunk * MAXB, n_sv)));
-    double* d_coh_doppler = e->r_doppler.p + n_cells;
-    CellRecord* d_coh_records = e->r_records.p + n_cells;
+    double* d_coh_doppler = r.d_doppler.p + n_cells;
+    CellRecord* d_coh_records = r.d_records.p + n_cells;
 
     // Every (satellite, bin) cell of a refinement pass has its own Doppler, so nothing is shared between PRNs: the
     // fused block-per-cell kernel does the same arithmetic without the spectra round trip through HBM.
     const bool use_fused = fused_supports(e->s);
-    FusedArgs fbase{};
-    const int* d_cell_prn = nullptr;
     if (use_fused) {
-        GB_TRY(fused_args(e, n_ms, &fbase));
         // [n_cells] replica row of every (satellite, bin) slot, then [n_sv] one per satellite for the coherent pass
-        GB_CUDA(e, e->r_cell_prn.ensure(static_cast<size_t>(n_cells) + n_sv));
-        GB_CUDA(e, e->rh_cell_prn.ensure(static_cast<size_t>(n_cells) + n_sv));
-        for (int c = 0; c < n_cells; ++c) e->rh_cell_prn.p[c] = prn_idx[c / MAXB];
-        for (int sv = 0; sv < n_sv; ++sv) e->rh_cell_prn.p[n_cells + sv] = prn_idx[sv];
-        GB_CUDA(e, cudaMemcpyAsync(e->r_cell_prn.p, e->rh_cell_prn.p, sizeof(int) * (n_cells + n_sv), cudaMemcpyHostToDevice,
+        GB_CUDA(e, r.d_cell_prn.ensure(static_cast<size_t>(n_cells) + n_sv));
+        GB_CUDA(e, r.h_cell_prn.ensure(static_cast<size_t>(n_cells) + n_sv));
+        for (int c = 0; c < n_cells; ++c) r.h_cell_prn.p[c] = prn_idx[c / MAXB];
+        for (int sv = 0; sv < n_sv; ++sv) r.h_cell_prn.p[n_cells + sv] = prn_idx[sv];
+        GB_CUDA(e, cudaMemcpyAsync(r.d_cell_prn.p, r.h_cell_prn.p, sizeof(int) * (n_cells + n_sv), cudaMemcpyHostToDevice,
                                    e->stream));
-        d_cell_prn = e->r_cell_prn.p;
     }
 
-    GB_LAUNCH(e, -1, launch_refine_init(n_sv, e->r_state.p, e->stream));
+    GB_LAUNCH(e, -1, launch_refine_init(n_sv, r.state.p, e->stream));
     for (double spread = 7000.0; spread >= 10.0; spread /= 2.0) {  // acquisition.py:78-89
-        GB_LAUNCH(e, -1, launch_refine_plan(n_sv, spread, e->r_state.p, e->r_doppler.p, e->stream));
-        if (use_fused) {
-            // one launch per pass: a CTA per (satellite, bin) slot, no spectra scratch
-            FusedArgs fa = fbase;
-            fa.doppler = e->r_doppler.p;
-            fa.prn = d_cell_prn;
-            fa.probe = nullptr;
-            fa.records = e->r_records.p;
-            fa.n_cells = n_cells;
-            GB_LAUNCH(e, 1, launch_acquire_fused(fa, e->s, GB200_NON_COHERENT, e->stream));
-        }
+        GB_LAUNCH(e, -1, launch_refine_plan(n_sv, spread, r.state.p, r.d_doppler.p, e->stream));
+        // fused: one launch per pass, a CTA per (satellite, bin) slot, no spectra scratch
+        if (use_fused)
+            GB_TRY(launch_fused(e, n_ms, GB200_NON_COHERENT, r.d_doppler.p, r.d_cell_prn.p, nullptr, r.d_records.p, n_cells));
         for (int sv0 = 0; !use_fused && sv0 < n_sv; sv0 += sv_per_chunk) {
             const int nsv = std::min(sv_per_chunk, n_sv - sv0);
-            GB_TRY(run_spectra(e, e->iq, n_ms, e->r_doppler.p + static_cast<size_t>(sv0) * MAXB, nsv * MAXB, nsv * MAXB));
-            CorrelateArgs ca = correlate_args(e, n_ms, GB200_NON_COHERENT, rsplit, e->r_records.p, nullptr);
-            plan.bind(ca, di, sv0 * gps, nsv * gps);
-            ca.cell_gate = e->r_doppler.p;
-            GB_LAUNCH(e, 1, launch_correlate(ca, std::min(ca.n_groups, e->num_sms), e->stream));
+            GB_TRY(run_list(e, plan, di, sv0 * gps, nsv * gps, n_ms, GB200_NON_COHERENT, rsplit,
+                            r.d_doppler.p + static_cast<size_t>(sv0) * MAXB, nsv * MAXB, r.d_records.p, nullptr, r.d_doppler.p,
+                            nullptr));
         }
-        GB_LAUNCH(e, -1, launch_refine_select(n_sv, e->N, e->r_records.p, e->r_doppler.p, e->r_state.p, e->stream));
+        GB_LAUNCH(e, -1, launch_refine_select(n_sv, e->N, r.d_records.p, r.d_doppler.p, r.state.p, e->stream));
     }
     // coherent integration at the kept Doppler (acquisition.py:120-136)
-    GB_LAUNCH(e, -1, launch_refine_coherent_plan(n_sv, e->r_state.p, d_coh_doppler, d_probe, e->stream));
+    GB_LAUNCH(e, -1, launch_refine_coherent_plan(n_sv, r.state.p, d_coh_doppler, d_probe, e->stream));
     if (use_fused) {
-        FusedArgs fa = fbase;
-        fa.doppler = d_coh_doppler;
-        fa.prn = d_cell_prn + n_cells;
-        fa.probe = d_probe;
-        fa.records = d_coh_records;
-        fa.n_cells = n_sv;
-        GB_LAUNCH(e, 1, launch_acquire_fused(fa, e->s, GB200_COHERENT, e->stream));
+        GB_TRY(launch_fused(e, n_ms, GB200_COHERENT, d_coh_doppler, r.d_cell_prn.p + n_cells, d_probe, d_coh_records, n_sv));
     } else {
-        GB_TRY(run_spectra(e, e->iq, n_ms, d_coh_doppler, n_sv, n_sv));
         const int crsplit = pick_rsplit(e, correlate_slots(GB200_COHERENT, n_ms, false), n_sv);
-        CorrelateArgs ca = correlate_args(e, n_ms, GB200_COHERENT, crsplit, d_coh_records, nullptr);
-        coh.bind(ca, di + plan.size(), 0, n_sv);
-        ca.cell_probe = d_probe;
-        GB_LAUNCH(e, 1, launch_correlate(ca, std::min(n_sv, e->num_sms), e->stream));
+        GB_TRY(run_list(e, coh, di + plan.size(), 0, n_sv, n_ms, GB200_COHERENT, crsplit, d_coh_doppler, n_sv, d_coh_records,
+                        d_probe, nullptr, nullptr));
     }
-    GB_LAUNCH(e, -1, launch_refine_finalize(n_sv, e->r_state.p, d_coh_records, e->r_results.p, e->stream));
-    return download(e, reinterpret_cast<RefineResult*>(out_host), e->r_results.p, n_sv, e->rh_results);
+    GB_LAUNCH(e, -1, launch_refine_finalize(n_sv, r.state.p, d_coh_records, r.d_results.p, e->stream));
+    return download(e, reinterpret_cast<RefineResult*>(out_host), r.d_results.p, n_sv, r.h_results);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -962,8 +949,7 @@ int gb200_grid_stream_submit(gb200_grid_stream* g, const float* iq_host, gb200_c
     GB_CUDA(e, cudaMemcpyAsync(sl.iq.p, src, n_iq * sizeof(float2), cudaMemcpyHostToDevice, g->s_in));
     GB_CUDA(e, cudaEventRecord(sl.h2d, g->s_in));
     GB_CUDA(e, cudaStreamWaitEvent(e->stream, sl.h2d, 0));
-    e->iq = sl.iq.p;
-    e->iq_samples = static_cast<int64_t>(n_iq);
+    bind_iq(e, sl.iq.p, static_cast<int64_t>(n_iq));
     GB_TRY(run_grid(e, g->n_blocks, g->M, g->prn.data(), g->P, g->dop.data(), g->D, g->kind, sl.rec.p));
     GB_CUDA(e, cudaEventRecord(sl.done, e->stream));
     GB_CUDA(e, cudaStreamWaitEvent(g->s_out, sl.done, 0));

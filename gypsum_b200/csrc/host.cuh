@@ -64,29 +64,32 @@ struct gb200_engine {
     gb::capi::DevBuf<int> d_ints;
     gb::capi::DevBuf<gb::CellRecord> d_records;
     gb::capi::DevBuf<float> d_profile;
-    // on-device refinement (gb200_detect)
-    gb::capi::DevBuf<gb::RefineState> r_state;
-    gb::capi::DevBuf<double> r_doppler;
-    gb::capi::DevBuf<gb::CellRecord> r_records;
-    gb::capi::DevBuf<int> r_ints;
-    gb::capi::DevBuf<gb::RefineResult> r_results;
-    gb::capi::DevBuf<int> r_cell_prn;
-    gb::capi::PinnedBuf<int> rh_cell_prn;
-    gb::capi::PinnedBuf<int> rh_ints;
-    gb::capi::PinnedBuf<gb::RefineResult> rh_results;
+    struct {  // gb200_detect, the on-device satellite search
+        gb::capi::DevBuf<gb::RefineState> state;
+        gb::capi::DevBuf<double> d_doppler;
+        gb::capi::DevBuf<gb::CellRecord> d_records;
+        gb::capi::DevBuf<int> d_ints, d_cell_prn;
+        gb::capi::DevBuf<gb::RefineResult> d_results;
+        gb::capi::PinnedBuf<int> h_ints, h_cell_prn;
+        gb::capi::PinnedBuf<gb::RefineResult> h_results;
+    } search;
     gb::capi::PinnedBuf<float2> h_iq, h_replica;
     gb::capi::PinnedBuf<gb::CellRecord> h_records;
     gb::capi::PinnedBuf<int> h_ints;
     gb::capi::PinnedBuf<double> h_doubles;
     gb::capi::PinnedBuf<float> h_profile;
-    std::vector<double> doppler_cache;  // what d_doppler[0..] currently holds (grid mode)
-    std::vector<int> prn_cache;         // what d_ints[0..] currently holds (grid mode)
-    bool grid_cache_valid = false;
+    struct {  // the grid axes d_doppler[0..] and d_ints[0..] hold, until a list-mode call reuses those buffers
+        std::vector<double> dop;
+        std::vector<int> prn;
+        bool valid = false;
+    } grid_axes;
     int n_prn = 0;
     const float2* iq = nullptr;
     int64_t iq_samples = 0;
     int64_t launches = 0;
-    size_t spec_budget_bytes = 512u << 20;
+    // read from the environment at gb200_create: GB200_SPEC_BUDGET_MB, GB200_L2_WINDOW_MB, GB200_L2_WINDOW_MIN_GROUPS
+    size_t spec_budget_bytes = 512u << 20, l2_window_bytes = 16u << 20;
+    int l2_window_min_groups = 2;
     bool timing = false;
     int fused = -1;  // acquire_cells kernel choice: -1 automatic, 0 doppler_spectra + correlate_cells, 1 fused block-per-cell
     bool fused_configured = false;

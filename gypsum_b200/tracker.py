@@ -19,7 +19,7 @@ import numpy as np
 
 from gypsum_b200 import _native
 from gypsum_b200.constants import ONE_MILLISECOND
-from gypsum_b200.utils import POOL, chips_of_replica
+from gypsum_b200.utils import POOL, chips_of_satellite
 
 
 class LostSatelliteLockError(Exception):  # tracker.py:33
@@ -109,17 +109,6 @@ class GpsSatelliteTrackingParameters:
 
     def is_locked(self) -> bool:
         return self._last_is_locked
-
-
-def _replica_index(ent, satellite, n: int) -> int:
-    code = getattr(getattr(satellite, "prn_code", None), "inner", None)
-    if code is not None and getattr(satellite, "scale_factor", n // 1023) == n // 1023:
-        chips = np.ascontiguousarray(np.asarray(code) != 0, dtype=np.uint8)
-    else:
-        chips, roll = chips_of_replica(satellite.prn_as_complex, n)
-        if roll:
-            raise ValueError("satellite replica must not be rolled")
-    return POOL.replica_index(ent, chips)
 
 
 # A record travels through this module as the plain tuple `np.void.item()` gives (one conversion per record instead of one
@@ -275,7 +264,7 @@ class GpsSatelliteTracker:
         fs, n = int(stream_attributes.samples_per_second), int(stream_attributes.samples_per_prn_transmission)
         self._ent = POOL.get(fs, n)
         self._eng = self._ent["engine"]
-        idx = _replica_index(self._ent, tracking_params.satellite, n)
+        idx = POOL.replica_index(self._ent, chips_of_satellite(tracking_params.satellite, n))
         self._pool = _pool_of(self._ent, code_phase, n)
         self._channel = self._pool.join(self, idx, tracking_params.current_doppler_shift,
                                         tracking_params.current_carrier_wave_phase_shift,
@@ -346,7 +335,7 @@ class TrackerBank:
         self._ent = POOL.get(fs, n, device)
         self.engine = self._ent["engine"]
         channels = list(channels)
-        idx = [_replica_index(self._ent, c[0], n) for c in channels]
+        idx = [POOL.replica_index(self._ent, chips_of_satellite(c[0], n)) for c in channels]
         self.native = _native.Tracker(self.engine, idx, [c[1] for c in channels], [c[2] for c in channels],
                                       [c[3] for c in channels])
         self.native.set_fix_solver(fix_solver)

@@ -42,14 +42,7 @@ class _EnginePool:
         return ent
 
     def replica_index(self, ent, chips: np.ndarray) -> int:
-        k = chips.tobytes()
-        idx = ent["codes"].get(k)
-        if idx is None:
-            idx = len(ent["table"])
-            ent["table"].append(chips)
-            ent["codes"][k] = idx
-            ent["engine"].set_replicas(np.stack(ent["table"]))
-        return idx
+        return self.ensure_table(ent, [chips])[0]
 
     def ensure_table(self, ent, chips_list) -> list[int]:
         """Register several codes with a single device upload."""
@@ -95,24 +88,42 @@ def chips_of_replica(prn_as_complex: np.ndarray, n: int) -> tuple[np.ndarray, in
     raise NotAChipReplica("replica is not chips repeated samples_per_ms/1023 times")
 
 
-def frequency_domain_correlation(antenna_samples: np.ndarray, prn_replica: np.ndarray) -> np.ndarray:
-    """utils.py:59-73: circular cross-correlation ifft(fft(x) conj(fft(prn))) of one millisecond -> complex128[N]."""
-    x = np.ascontiguousarray(antenna_samples, dtype=np.complex64)
-    n = x.size
+def chips_of_satellite(satellite, n: int) -> np.ndarray:
+    """chips uint8[1023] of a satellite: its PRN code when its replica has n/1023 samples per chip, else recovered from its
+    replica (prn_as_complex), which must not be rolled."""
+    code = getattr(getattr(satellite, "prn_code", None), "inner", None)
+    if code is not None and getattr(satellite, "scale_factor", n // 1023) == n // 1023:
+        return np.ascontiguousarray(np.asarray(code) != 0, dtype=np.uint8)
+    chips, roll = chips_of_replica(satellite.prn_as_complex, n)
+    if roll:
+        raise ValueError("satellite replica must not be rolled")
+    return chips
+
+
+def _profile(x: np.ndarray, fs: int, n: int, n_ms: int, prn_replica, doppler: float, kind: int) -> np.ndarray:
+    """The correlation profile of the n_ms milliseconds x against the replica at doppler, widened as the reference's:
+    through the replica table when the replica is chips (the roll undone on the result), else correlated directly."""
     rep = np.asarray(prn_replica)
     if rep.shape != (n,):
         raise ValueError(f"replica must have {n} samples")
-    ent = POOL.get(n * 1000, n)
+    ent = POOL.get(fs, n)
     eng = ent["engine"]
+    wide = np.complex128 if kind == _native.COHERENT else np.float64
     try:
         chips, roll = chips_of_replica(rep, n)
     except NotAChipReplica:  # any other replica: direct circular correlation on the device
         eng.upload_iq(x)
-        return eng.correlation_profile_replica(rep, 0.0, 1, _native.COHERENT).astype(np.complex128)
+        return eng.correlation_profile_replica(rep, doppler, n_ms, kind).astype(wide)
     idx = POOL.replica_index(ent, chips)
     eng.upload_iq(x)
-    prof = eng.correlation_profile(idx, 0.0, 1, _native.COHERENT).astype(np.complex128)
+    prof = eng.correlation_profile(idx, doppler, n_ms, kind).astype(wide)
     return np.roll(prof, -roll) if roll else prof
+
+
+def frequency_domain_correlation(antenna_samples: np.ndarray, prn_replica: np.ndarray) -> np.ndarray:
+    """utils.py:59-73: circular cross-correlation ifft(fft(x) conj(fft(prn))) of one millisecond -> complex128[N]."""
+    x = np.ascontiguousarray(antenna_samples, dtype=np.complex64)
+    return _profile(x, x.size * 1000, x.size, 1, prn_replica, 0.0, _native.COHERENT)
 
 
 def integrate_correlation_with_doppler_shifted_prn(
@@ -126,21 +137,7 @@ def integrate_correlation_with_doppler_shifted_prn(
     n_ms = data.size // n  # utils.py:34-38: a trailing partial chunk is dropped
     if n_ms == 0:
         return np.zeros(n, dtype=complex if kind == _native.COHERENT else np.float64)
-    rep = np.asarray(prn_as_complex)
-    if rep.shape != (n,):
-        raise ValueError(f"replica must have {n} samples")
-    ent = POOL.get(fs, n)
-    eng = ent["engine"]
-    wide = np.complex128 if kind == _native.COHERENT else np.float64
-    try:
-        chips, roll = chips_of_replica(rep, n)
-    except NotAChipReplica:  # any other replica: direct circular correlation on the device
-        eng.upload_iq(data[: n_ms * n])
-        return eng.correlation_profile_replica(rep, float(doppler_shift), n_ms, kind).astype(wide)
-    idx = POOL.replica_index(ent, chips)
-    eng.upload_iq(data[: n_ms * n])
-    prof = eng.correlation_profile(idx, float(doppler_shift), n_ms, kind).astype(wide)
-    return np.roll(prof, -roll) if roll else prof
+    return _profile(data[: n_ms * n], fs, n, n_ms, prn_as_complex, float(doppler_shift), kind)
 
 
 def get_normalized_correlation_peak_strength(profile: np.ndarray) -> float:

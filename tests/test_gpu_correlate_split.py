@@ -357,8 +357,8 @@ def window_shape(s, m, sms, rotating):
 @pytest.mark.parametrize("rotating", [False, True], ids=["few_groups", "rotating_extras"])
 @pytest.mark.parametrize("m", [1, 3])
 def test_l2_windows_against_oracle(native_lib, sms, tmp_path, m, rotating):
-    """GB200_L2_WINDOW_MB = 1 and GB200_L2_WINDOW_MIN_GROUPS = 0 in a child process (the knobs are read once per process),
-    S = 2: every record of the windowed walk against the oracle and the guard rows, not only against the unwindowed launch."""
+    """GB200_L2_WINDOW_MB = 1 and GB200_L2_WINDOW_MIN_GROUPS = 0 for an engine created in a child process, S = 2: every
+    record of the windowed walk against the oracle and the guard rows, not only against the unwindowed launch."""
     s = 2
     n, fs = rate(s)
     P, nb, D, wc = window_shape(s, m, sms, rotating)

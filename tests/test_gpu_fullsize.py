@@ -161,8 +161,8 @@ e.close()
 @pytest.mark.parametrize("n, nb", [(2046, 20), (16368, 3)])
 def test_l2_windows_leave_every_record_unchanged(engines, tmp_path, n, nb):
     """The one-warp kernel walks batches larger than L2 in windows of units (group order window / PRN / chunk, extra groups going
-    round the CTAs).  That only reorders independent cells: with windows forced onto a small batch (a child process, the knobs
-    are read once per process) every record is byte-identical to the single-window launch's, also with a ragged last window."""
+    round the CTAs).  That only reorders independent cells: with windows forced onto a small batch (an engine
+    created in a child process) every record is byte-identical to the single-window launch's, also with a ragged last window."""
     rng = np.random.default_rng(n + nb)
     x = (rng.standard_normal(2 * n * nb).astype(np.float32)).view(np.complex64)
     x[:n] += o.synth_iq(0, n, 1, n * 1000, [(25, 1500.0, 777, 0.3, 0.3)], sigma=0.0)
