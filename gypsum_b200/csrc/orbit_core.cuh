@@ -415,19 +415,23 @@ GB_HD inline void orbit_observe(const OrbitSnap& s, int m, SvObservation& o) {
 // one channel's call
 // ---------------------------------------------------------------------------------------------------------------------
 
-// The state the call starts from: the carried state, tracked from millisecond 0 unless it is dropped there.
-GB_HD GB_INLINE void orbit_begin(OrbitSnap& s, int drop_ms) {
+// The state the call starts from: the carried state, tracked from millisecond 0 unless it is dropped there.  Returns
+// true when the satellite starts counting here, so that millisecond 0 is the first one it is seen in.
+GB_HD GB_INLINE bool orbit_begin(OrbitSnap& s, int drop_ms) {
     s.ms = -1;
     if (!s.frozen && drop_ms != 0 && !s.counting) {  // handle_prn_observed: a satellite seen for the first time starts at 0
         s.counting = 1;
         s.count = 0;
+        return true;
     }
+    return false;
 }
 
 // One decoder event at millisecond m (non-decreasing within the call) of a channel dropped at drop_ms (-1 = never); f:
-// the event's fields when it is a subframe (kind 0).  Returns true when the state changed and `s` (the state at the end
-// of m) belongs in the change table.
-GB_HD inline bool orbit_event(OrbitSnap& s, const SubframeEvent& ev, int m, int drop_ms, const SubframeFields& f) {
+// the event's fields when it is a subframe (kind 0); fresh: orbit_begin started the channel counting.  The events of
+// one millisecond apply in order, so a subframe before a raise in the same millisecond holds and one after it does not
+// (DESIGN.md §8b).  Returns true when the state changed and `s` (the state at the end of m) belongs in the change table.
+GB_HD inline bool orbit_event(OrbitSnap& s, const SubframeEvent& ev, int m, int drop_ms, const SubframeFields& f, bool fresh) {
     if (s.frozen || (drop_ms >= 0 && m >= drop_ms)) return false;  // the receiver has dropped this pipeline
     if (ev.kind == kNavSubframe) {
         orbit_advance(s, m);
@@ -435,6 +439,7 @@ GB_HD inline bool orbit_event(OrbitSnap& s, const SubframeEvent& ev, int m, int 
         return true;
     }
     if (ev.kind == kNavRaised) {  // uncaught ValueError: the receiver stops before it counts millisecond m
+        if (fresh && m == 0 && s.ms < 0) s.counting = 0;  // ... so a satellite first seen at m was never counted
         s.count = orbit_count_at(s, m - 1 > s.ms ? m - 1 : s.ms);
         s.ms = m;
         s.frozen = 1;
@@ -449,7 +454,7 @@ GB_HD inline bool orbit_event(OrbitSnap& s, const SubframeEvent& ev, int m, int 
 template <class MsOf>
 GB_HD inline void orbit_walk(OrbitSnap& s, const SubframeEvent* ev, int n, MsOf ms_of, int drop_ms, int n_ms,
                              SubframeFields* fields, int& n_fields, OrbitSnap* chg, int& n_chg) {
-    orbit_begin(s, drop_ms);
+    const bool fresh = orbit_begin(s, drop_ms);
     n_fields = n_chg = 0;
     chg[n_chg++] = s;
     for (int j = 0; j < n; ++j) {
@@ -462,7 +467,7 @@ GB_HD inline void orbit_walk(OrbitSnap& s, const SubframeEvent* ev, int n, MsOf 
             f.ms = m;
             fields[n_fields++] = f;
         }
-        if (orbit_event(s, e, m, drop_ms, f)) chg[n_chg++] = s;
+        if (orbit_event(s, e, m, drop_ms, f, fresh)) chg[n_chg++] = s;
     }
     if (drop_ms >= 0 && !s.frozen) {
         orbit_advance(s, drop_ms);

@@ -203,7 +203,11 @@ class OrbitOracle:
 
 def run_call(sv: OrbitOracle, events, drop_ms: int, n_ms: int, observe=True):
     """One call of one channel: events [(kind, words, trailing_edge, ms)] in millisecond order, the drop millisecond
-    (-1 = none).  Returns the parsed fields of the kind-0 events and, with observe, the observation of every ms."""
+    (-1 = none).  Returns the parsed fields of the kind-0 events and, with observe, the observation of every ms.
+
+    The events of one millisecond apply in order (DESIGN.md §8b): a raise freezes the channel after the subframes before
+    it in its millisecond, so that millisecond is counted only when one of them precedes the raise; what follows the
+    raise is ignored.  The reference's decoder never emits both in one millisecond."""
     fields = [(j, ms, parse(w)) for j, (kind, w, _, ms) in enumerate(events) if kind == nav.KIND_SUBFRAME]
     by_ms: dict = {}
     for kind, w, te, ms in events:
@@ -211,21 +215,29 @@ def run_call(sv: OrbitOracle, events, drop_ms: int, n_ms: int, observe=True):
     obs = []
     tracked = True
     for m in range(n_ms):
-        if not sv.frozen:
-            if m == drop_ms and tracked:
-                sv.lost()
-                tracked = False
-            raised = any(k == nav.KIND_RAISED for k, _, _ in by_ms.get(m, ())) and tracked
-            if raised:
-                sv.frozen = True  # the step of millisecond m never returns: nothing of it is counted
-            elif tracked:
-                sv.prn_observed()
-                for kind, w, te in by_ms.get(m, ()):
-                    if kind == nav.KIND_SUBFRAME:
-                        sv.subframe(parse(w), te)
+        tracked = step(sv, by_ms.get(m, []), m == drop_ms, tracked)
         if observe:
             obs.append(sv.observe())
     return fields, obs
+
+
+def step(sv: OrbitOracle, evs, dropped_here: bool, tracked: bool) -> bool:
+    """One millisecond of run_call: its events [(kind, words, trailing_edge)] in order, whether the channel is dropped
+    at it and whether it is still tracked.  Returns whether it is tracked after it."""
+    if sv.frozen:
+        return tracked
+    if dropped_here and tracked:
+        sv.lost()
+        tracked = False
+    r = next((i for i, (k, _, _) in enumerate(evs) if k == nav.KIND_RAISED), len(evs))
+    before = [(w, te) for k, w, te in evs[:r] if k == nav.KIND_SUBFRAME]
+    if tracked and (r == len(evs) or before):
+        sv.prn_observed()
+        for w, te in before:
+            sv.subframe(parse(w), te)
+    if tracked and r < len(evs):
+        sv.frozen = True  # the step of millisecond m never returns: nothing after the raise is counted
+    return tracked
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -172,23 +172,10 @@ def params_timeline(chans, n_ms, sv=None):
 
 def _replay(o, events, drop_ms, n_ms, out):
     """orb.run_call, keeping the parameters after every millisecond in out [n_ms][26]."""
-    from oracle import nav_oracle as nav
-
     by_ms: dict = {}
     for kind, w, te, ms in events:
         by_ms.setdefault(ms, []).append((kind, w, te))
     tracked = True
     for m in range(n_ms):
-        if not o.frozen:
-            if m == drop_ms and tracked:
-                o.lost()
-                tracked = False
-            raised = any(k == nav.KIND_RAISED for k, _, _ in by_ms.get(m, ())) and tracked
-            if raised:
-                o.frozen = True
-            elif tracked:
-                o.prn_observed()
-                for kind, w, te in by_ms.get(m, ()):
-                    if kind == nav.KIND_SUBFRAME:
-                        o.subframe(orb.parse(w), te)
+        tracked = orb.step(o, by_ms.get(m, []), m == drop_ms, tracked)
         out[m] = [np.nan if v is None else float(v) for v in o.p]
