@@ -2,6 +2,7 @@
 // holds the engine's lifetime, its IQ and every acquisition entry point; receiver.cu holds the trackers.
 // Host side of the reference path it replaces: gypsum/acquisition.py:154-219 (the per-bin scan and its memo
 // wrapper) and gypsum/utils.py:77-108.
+#include <cmath>
 #include <cstdlib>
 #include <map>
 #include <numeric>
@@ -163,9 +164,18 @@ int check_kind(gb200_engine* e, int kind) {
     return GB200_OK;
 }
 
+// Every Doppler a caller passes is finite.  NaN is gb200_detect's own "slot switched off" mark (k_doppler_spectra and
+// k_acquire_fused skip such a bin, leaving its spectra or record unwritten), and +-inf gives a NaN carrier; the reference
+// returns an all-NaN profile for both, which no record can stand for.
+int check_dopplers(gb200_engine* e, const double* dop, int n) {
+    for (int i = 0; i < n; ++i)
+        if (!std::isfinite(dop[i])) GB_FAIL(e, GB200_EINVAL, "Doppler %d is not finite (%g Hz)", i, dop[i]);
+    return GB200_OK;
+}
+
 int check_grid(gb200_engine* e, int n_blocks, int P, int D, const int32_t* prn_idx, const double* dop) {
     if (n_blocks < 1 || P < 1 || D < 1 || !prn_idx || !dop) GB_FAIL(e, GB200_EINVAL, "empty grid");
-    return GB200_OK;
+    return check_dopplers(e, dop, D);
 }
 
 // What every acquisition needs before its own arguments are looked at.
@@ -264,6 +274,7 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
               int kind, CellRecord* rec_dev, float* profile_dev) {
     GB_TRY(check_common(e, M, kind));
     if (n_cells < 1 || !prn_idx || !dop) GB_FAIL(e, GB200_EINVAL, "empty cell list");
+    GB_TRY(check_dopplers(e, dop, n_cells));
     GB_TRY(check_samples(e, M));
     GB_TRY(check_prns(e, prn_idx, n_cells));
     e->grid_axes.valid = false;  // d_ints / d_doppler are about to be overwritten
@@ -732,6 +743,7 @@ int gb200_correlation_profile_replica(gb200_engine* e, const float* replica_host
     if (!e) return GB200_EINVAL;
     if (!replica_host || !out_host) GB_FAIL(e, GB200_EINVAL, "null buffer");
     GB_TRY(check_kind(e, kind));
+    GB_TRY(check_dopplers(e, &dop, 1));
     GB_TRY(check_iq(e, n_ms));
     GB_TRY(check_samples(e, n_ms));
     GB_CUDA(e, cudaSetDevice(e->device));

@@ -6,6 +6,7 @@ reference's, computed in float32 (tolerance: DESIGN.md section 6).
 """
 from __future__ import annotations
 
+import math
 from enum import Enum, auto
 
 import numpy as np
@@ -106,9 +107,11 @@ def _profile(x: np.ndarray, fs: int, n: int, n_ms: int, prn_replica, doppler: fl
     rep = np.asarray(prn_replica)
     if rep.shape != (n,):
         raise ValueError(f"replica must have {n} samples")
+    wide = np.complex128 if kind == _native.COHERENT else np.float64
+    if not math.isfinite(doppler):  # a NaN carrier: every value of the reference's profile is NaN (the engine refuses it)
+        return np.full(n, complex(math.nan, math.nan) if kind == _native.COHERENT else math.nan, dtype=wide)
     ent = POOL.get(fs, n)
     eng = ent["engine"]
-    wide = np.complex128 if kind == _native.COHERENT else np.float64
     try:
         chips, roll = chips_of_replica(rep, n)
     except NotAChipReplica:  # any other replica: direct circular correlation on the device

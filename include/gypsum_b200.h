@@ -87,7 +87,10 @@ int gb200_ring_appended(const gb200_ring* r, int64_t* total_ms);
 /* Benchmark-shaped search grid (SURVEY.md 8d): the loaded IQ holds n_blocks independent blocks of
  * ms_per_block milliseconds; every (block, prn_idx[a], doppler_hz[b]) cell is one
  * utils.py:77 integrate_correlation_with_doppler_shifted_prn evaluation reduced to a record.
- * out[(block*n_prn + a)*n_doppler + b].                                                             */
+ * out[(block*n_prn + a)*n_doppler + b].
+ * Every Doppler a caller passes -- to the grid calls below, gb200_grid_stream_create, gb200_acquire_cells and both
+ * gb200_correlation_profile calls -- must be finite: NaN or +-inf is GB200_EINVAL naming the first such index, and
+ * nothing is launched (the reference's profile of such a cell is all NaN, which no record can stand for).          */
 int gb200_acquire_grid(gb200_engine* e, int n_blocks, int ms_per_block, const int32_t* prn_idx, int n_prn,
                        const double* doppler_hz, int n_doppler, int integration_type, gb200_cell_record* out_host);
 int gb200_acquire_grid_device(gb200_engine* e, int n_blocks, int ms_per_block, const int32_t* prn_idx, int n_prn,

@@ -128,6 +128,102 @@ def check_grid(rec, x, fs, n, svs, dop, what, kind=o.NON_COHERENT, ref=None):
     return len(bad)
 
 
+def _cells_cols(x, fs, n, svs, dop, kind, probe, cols):
+    """vector_cells over the Doppler columns cols ([cell indices] of one bit-equal Doppler each)."""
+    out = []
+    for idx in cols:
+        pr = None if probe is None else np.asarray(probe)[idx][:, None]
+        out.append(_vector_cols(x, fs, n, [svs[i] for i in idx], dop[idx[:1]], kind, pr))
+    return out
+
+
+def _cell_list_worker(args):
+    return _cells_cols(*args)
+
+
+def vector_cells(x, fs, n, svs, dop, kind=o.NON_COHERENT, probe=None):
+    """vector_grid for a cell list: cell i is (svs[i], dop[i]), and with probe its profile value at lag probe[i].  Returns
+    (peak, argmax, sum, count, probe values), each [len(svs)].  Cells of bit-equal Dopplers share one wiped-off forward FFT
+    per millisecond; long lists are spread over the host's cores by Doppler."""
+    dop = np.asarray(dop, dtype=np.float64)
+    by_dop = {}
+    for i, f in enumerate(dop):
+        by_dop.setdefault(f.tobytes(), []).append(i)
+    cols = list(by_dop.values())
+    procs = max(1, min(len(cols), os.cpu_count() or 1, len(cols) * len(x) // (1 << 22)))
+    parts = [cols[i::procs] for i in range(procs)]
+    if procs == 1:
+        res = [_cells_cols(x, fs, n, list(svs), dop, kind, probe, cols)]
+    else:
+        with _pool(procs) as pool:
+            res = pool.map(_cell_list_worker, [(x, fs, n, list(svs), dop, kind, probe, p) for p in parts])
+    out = [np.zeros(dop.size, np.float64), np.zeros(dop.size, np.int64), np.zeros(dop.size, np.float64),
+           np.zeros(dop.size, np.int64), np.zeros(dop.size, complex)]
+    for p, r in zip(parts, res):
+        for idx, col in zip(p, r):
+            for o_, a in zip(out, col):
+                o_[idx] = a[:, 0]
+    return tuple(out)
+
+
+def check_cells(rec, ref, x, fs, n, svs, dop, what, kind=o.NON_COHERENT, probe=None):
+    """Every record of a cell list against vector_cells' ref, each against its own profile's maximum: peak and sum within
+    MAG_TOL of the oracle's, strength within 1e-4 (NaN where the oracle's is, as for all-zero input), count exact, argmax
+    exact bar near-ties proved on the float64 profile; coherent probes within MAG_TOL * peak of the oracle's complex value
+    at the probe lag, and exactly 0 without a probe or for non-coherent cells.  Returns the number of near-tie proofs."""
+    peak, arg, total, count, val = ref
+    assert rec.shape == peak.shape, what
+    assert (np.abs(rec["peak"] - peak) <= MAG_TOL * peak).all(), (what, np.flatnonzero(np.abs(rec["peak"] - peak) > MAG_TOL * peak)[:8])
+    assert (np.abs(rec["sum"] - total) <= MAG_TOL * total).all(), (what, np.flatnonzero(np.abs(rec["sum"] - total) > MAG_TOL * total)[:8])
+    assert np.array_equal(rec["count"], count), (what, np.flatnonzero(rec["count"] != count)[:8])
+    bad = np.flatnonzero(rec["argmax"] != arg)
+    for i in bad:
+        prof = np.abs(o.integrate(kind, x, fs, n, dop[i], o.replica(svs[i], n)))
+        assert prof.max() - prof[rec["argmax"][i]] <= MAG_TOL * prof.max(), (what, i, rec["argmax"][i], arg[i])
+    with np.errstate(invalid="ignore", divide="ignore"):
+        got_s = o.strength_from_record(rec["peak"].astype(np.float64), rec["sum"], rec["count"], n)
+        want_s = o.strength_from_record(peak, total, count, n)
+    assert np.array_equal(np.isnan(got_s), np.isnan(want_s)), what
+    ok = ~np.isnan(want_s)
+    assert (np.abs(got_s[ok] - want_s[ok]) <= 1e-4 * want_s[ok]).all(), what
+    got_p = rec["probe_re"].astype(np.float64) + 1j * rec["probe_im"]
+    if probe is None or kind != o.COHERENT:
+        assert (got_p == 0).all(), (what, np.flatnonzero(got_p != 0)[:8])
+    else:
+        assert (np.abs(got_p - val) <= MAG_TOL * peak).all(), (what, np.flatnonzero(np.abs(got_p - val) > MAG_TOL * peak)[:8])
+    return len(bad)
+
+
+# ---- gb200_acquire_cells' kernel choice (run_cells) -------------------------------------------------------------------
+FUSED_CELL_LIMIT = 8192  # lists of at most this many cell-milliseconds always take the fused kernel
+
+
+def fused_choice(s, dop, m, profile=False):
+    """run_cells' automatic choice restated: True for the fused block-per-cell kernel, False for doppler_spectra +
+    correlate_cells.  Fused only where it covers the rate (S = 2, 4) and no profile is wanted, and then when more than a
+    quarter of the cells have distinct Dopplers or n_cells * M <= 8192.  Distinct as std::sort + std::unique count them:
+    -0.0 and 0.0 are one value."""
+    n_cells, n_unique = len(dop), len({float(f) for f in dop})
+    return s in FUSED_RATES and not profile and (n_unique * 4 > n_cells or n_cells * m <= FUSED_CELL_LIMIT)
+
+
+def choice_list(case, s, seed):
+    """(PRN entries, Dopplers, M) of a list on one side of one of fused_choice's thresholds, unsorted, with -0.0 and 0.0
+    both in it (one distinct value; counted as two, "unique_at" would cross its threshold):
+      unique_at    4k cells, k distinct Dopplers, n_cells * M > 8192    split
+      unique_past  4k cells, k + 1 distinct                             fused
+      size_at      n_cells * M == 8192, few distinct                    fused
+      size_past    n_cells * M == 8193, few distinct                    split"""
+    rng = np.random.default_rng(seed)
+    n_cells, m, n_unique = {"unique_at": (2732, 3, 683), "unique_past": (2732, 3, 684), "size_at": (8192, 1, 5),
+                            "size_past": (8193, 1, 5)}[case]
+    others = rng.permutation(np.arange(1, 4 * n_unique) * 37.25 - 50000.0)[:n_unique - 1]
+    values = np.concatenate([[-0.0, 0.0], others])
+    dop = np.concatenate([values, rng.choice(values, n_cells - values.size)])[rng.permutation(n_cells)]
+    prns = rng.integers(0, 32, n_cells)
+    return prns, dop, m
+
+
 def assert_records_equal(a, b, what, sum_rtol=0):
     """peak, argmax and count exact; sum exact, or within sum_rtol * max(b's sums) where the two launches add a cell's
     values in a different order."""
