@@ -24,6 +24,7 @@ GB_HD GB_INLINE float2 c_fma_j(float c, float2 x, float2 y) {                   
     return GB_FMA2(make_float2(-x.y, x.x), make_float2(c, c), y);
 }
 GB_HD GB_INLINE float2 c_scale(float c, float2 x) { return GB_MUL2(x, make_float2(c, c)); }                 // c x
+GB_HD GB_INLINE float2 c_scale_j(float c, float2 x) { return GB_MUL2(make_float2(-x.y, x.x), make_float2(c, c)); }  // c (j x)
 // Complex products: a multiply of the rotated operand by the imaginary part, then an fma by the real part.
 // z * w = (fma(zr, wr, -(zi wi)), fma(zi, wr, zr wi))
 GB_HD GB_INLINE float2 cmul(float2 z, float2 w) {

@@ -65,7 +65,8 @@ int pick_rsplit(const gb200_engine* e, int slots, long long n_cells) {
 size_t unit_floats2(const gb200_engine* e, int M) { return static_cast<size_t>(M) * e->s * 2 * kFft; }
 
 // doppler_spectra of n_units (block, Doppler) units, n_doppler per block, blocks of M milliseconds consecutive from iq.
-int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int n_doppler, int n_units) {
+// pfa: for the one-warp correlate kernel (spectra_pfa).
+int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int n_doppler, int n_units, bool pfa) {
     SpectraArgs sa{};
     sa.iq = iq;
     sa.doppler = dop;
@@ -79,6 +80,7 @@ int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int
     sa.M = M;
     sa.n_doppler = n_doppler;
     sa.n_units = n_units;
+    sa.pfa = pfa ? 1 : 0;
     GB_LAUNCH(e, 0, launch_doppler_spectra(sa, e->stream));
     return GB200_OK;
 }
@@ -88,6 +90,7 @@ CorrelateArgs correlate_args(const gb200_engine* e, int M, int kind, int rsplit,
     CorrelateArgs ca{};
     ca.spec = e->spec.p;
     ca.crep = e->crep.p;
+    ca.crep1023 = e->crep1023.p;
     ca.tw1 = e->tw1.p;
     ca.tw2 = e->tw2.p;
     ca.records = records;
@@ -149,7 +152,7 @@ struct ListPlan {
 // dop (spectrum unit u holds dop[u]), then correlate_cells.  probe, gate and profile are optional (see CorrelateArgs).
 int run_list(gb200_engine* e, const ListPlan& plan, const int* dev, int g0, int n_groups, int M, int kind, int rsplit,
              const double* dop, int n_units, CellRecord* records, const int* probe, const double* gate, float* profile) {
-    GB_TRY(run_spectra(e, e->iq, M, dop, n_units, n_units));
+    GB_TRY(run_spectra(e, e->iq, M, dop, n_units, n_units, spectra_pfa(kind, profile != nullptr)));
     CorrelateArgs ca = correlate_args(e, M, kind, rsplit, records, profile);
     plan.bind(ca, dev, g0, n_groups);
     ca.cell_probe = probe;
@@ -237,7 +240,7 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
     for (int b0 = 0; b0 < n_blocks; b0 += nb) {
         const int nbb = std::min(nb, n_blocks - b0);
         const int chunks = (nbb * D + cpg - 1) / cpg;  // groups per PRN: its nbb*D cells in chunks of cpg
-        GB_TRY(run_spectra(e, e->iq + static_cast<size_t>(b0) * M * e->N, M, e->d_doppler.p, D, nbb * D));
+        GB_TRY(run_spectra(e, e->iq + static_cast<size_t>(b0) * M * e->N, M, e->d_doppler.p, D, nbb * D, spectra_pfa(kind, false)));
 
         CorrelateArgs ca = correlate_args(e, M, kind, rsplit, rec_dev + static_cast<size_t>(b0) * P * D, nullptr);
         ca.n_groups = P * chunks;
@@ -474,8 +477,9 @@ int gb200_set_replicas(gb200_engine* e, const uint8_t* chips, int n_prn) {
     GB_CUDA(e, cudaStreamSynchronize(e->stream));
     GB_CUDA(e, e->chips.ensure(static_cast<size_t>(n_prn) * kChips));
     GB_CUDA(e, e->crep.ensure(static_cast<size_t>(n_prn) * 2 * kFft));
+    GB_CUDA(e, e->crep1023.ensure(static_cast<size_t>(n_prn) * kPfaVecF2));
     GB_CUDA(e, cudaMemcpyAsync(e->chips.p, chips, static_cast<size_t>(n_prn) * kChips, cudaMemcpyHostToDevice, e->stream));
-    GB_LAUNCH(e, -1, launch_replica_spectra(e->chips.p, n_prn, e->crep.p, e->stream));
+    GB_LAUNCH(e, -1, launch_replica_spectra(e->chips.p, n_prn, e->crep.p, e->crep1023.p, e->stream));
     GB_CUDA(e, cudaStreamSynchronize(e->stream));
     e->n_prn = n_prn;
     return GB200_OK;
@@ -592,7 +596,7 @@ int gb200_acquire_grid_host(gb200_engine* e, const float* iq_host, int n_blocks,
     auto key = [&] {
         return gb200_engine::HostGraph::Key{n_blocks, M, P, D, kind, {dop, dop + D}, {prn_idx, prn_idx + P},
                                             e->iq_own.p, e->d_records.p, e->h_iq.p, e->h_records.p, e->spec.p,
-                                            e->d_doppler.p, e->d_ints.p, e->crep.p, rec_target, e->stream};
+                                            e->d_doppler.p, e->d_ints.p, e->crep.p, e->crep1023.p, rec_target, e->stream};
     };
     const bool same = g.seen && g.key == key();
     auto enqueue = [&]() -> int {

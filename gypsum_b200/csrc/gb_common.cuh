@@ -20,6 +20,7 @@ namespace gb {
 constexpr int kChips = 1023;   // constants.py:7  PRN_CHIP_COUNT
 constexpr int kFft = 1024;     // one warp-level transform
 constexpr int kPad = 2048;     // zero-padded length carrying a length-1023 circular correlation (>= 2*1023-1)
+constexpr int kPfaVecF2 = 1088;  // one exact DFT-1023 spectrum, pair-interleaved as X[k1, k2] at pidx(k2, k1) (warp_pfa.cuh)
 constexpr int kTStride = 34;   // padded row of the 32x32 transpose tile (float2 units): 16-byte aligned rows, conflict-free
                                // for the 64-bit column writes and the 128-bit row reads
 constexpr int kTileF2 = 32 * kTStride;

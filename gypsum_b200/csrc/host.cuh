@@ -58,7 +58,7 @@ using PinnedBuf = Buf<T, PinnedMemory>;
 struct gb200_engine {
     int device = 0, fs = 0, N = 0, s = 0, num_sms = 132;
     cudaStream_t own_stream = nullptr, stream = nullptr;
-    gb::capi::DevBuf<float2> tw1, tw2, crep, iq_own, spec, d_replica;
+    gb::capi::DevBuf<float2> tw1, tw2, crep, crep1023, iq_own, spec, d_replica;
     gb::capi::DevBuf<uint8_t> chips;
     gb::capi::DevBuf<double> d_doppler;
     gb::capi::DevBuf<int> d_ints;
@@ -103,11 +103,11 @@ struct gb200_engine {
             std::vector<double> dop;
             std::vector<int> prn;
             const void *iq_dev = nullptr, *rec_dev = nullptr, *iq_stage = nullptr, *rec_stage = nullptr, *spec = nullptr;
-            const void *d_dop = nullptr, *d_prn = nullptr, *crep = nullptr;  // what the captured kernels dereference besides the above
+            const void *d_dop = nullptr, *d_prn = nullptr, *crep = nullptr, *crep1023 = nullptr;  // what the captured kernels dereference besides the above
             const void* rec_target = nullptr;  // where the captured correlate kernel stores its records
             cudaStream_t stream = nullptr;
             auto ids() const {
-                return std::tie(n_blocks, M, P, D, kind, iq_dev, rec_dev, iq_stage, rec_stage, spec, d_dop, d_prn, crep, rec_target,
+                return std::tie(n_blocks, M, P, D, kind, iq_dev, rec_dev, iq_stage, rec_stage, spec, d_dop, d_prn, crep, crep1023, rec_target,
                                 stream);
             }
             // the axes compare bit for bit, as the device copies of them do (upload_grid_axes)

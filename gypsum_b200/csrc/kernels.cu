@@ -8,14 +8,22 @@
 //                     memory with a TMA bulk copy), inverse warp FFTs (utils.py:73), |.| accumulation over ms
 //                     (utils.py:102-104) in registers, peak/argmax/sum/count reduction with REDUX / warp shuffles
 //                     (acquisition.py:181-189, utils.py:111-116).  Two kernels, chosen by launch_correlate:
-//                     k_correlate_w2048 (one warp per pruned inverse FFT-2048; every non-coherent, record-only launch)
+//                     k_correlate_pfa (one warp per exact inverse DFT-1023; every non-coherent, record-only launch)
 //                     and k_correlate_cells (a warp pair per transform pair; coherent launches, probes, full profiles).
 //   refine_*          planning / selection kernels of the on-device search (acquisition.py:70-152).
 #include "kernels.cuh"
 #include "ptx_helpers.cuh"
 #include "warp_fft.cuh"
+#include "warp_pfa.cuh"
 
 namespace gb {
+
+__constant__ float c_row31[32][16] = GB_ROW31_COEF;  // staged into shared memory by the kernels that run warp_pfa.cuh
+
+// coef[lane * 16 + k] = c_row31[lane][k], by a whole CTA
+__device__ __forceinline__ void stage_row31(float* coef) {
+    for (int t = threadIdx.x; t < 32 * 16; t += blockDim.x) coef[t] = c_row31[t >> 4][t & 15];
+}
 
 // ---------------------------------------------------------------------------------------------------------
 // One-time setup
@@ -55,6 +63,27 @@ __global__ void __launch_bounds__(128) k_replica_spectra(const uint8_t* chips, f
     crep[(static_cast<size_t>(p) * 2 + (g & 1)) * kFft + zpos(g >> 1)] = make_float2(static_cast<float>(re), static_cast<float>(im));
 }
 
+// crep1023[p][pidx(k2, k1)] = conj(DFT1023(c_p))[pfa_bin(k1, k2)] / 1023 (zero for k1 = 31), direct float64 DFT with an
+// exact-phase table: the replica spectrum of the one-warp kernel, in its permuted bin order.
+__global__ void __launch_bounds__(128) k_replica_spectra1023(const uint8_t* chips, float2* crep1023) {
+    __shared__ double2 cs[kChips];
+    __shared__ uint8_t c[1024];
+    const int p = blockIdx.y;
+    for (int t = threadIdx.x; t < kChips; t += blockDim.x) {
+        double s, co;
+        sincospi(2.0 * t / kChips, &s, &co);
+        cs[t] = make_double2(co, s);
+        c[t] = chips[p * kChips + t];
+    }
+    __syncthreads();
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;  // = pidx(k2, k1)
+    if (t >= kPfaVecF2) return;
+    const int k1 = (t >> 1) & 31, k2 = ((t >> 6) << 1) | (t & 1);
+    double re = 0.0, im = 0.0;
+    if (k1 < 31) replica_spectrum_bin1023(c, pfa_bin(k1, k2), cs, re, im);
+    crep1023[static_cast<size_t>(p) * kPfaVecF2 + t] = make_float2(static_cast<float>(re), static_cast<float>(im));
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // doppler_spectra
 // ---------------------------------------------------------------------------------------------------------
@@ -66,9 +95,10 @@ constexpr int kCarrierTable = 64;  // >= ceil(N / threads) for every supported r
 // When every (branch, parity) task has its own warp (2S <= 8) the transpose tiles take the place of the polyphase rows,
 // which are dead once every warp holds its vector in registers: 35 KB instead of 52 KB per 2.046 Msps CTA.
 __host__ __device__ constexpr bool spec_alias(int s) { return 2 * s <= 8; }
+constexpr int kSpecTileF2 = kPfaTileF2 > kTileF2 ? kPfaTileF2 : kTileF2;  // a warp's tile, either transform
 __host__ __device__ constexpr int spec_f2(int s) {  // float2 of rows + tiles
-    return spec_alias(s) ? (s * kFft > spec_warps(s) * kTileF2 ? s * kFft : spec_warps(s) * kTileF2)
-                         : s * kFft + spec_warps(s) * kTileF2;
+    return spec_alias(s) ? (s * kFft > spec_warps(s) * kSpecTileF2 ? s * kFft : spec_warps(s) * kSpecTileF2)
+                         : s * kFft + spec_warps(s) * kSpecTileF2;
 }
 
 // 2.046 Msps: a register cap of four CTAs per SM (128 registers).  The cap of five (96 registers) spilled 216 B per thread, and
@@ -79,8 +109,9 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_
     constexpr int kSpecThreads = kSpecWarps * 32;
     extern __shared__ __align__(16) float2 smem[];
     float2* ypoly = smem;                                       // [S][1024], rows in zpos() order
-    float2* tiles = spec_alias(S) ? smem : smem + S * kFft;     // [kSpecWarps][kTileF2]
+    float2* tiles = spec_alias(S) ? smem : smem + S * kFft;     // [kSpecWarps][kSpecTileF2]
     float2* coarse = smem + spec_f2(S);                         // [kCarrierTable] carrier at samples 0, T, 2T, ... (T threads)
+    float* coef = reinterpret_cast<float*>(coarse + kCarrierTable);  // [32][16] spread-row coefficients (a.pfa)
 
     const int unit = blockIdx.x / a.M, i = blockIdx.x % a.M;
     const int b = unit / a.n_doppler, d = unit % a.n_doppler;
@@ -107,6 +138,7 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_
         v[k] = n < kChips * S ? src[n] : make_float2(0.f, 0.f);
     }
     if (tid < kIter) coarse[tid] = carrier_at(f, static_cast<double>(tid * kSpecThreads + i * a.N), a.inv_fs);
+    if (a.pfa) stage_row31(coef);
     const float2 fine = carrier_at(f, static_cast<double>(tid), a.inv_fs);
     __syncthreads();
     // wipe-off; de-interleave by polyphase branch
@@ -138,8 +170,30 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_
     __syncthreads();
 
     const int warp = tid >> 5, lane = tid & 31;
-    float2* tile = tiles + warp * kTileF2;
+    float2* tile = tiles + warp * kSpecTileF2;
     float2* __restrict__ dst0 = a.spec + (static_cast<size_t>(unit) * a.M + i) * S * 2 * kFft;
+    if (a.pfa) {
+        // one task per branch: DFT1023(z_r) in the permuted bin order of warp_pfa.cuh, in the first of the branch's two slots
+        for (int r0 = 0; r0 < S; r0 += kSpecWarps) {
+            const int r = r0 + warp;
+            float2 y[31], e;
+            if (r < S) pfa_fwd_gather(y, e, lane, ypoly + r * kFft);
+            if (spec_alias(S)) __syncthreads();  // every warp runs the same rounds; the rows are dead, the tiles may take their place
+            if (r < S) {
+                pfa_fwd_phase1(e, lane, tile);
+                __syncwarp();
+                pfa_fwd_phase2(y, lane, tile);
+                __syncwarp();
+                pfa_fwd_phase3(lane, tile, coef);
+                __syncwarp();
+                pfa_fwd_phase4(y, lane, tile);
+                __syncwarp();
+                pfa_fwd_phase5(lane, tile, dst0 + static_cast<size_t>(r) * 2 * kFft);
+                __syncwarp();
+            }
+        }
+        return;
+    }
     for (int task = warp; task < 2 * S; task += kSpecWarps) {
         const int r = task >> 1, half = task & 1;
         float2 x[32];
@@ -200,12 +254,13 @@ __device__ __forceinline__ GroupCell decode_group(const CorrelateArgs& a, int g,
 
 // Stages conj(FFT(replica)) of a new PRN into crep_s with a TMA bulk copy once every warp is done with the previous one, then
 // de-phases the warps by stagger_ns: warps that restart in step after the CTA-wide barrier convoy on the shared-memory pipe.
-__device__ __forceinline__ void stage_replica(const CorrelateArgs& a, int prn, float2* crep_s, uint64_t* mbar, uint32_t& parity,
+// crep holds one spectrum of n_f2 float2 per PRN.
+__device__ __forceinline__ void stage_replica(const float2* crep, int n_f2, int prn, float2* crep_s, uint64_t* mbar, uint32_t& parity,
                                               unsigned stagger_ns) {
     __syncthreads();
     if (threadIdx.x == 0) {
-        mbar_expect_tx(mbar, 2 * kFft * sizeof(float2));
-        bulk_g2s(crep_s, a.crep + static_cast<size_t>(prn) * 2 * kFft, 2 * kFft * sizeof(float2), mbar);
+        mbar_expect_tx(mbar, n_f2 * sizeof(float2));
+        bulk_g2s(crep_s, crep + static_cast<size_t>(prn) * n_f2, n_f2 * sizeof(float2), mbar);
     }
     mbar_wait(mbar, parity);
     parity ^= 1;
@@ -263,7 +318,7 @@ __global__ void __launch_bounds__(kPairs * 64, 1) k_correlate_cells(const Correl
         const bool active = gc.active;
         const int unit = gc.unit, out = gc.out;
         if (gc.prn != cur_prn) {
-            stage_replica(a, gc.prn, crep_s, mbar, parity, pair * 300);
+            stage_replica(a.crep, 2 * kFft, gc.prn, crep_s, mbar, parity, pair * 300);
             cur_prn = gc.prn;
         }
 
@@ -369,35 +424,25 @@ __global__ void __launch_bounds__(kPairs * 64, 1) k_correlate_cells(const Correl
 
 // ---------------------------------------------------------------------------------------------------------
 // correlate_cells, one warp per transform (non-coherent searches).  Same cell / group bookkeeping as above, but a
-// single warp owns a whole (cell, polyphase branch): it loads both half-spectra, multiplies by the replica spectrum
-// and runs the pruned inverse FFT-2048 of warp_fft.cuh (two FFT-32, 64x32 transpose, one FFT-64 per thread).  Per
-// transform pair this moves 40 KB through the shared-memory pipe instead of 52 KB and needs no partner warp: no
-// exchange tile, no pair barriers, no recombination twiddles, half the twiddle-table reads.
+// single warp owns a whole (cell, polyphase branch): it loads the branch's spectrum DFT1023(z_r) (permuted bin order, see
+// warp_pfa.cuh), multiplies by the replica spectrum and runs the exact inverse DFT-1023 of warp_pfa.cuh (one DFT-33 column per
+// lane, a 33x33 transpose, one DFT-31 row per lane and the 33rd row spread over the warp).  No partner warp, no twiddles.
 // ---------------------------------------------------------------------------------------------------------
 template <int NW, bool SINGLE_MS>
-__global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateArgs a) {
+__global__ void __launch_bounds__(NW * 32, 1) k_correlate_pfa(const CorrelateArgs a) {
     extern __shared__ __align__(16) float2 smem[];
-    constexpr int kCrepOdd = kFft;
-    float2* crep_s = smem;              // [2][1024]
-    float2* tw1_s = crep_s + 2 * kFft;  // [32][32]
-    float2* tw1o_s = tw1_s + kFft;      // [16][32] odd-parity products, k1 >= 16
-    float2* tiles = tw1o_s + kFft / 2;  // [NW][kTile64F2]
-    PeakPartial* partial = reinterpret_cast<PeakPartial*>(tiles + NW * kTile64F2);  // [NW]
+    float2* crep_s = smem;                                   // [kPfaVecF2]
+    float* coef = reinterpret_cast<float*>(crep_s + kPfaVecF2);  // [32][16]
+    float2* tiles = crep_s + kPfaVecF2 + 256;                // [NW][kPfaTileF2]
+    PeakPartial* partial = reinterpret_cast<PeakPartial*>(tiles + NW * kPfaTileF2);  // [NW]
     uint64_t* mbar = reinterpret_cast<uint64_t*>(partial + NW);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    float2* tile = tiles + warp * kTile64F2;
+    float2* tile = tiles + warp * kPfaTileF2;
 
     uint32_t parity = 0;
     if (threadIdx.x == 0) mbar_init(mbar, 1);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(mbar, kFft * sizeof(float2));
-        bulk_g2s(tw1_s, a.tw1, kFft * sizeof(float2), mbar);
-    }
-    mbar_wait(mbar, parity);
-    parity ^= 1;
-    if (warp == 0) w2048_odd_twiddles(lane, tw1_s, tw1o_s);
+    stage_row31(coef);
     __syncthreads();
     asm volatile("griddepcontrol.wait;" ::: "memory");  // PDL against doppler_spectra, see launch_correlate
 
@@ -445,7 +490,7 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
         const bool active = gc.active;
         const int unit = gc.unit, out = gc.out;
         if (gc.prn != cur_prn) {
-            stage_replica(a, gc.prn, crep_s, mbar, parity, (warp >> 2) * a.stag_a + (warp & 3) * a.stag_b);
+            stage_replica(a.crep1023, kPfaVecF2, gc.prn, crep_s, mbar, parity, (warp >> 2) * a.stag_a + (warp & 3) * a.stag_b);
             cur_prn = gc.prn;
         }
 
@@ -460,33 +505,32 @@ __global__ void __launch_bounds__(NW * 32, 1) k_correlate_w2048(const CorrelateA
                 const int n_iter = SINGLE_MS ? 1 : a.M;
                 for (int it = 0; it < n_iter; ++it) {
                     const float2* __restrict__ p = spec_u + static_cast<size_t>(it * a.s + r) * 2 * kFft;
+                    float2 y[31];
                     {
-                        float2 hx[32];
-                        load_mul_vec(hx, lane, p, crep_s);  // even bins
-                        w2048_phase1<0>(hx, lane, tw1_s, tile);
-                    }
-                    {
-                        float2 hx[32];
-                        load_mul_vec(hx, lane, p + kFft, crep_s + kFft);  // odd bins
-                        w2048_phase1_odd(hx, lane, tw1_s, tw1o_s, tile);
+                        float2 x[33];
+                        pfa_load_mul(x, lane, p, crep_s);
+                        pfa_inv_phase1(x, lane, tile);
                     }
                     __syncwarp();
-                    float2 x[64];
-                    w2048_phase2(x, lane, tile);
+                    pfa_inv_phase2(y, lane, tile);
+                    __syncwarp();
+                    pfa_inv_phase3(y, lane, tile, coef);
+                    __syncwarp();
+                    const float2 e = pfa_inv_phase4(lane, tile);
                     __syncwarp();  // the tile may be overwritten by the next transform
 #pragma unroll
-                    for (int k = 0; k < 32; ++k) {
-                        if (SINGLE_MS) acc[k] = gb_mag(x[k]);  // = 0 + |x|: magnitudes are never -0
-                        else acc[k] += gb_mag(x[k]);
+                    for (int k = 0; k < 31; ++k) {
+                        if (SINGLE_MS) acc[k] = gb_mag(y[k]);  // = 0 + |x|: magnitudes are never -0
+                        else acc[k] += gb_mag(y[k]);
                     }
+                    if (SINGLE_MS) acc[31] = gb_mag(e);
+                    else acc[31] += gb_mag(e);
                 }
-                // lags q = lane + 32 k; the two float sums are added in the order of thread_peak16's halves
                 Peak t;
-                float fsum[2];
-                thread_peak32(acc, lane, a.s, r, t, fsum);
-                t.sum = static_cast<double>(fsum[0]);
+                float fsum;
+                thread_peak_pfa(acc, lane, a.s, r, t, fsum);
+                t.sum = static_cast<double>(fsum);
                 peak_merge(pk, t);
-                pk.sum += static_cast<double>(fsum[1]);
             }
             warp_reduce_peak(pk);
             if (lane == 0) {
@@ -694,15 +738,14 @@ cudaError_t launch_refine_finalize(int n_sv, const RefineState* st, const CellRe
 // launch wrappers
 // ---------------------------------------------------------------------------------------------------------
 size_t spectra_smem_bytes(int s) {
-    return (static_cast<size_t>(spec_f2(s)) + kCarrierTable) * sizeof(float2);
+    return (static_cast<size_t>(spec_f2(s)) + kCarrierTable + 256) * sizeof(float2);
 }
 size_t correlate_smem_bytes() {
     return (4 * static_cast<size_t>(kFft) + 2 * kPairs * kTileF2) * sizeof(float2) + 2 * kPairs * sizeof(PeakPartial) + 16;
 }
 
-size_t correlate_w2048_smem_bytes(int nw) {
-    return (3 * static_cast<size_t>(kFft) + kFft / 2 + static_cast<size_t>(nw) * kTile64F2) * sizeof(float2) +
-           nw * sizeof(PeakPartial) + 16;
+size_t correlate_pfa_smem_bytes(int nw) {
+    return (kPfaVecF2 + 256 + static_cast<size_t>(nw) * kPfaTileF2) * sizeof(float2) + nw * sizeof(PeakPartial) + 16;
 }
 
 bool spectra_supports(int s) {
@@ -728,19 +771,20 @@ cudaError_t configure_kernels() {
     if ((e = cudaFuncSetAttribute(k_correlate_cells<kKindCoherent, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm))) return e;
     if ((e = cudaFuncSetAttribute(k_correlate_cells<kKindCoherent, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm))) return e;
     if ((e = cudaFuncSetAttribute(k_correlate_cells<kKindNonCoherent, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm))) return e;
-    if ((e = cudaFuncSetAttribute(k_correlate_w2048<12, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(correlate_w2048_smem_bytes(12)))) != cudaSuccess)
+    if ((e = cudaFuncSetAttribute(k_correlate_pfa<12, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(correlate_pfa_smem_bytes(12)))) != cudaSuccess)
         return e;
-    return cudaFuncSetAttribute(k_correlate_w2048<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                static_cast<int>(correlate_w2048_smem_bytes(8)));
+    return cudaFuncSetAttribute(k_correlate_pfa<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                static_cast<int>(correlate_pfa_smem_bytes(8)));
 }
 
 cudaError_t launch_init_tables(float2* tw1, float2* tw2, cudaStream_t st) {
     k_init_tables<<<4, 256, 0, st>>>(tw1, tw2);
     return cudaGetLastError();
 }
-cudaError_t launch_replica_spectra(const uint8_t* chips_dev, int n_prn, float2* crep, cudaStream_t st) {
+cudaError_t launch_replica_spectra(const uint8_t* chips_dev, int n_prn, float2* crep, float2* crep1023, cudaStream_t st) {
     k_replica_spectra<<<dim3(kPad / 128, n_prn), 128, 0, st>>>(chips_dev, crep);
+    k_replica_spectra1023<<<dim3((kPfaVecF2 + 127) / 128, n_prn), 128, 0, st>>>(chips_dev, crep1023);
     return cudaGetLastError();
 }
 cudaError_t launch_doppler_spectra(const SpectraArgs& a, cudaStream_t st) {
@@ -756,11 +800,12 @@ cudaError_t launch_doppler_spectra(const SpectraArgs& a, cudaStream_t st) {
 }
 
 // Start stagger of the one-warp kernel's warps after each replica re-stage, in ns: (warp / 4) * row + (warp % 4) * column.
-constexpr int kW2048StaggerRowNs = 600, kW2048StaggerColNs = 150;
+constexpr int kPfaStaggerRowNs = 600, kPfaStaggerColNs = 150;
 
 // Coherent launches, coherent probes and full profiles need the pair kernel; every other launch takes the one-warp kernel,
 // which is faster on every record-only shape measured on the H100 (DESIGN.md §4).
 static bool pair_kernel(int kind, bool profile) { return kind == kKindCoherent || profile; }
+bool spectra_pfa(int kind, bool profile) { return !pair_kernel(kind, profile); }
 
 int correlate_slots(int kind, int M, bool profile) {
     if (pair_kernel(kind, profile)) return kPairs;
@@ -769,7 +814,7 @@ int correlate_slots(int kind, int M, bool profile) {
 
 // Launch as a programmatic dependent of the previous kernel in the stream (doppler_spectra): the grid may start its
 // prologue while the producer drains; it blocks at griddepcontrol.wait until the producer's writes are visible.  Only
-// k_correlate_w2048 executes that wait, so only it may be launched this way.
+// k_correlate_pfa executes that wait, so only it may be launched this way.
 template <class K>
 static void launch_dependent(K kernel, const CorrelateArgs& a, int grid, int block, size_t sm, cudaStream_t st) {
     cudaLaunchConfig_t cfg{};
@@ -794,10 +839,10 @@ cudaError_t launch_correlate(const CorrelateArgs& a0, int grid, cudaStream_t st)
         return cudaGetLastError();
     }
     CorrelateArgs a = a0;
-    a.stag_a = kW2048StaggerRowNs;
-    a.stag_b = kW2048StaggerColNs;
-    if (a.M == 1) launch_dependent(k_correlate_w2048<12, true>, a, grid, 12 * 32, correlate_w2048_smem_bytes(12), st);
-    else launch_dependent(k_correlate_w2048<8, false>, a, grid, 8 * 32, correlate_w2048_smem_bytes(8), st);
+    a.stag_a = kPfaStaggerRowNs;
+    a.stag_b = kPfaStaggerColNs;
+    if (a.M == 1) launch_dependent(k_correlate_pfa<12, true>, a, grid, 12 * 32, correlate_pfa_smem_bytes(12), st);
+    else launch_dependent(k_correlate_pfa<8, false>, a, grid, 8 * 32, correlate_pfa_smem_bytes(8), st);
     return cudaGetLastError();
 }
 

@@ -16,15 +16,17 @@ struct SpectraArgs {
     const float2* tw1;       // [32][32]  exp(-2 pi i lane k1 / 1024)
     const float2* tw2;       // [1024]    exp(-2 pi i n / 2048)
     long long block_stride;  // samples between consecutive blocks (= M*N)
+    int pfa;                 // spectra for k_correlate_pfa: DFT1023(z_r) per branch r (warp_pfa.cuh order) in [r][0]; else both halves
     double inv_fs;
     int N, s, M, n_doppler, n_units;  // n_units = n_blocks * n_doppler
 };
 
-// correlate_cells: one warp (k_correlate_w2048) or warp pair (k_correlate_cells) per (cell, r-range); every slot of a CTA
+// correlate_cells: one warp (k_correlate_pfa) or warp pair (k_correlate_cells) per (cell, r-range); every slot of a CTA
 // works on the same PRN.
 struct CorrelateArgs {
     const float2* spec;
     const float2* crep;  // [n_prn][2][1024]  conj(FFT2048(c'))/2048, even / odd bins
+    const float2* crep1023;  // [n_prn][kPfaVecF2]  conj(DFT1023(c))/1023 in warp_pfa.cuh's bin order (k_correlate_pfa)
     const float2* tw1;   // [32][32]
     const float2* tw2;   // [1024]
     CellRecord* records;
@@ -34,7 +36,7 @@ struct CorrelateArgs {
     int n_groups;
     // grid mode (cells = blocks x prn list x doppler list)
     int grid_mode, P, D, n_blocks, chunks;  // chunks = ceil(n_blocks * D / cells_per_group): groups per PRN
-    int win_chunks;  // k_correlate_w2048, grid mode: chunks per L2 window (0 = the whole batch is one window), see the kernel
+    int win_chunks;  // k_correlate_pfa, grid mode: chunks per L2 window (0 = the whole batch is one window), see the kernel
     const int* prn_idx;           // [P]
     // list mode (cells sorted by PRN)
     const int* grp_first;
@@ -43,7 +45,7 @@ struct CorrelateArgs {
     const int* cell_u;      // spectrum unit of each sorted cell
     const int* cell_out;    // where its record goes
     const int* cell_probe;  // coherent probe index or -1 (both modes, indexed by output slot; may be null)
-    int stag_a, stag_b;       // k_correlate_w2048 start stagger in ns: (warp / 4) * stag_a + (warp % 4) * stag_b (set by launch_correlate)
+    int stag_a, stag_b;       // k_correlate_pfa start stagger in ns: (warp / 4) * stag_a + (warp % 4) * stag_b (set by launch_correlate)
     const double* cell_gate;  // optional, indexed by output slot: NaN = this cell is switched off (device-planned lists)
 };
 
@@ -228,11 +230,13 @@ cudaError_t launch_decode_subframes(const NavArgs& a, cudaStream_t st);
 size_t spectra_smem_bytes(int s);
 bool spectra_supports(int s);
 cudaError_t launch_init_tables(float2* tw1, float2* tw2, cudaStream_t st);
-cudaError_t launch_replica_spectra(const uint8_t* chips_dev, int n_prn, float2* crep, cudaStream_t st);
+cudaError_t launch_replica_spectra(const uint8_t* chips_dev, int n_prn, float2* crep, float2* crep1023, cudaStream_t st);
 cudaError_t launch_doppler_spectra(const SpectraArgs& a, cudaStream_t st);
 // Slots per CTA of the correlate kernel that runs a launch of this kind, M milliseconds and profile output: warps of the
 // one-warp-per-transform kernel, or warp pairs of the pair kernel.  rsplit must divide it.
 int correlate_slots(int kind, int M, bool profile);
+// Whether the correlate launch of (kind, profile) reads spectra made with SpectraArgs::pfa.
+bool spectra_pfa(int kind, bool profile);
 // Runs the kernel correlate_slots(a.kind, a.M, a.profile != nullptr) describes.
 cudaError_t launch_correlate(const CorrelateArgs& a, int grid, cudaStream_t st);
 cudaError_t launch_correlate_generic(const float2* iq, const float2* replica, int N, int n_ms, double doppler, double inv_fs,
