@@ -49,6 +49,10 @@ SYMBOLS = {
     "gb200_acquire_grid_host": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, _P]),
     "gb200_acquire_grid_best": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, _P]),
     "gb200_acquire_grid_best_device": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, _P]),
+    "gb200_acquire_grid_semicoherent": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
+    "gb200_acquire_grid_semicoherent_device": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
+    "gb200_acquire_grid_semicoherent_best": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
+    "gb200_acquire_grid_semicoherent_best_device": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
     "gb200_ring_create": (C.c_int, [_P, C.c_int, C.POINTER(_P)]),
     "gb200_ring_destroy": (C.c_int, [_P]),
     "gb200_ring_append": (C.c_int, [_P, _P, C.c_int]),
@@ -299,6 +303,50 @@ class Engine:
             self._lib.gb200_acquire_grid_device(self._h, n_blocks, ms_per_block, _ptr(prn), prn.size, _ptr(dop), dop.size,
                                                 kind, _P(out_device_ptr)),
             "gb200_acquire_grid_device",
+        )
+
+    def acquire_grid_semicoherent(self, n_blocks: int, ms_per_block: int, coherent_ms: int, prn_idx, doppler_hz,
+                                  out: np.ndarray | None = None) -> np.ndarray:
+        """Semi-coherent grid (gb200_acquire_grid_semicoherent): per cell the profile sum_k |coherent sum of milliseconds
+        k*coherent_ms .. (k+1)*coherent_ms - 1|, reduced to RECORD_DTYPE [n_blocks, n_prn, n_doppler]."""
+        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
+        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
+        out = _records_out(out, (n_blocks, prn.size, dop.size))
+        self._check(
+            self._lib.gb200_acquire_grid_semicoherent(self._h, n_blocks, ms_per_block, coherent_ms, _ptr(prn), prn.size,
+                                                      _ptr(dop), dop.size, _ptr(out)),
+            "gb200_acquire_grid_semicoherent",
+        )
+        return out
+
+    def acquire_grid_semicoherent_device(self, n_blocks, ms_per_block, coherent_ms, prn: np.ndarray, dop: np.ndarray,
+                                         out_device_ptr: int):
+        """prn (int32) / dop (float64) must be contiguous arrays kept alive by the caller; enqueue only."""
+        self._check(
+            self._lib.gb200_acquire_grid_semicoherent_device(self._h, n_blocks, ms_per_block, coherent_ms, _ptr(prn), prn.size,
+                                                             _ptr(dop), dop.size, _P(out_device_ptr)),
+            "gb200_acquire_grid_semicoherent_device",
+        )
+
+    def acquire_grid_semicoherent_best(self, n_blocks: int, ms_per_block: int, coherent_ms: int, prn_idx,
+                                       doppler_hz) -> np.ndarray:
+        """The semi-coherent grid's best bin per (block, prn) row: BEST_DTYPE [n_blocks, n_prn]."""
+        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
+        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
+        out = np.empty((n_blocks, prn.size), dtype=BEST_DTYPE)
+        self._check(
+            self._lib.gb200_acquire_grid_semicoherent_best(self._h, n_blocks, ms_per_block, coherent_ms, _ptr(prn), prn.size,
+                                                           _ptr(dop), dop.size, _ptr(out)),
+            "gb200_acquire_grid_semicoherent_best",
+        )
+        return out
+
+    def acquire_grid_semicoherent_best_device(self, n_blocks, ms_per_block, coherent_ms, prn: np.ndarray, dop: np.ndarray,
+                                              out_device_ptr: int):
+        self._check(
+            self._lib.gb200_acquire_grid_semicoherent_best_device(self._h, n_blocks, ms_per_block, coherent_ms, _ptr(prn),
+                                                                  prn.size, _ptr(dop), dop.size, _P(out_device_ptr)),
+            "gb200_acquire_grid_semicoherent_best_device",
         )
 
     def acquire_cells(self, prn_idx, doppler_hz, n_ms: int, kind: int = NON_COHERENT, probe_idx=None) -> np.ndarray:

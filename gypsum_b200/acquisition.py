@@ -142,6 +142,42 @@ class GpsSatelliteDetector:
             for i, (sid, k) in enumerate(zip(satellite_ids, kept))
         ]
 
+    def acquire_weak_satellites(self, satellite_ids, antenna_data, stream_attributes, coherent_ms: int,
+                                doppler_spread: float = 7000.0, doppler_step: float | None = None
+                                ) -> list[SatelliteAcquisitionAttemptResult]:
+        """Semi-coherent acquisition for satellites too weak for the reference's search: over the whole window (uploaded
+        samples or a DeviceSampleRing window, a whole number of coherent_ms-ms segments), every satellite's profile
+        sum_k |coherent sum of segment k| on the Doppler bins arange(-spread, spread + step / 2, step), step 500 /
+        coherent_ms Hz by default, in one gb200_acquire_grid_semicoherent_best call.  Then one coherent integration of
+        the first coherent_ms milliseconds at each satellite's best bin gives the carrier phase at its code phase.
+
+        One result per satellite, NOT thresholded: the reference's strength threshold was set for its own statistic.
+        Keep coherent_ms within a navigation data bit (20 ms): a bit edge inside a segment cancels part of it."""
+        if isinstance(coherent_ms, bool) or int(coherent_ms) != coherent_ms or coherent_ms < 1:
+            raise ValueError(f"coherent_ms must be a positive whole number of milliseconds (got {coherent_ms!r})")
+        coherent_ms = int(coherent_ms)
+        spread = float(doppler_spread)
+        step = 500.0 / coherent_ms if doppler_step is None else float(doppler_step)
+        if not (np.isfinite(spread) and spread >= 0.0):
+            raise ValueError(f"doppler_spread must be finite and >= 0 (got {doppler_spread!r})")
+        if not (np.isfinite(step) and step > 0.0):
+            raise ValueError(f"doppler_step must be finite and > 0 (got {doppler_step!r})")
+        if not satellite_ids:
+            return []
+        satellite_ids = list(satellite_ids)
+        eng, prn_idx, n, n_ms = self._prepare(satellite_ids, antenna_data, stream_attributes)
+        bins = np.arange(-spread, spread + step / 2, step)
+        best = eng.acquire_grid_semicoherent_best(1, n_ms, coherent_ms, prn_idx, bins)[0]
+        rec = eng.acquire_cells(prn_idx, best["doppler"], coherent_ms, _native.COHERENT, probe_idx=best["code_phase"])
+        phase = np.angle(rec["probe_re"].astype(np.float64) + 1j * rec["probe_im"].astype(np.float64))
+        return [
+            SatelliteAcquisitionAttemptResult(
+                satellite_id=sid, doppler_shift=float(best["doppler"][i]), carrier_wave_phase_shift=float(phase[i]),
+                prn_phase_shift=int(best["code_phase"][i]), correlation_strength=float(best["strength"][i]),
+            )
+            for i, sid in enumerate(satellite_ids)
+        ]
+
     # -- the reference's methods ---------------------------------------------------------------------------------
     def detect_satellites_in_antenna_data(self, satellites_to_search_for, antenna_data, stream_attributes):
         """acquisition.py:52-68."""

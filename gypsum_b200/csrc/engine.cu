@@ -65,8 +65,9 @@ int pick_rsplit(const gb200_engine* e, int slots, long long n_cells) {
 size_t unit_floats2(const gb200_engine* e, int M) { return static_cast<size_t>(M) * e->s * 2 * kFft; }
 
 // doppler_spectra of n_units (block, Doppler) units, n_doppler per block, blocks of M milliseconds consecutive from iq.
-// pfa: for the one-warp correlate kernel (spectra_pfa).
-int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int n_doppler, int n_units, bool pfa) {
+// pfa: for the one-warp correlate kernel (spectra_pfa).  T > 1: one spectrum per segment of T milliseconds (M / T per unit,
+// T divides M) instead of one per millisecond.
+int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int n_doppler, int n_units, bool pfa, int T = 1) {
     SpectraArgs sa{};
     sa.iq = iq;
     sa.doppler = dop;
@@ -77,7 +78,8 @@ int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int
     sa.inv_fs = 1.0 / static_cast<double>(e->fs);
     sa.N = e->N;
     sa.s = e->s;
-    sa.M = M;
+    sa.M = M / T;
+    sa.T = T;
     sa.n_doppler = n_doppler;
     sa.n_units = n_units;
     sa.pfa = pfa ? 1 : 0;
@@ -181,6 +183,14 @@ int check_grid(gb200_engine* e, int n_blocks, int P, int D, const int32_t* prn_i
     return check_dopplers(e, dop, D);
 }
 
+// A semi-coherent grid sums coherent_ms milliseconds at a time, and every block is a whole number of such segments.
+int check_segments(gb200_engine* e, int ms_per_block, int coherent_ms) {
+    if (coherent_ms < 1) GB_FAIL(e, GB200_EINVAL, "coherent_ms must be at least 1 (got %d)", coherent_ms);
+    if (ms_per_block % coherent_ms != 0)
+        GB_FAIL(e, GB200_EINVAL, "ms_per_block (%d) is not a whole number of %d-ms coherent segments", ms_per_block, coherent_ms);
+    return GB200_OK;
+}
+
 // What every acquisition needs before its own arguments are looked at.
 int check_common(gb200_engine* e, int n_ms, int kind) {
     GB_TRY(check_kind(e, kind));
@@ -218,9 +228,10 @@ int upload_grid_axes(gb200_engine* e, const int32_t* prn_idx, int P, const doubl
 }
 
 // grid mode: all cells of n_blocks x prn list x doppler list; records written to rec_dev (device).  The caller has applied
-// check_grid.
+// check_grid.  T > 1 (non-coherent kind, check_segments applied): a semi-coherent grid, whose correlate launch is the
+// non-coherent one over the M / T segment spectra of each unit.
 int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D, int kind,
-             CellRecord* rec_dev) {
+             CellRecord* rec_dev, int T = 1) {
     GB_TRY(check_common(e, M, kind));
     if (static_cast<int64_t>(n_blocks) * M * e->N > e->iq_samples)
         GB_FAIL(e, GB200_EINVAL, "grid needs %lld samples, %lld loaded", static_cast<long long>(n_blocks) * M * e->N,
@@ -228,21 +239,23 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
     GB_TRY(check_prns(e, prn_idx, P));
     GB_TRY(upload_grid_axes(e, prn_idx, P, dop, D));
 
-    const size_t unit = unit_floats2(e, M);
+    const int K = M / T;  // spectra per unit
+    const size_t unit = unit_floats2(e, K);
     const size_t per_block = unit * D;
     int nb = static_cast<int>(std::max<size_t>(1, e->spec_budget_bytes / (per_block * sizeof(float2))));
     nb = std::min(nb, n_blocks);
     GB_CUDA(e, e->spec.ensure(per_block * nb));
 
-    const int slots = correlate_slots(kind, M, false);
+    const int slots = correlate_slots(kind, K, false);
     const int rsplit = pick_rsplit(e, slots, static_cast<long long>(nb) * P * D);
     const int cpg = slots / rsplit;
     for (int b0 = 0; b0 < n_blocks; b0 += nb) {
         const int nbb = std::min(nb, n_blocks - b0);
         const int chunks = (nbb * D + cpg - 1) / cpg;  // groups per PRN: its nbb*D cells in chunks of cpg
-        GB_TRY(run_spectra(e, e->iq + static_cast<size_t>(b0) * M * e->N, M, e->d_doppler.p, D, nbb * D, spectra_pfa(kind, false)));
+        GB_TRY(run_spectra(e, e->iq + static_cast<size_t>(b0) * M * e->N, M, e->d_doppler.p, D, nbb * D, spectra_pfa(kind, false),
+                           T));
 
-        CorrelateArgs ca = correlate_args(e, M, kind, rsplit, rec_dev + static_cast<size_t>(b0) * P * D, nullptr);
+        CorrelateArgs ca = correlate_args(e, K, kind, rsplit, rec_dev + static_cast<size_t>(b0) * P * D, nullptr);
         ca.n_groups = P * chunks;
         ca.grid_mode = 1;
         ca.P = P;
@@ -369,11 +382,11 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
 }
 
 // The grid's records into d_records, after check_grid; with best, then each (block, PRN) row's best bin into best
-// (acquisition.py:179-189 on the device).
+// (acquisition.py:179-189 on the device).  T as for run_grid.
 int grid_records(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D, int kind,
-                 BestRecord* best) {
+                 BestRecord* best, int T = 1) {
     GB_CUDA(e, e->d_records.ensure(static_cast<size_t>(n_blocks) * P * D));
-    GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p));
+    GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p, T));
     if (best) GB_LAUNCH(e, -1, launch_best_bins(n_blocks * P, D, e->N, e->d_records.p, e->d_doppler.p, best, e->stream));
     return GB200_OK;
 }
@@ -549,6 +562,56 @@ int gb200_acquire_grid_best(gb200_engine* e, int n_blocks, int M, const int32_t*
     GB_CUDA(e, e->d_best.ensure(n));
     GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_best.p));
     return download(e, reinterpret_cast<BestRecord*>(out_host), e->d_best.p, n, e->h_best);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// semi-coherent grids: the non-coherent sum of |coherent sum of coherent_ms milliseconds|.  coherent_ms == 1 is the
+// non-coherent grid itself (the same kernels, launched the same way).
+// ---------------------------------------------------------------------------------------------------------
+int gb200_acquire_grid_semicoherent(gb200_engine* e, int n_blocks, int M, int coherent_ms, const int32_t* prn_idx, int P,
+                                    const double* dop, int D, gb200_cell_record* out_host) {
+    if (!e) return GB200_EINVAL;
+    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
+    GB_CUDA(e, cudaSetDevice(e->device));
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
+    GB_TRY(check_segments(e, M, coherent_ms));
+    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, nullptr, coherent_ms));
+    return fetch_records(e, static_cast<size_t>(n_blocks) * P * D, out_host);
+}
+
+int gb200_acquire_grid_semicoherent_device(gb200_engine* e, int n_blocks, int M, int coherent_ms, const int32_t* prn_idx, int P,
+                                           const double* dop, int D, void* out_device) {
+    if (!e) return GB200_EINVAL;
+    if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
+    GB_CUDA(e, cudaSetDevice(e->device));
+    GB_TRY(check_common(e, M, GB200_NON_COHERENT));
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
+    GB_TRY(check_segments(e, M, coherent_ms));
+    return run_grid(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, static_cast<CellRecord*>(out_device), coherent_ms);
+}
+
+int gb200_acquire_grid_semicoherent_best(gb200_engine* e, int n_blocks, int M, int coherent_ms, const int32_t* prn_idx, int P,
+                                         const double* dop, int D, gb200_best_record* out_host) {
+    if (!e) return GB200_EINVAL;
+    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
+    GB_CUDA(e, cudaSetDevice(e->device));
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
+    GB_TRY(check_segments(e, M, coherent_ms));
+    const size_t n = static_cast<size_t>(n_blocks) * P;
+    GB_CUDA(e, e->d_best.ensure(n));
+    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, e->d_best.p, coherent_ms));
+    return download(e, reinterpret_cast<BestRecord*>(out_host), e->d_best.p, n, e->h_best);
+}
+
+int gb200_acquire_grid_semicoherent_best_device(gb200_engine* e, int n_blocks, int M, int coherent_ms, const int32_t* prn_idx,
+                                                int P, const double* dop, int D, void* out_device) {
+    if (!e) return GB200_EINVAL;
+    if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
+    GB_CUDA(e, cudaSetDevice(e->device));
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
+    GB_TRY(check_segments(e, M, coherent_ms));
+    return grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, static_cast<BestRecord*>(out_device),
+                        coherent_ms);
 }
 
 // Host to host in one call.  The first call of a shape runs eagerly (it may have to upload the axes and grow buffers,

@@ -4,6 +4,8 @@
 //   doppler_spectra   per (Doppler, ms): carrier wipe-off (utils.py:93-97), polyphase boxcar, forward warp FFTs.
 //                     This half of utils.py:65 does not depend on the PRN, so it is computed once per Doppler
 //                     bin and shared by all PRNs instead of being redone per cell as the reference does.
+//                     segment_spectra is the same per (Doppler, segment of T ms) of a semi-coherent grid: the T
+//                     wiped-off milliseconds are summed before the one forward transform.
 //   correlate_cells   per (PRN, Doppler) cell: x conj(FFT(replica)) (utils.py:69, spectrum staged into shared
 //                     memory with a TMA bulk copy), inverse warp FFTs (utils.py:73), |.| accumulation over ms
 //                     (utils.py:102-104) in registers, peak/argmax/sum/count reduction with REDUX / warp shuffles
@@ -101,10 +103,12 @@ __host__ __device__ constexpr int spec_f2(int s) {  // float2 of rows + tiles
                          : s * kFft + spec_warps(s) * kSpecTileF2;
 }
 
-// 2.046 Msps: a register cap of four CTAs per SM (128 registers).  The cap of five (96 registers) spilled 216 B per thread, and
-// the benchmark's 256-block launch took 0.214 ms against 0.168 ms at four (H100, DESIGN.md section 4).
-template <int S>
-__global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_spectra(const SpectraArgs a) {
+// The body of both spectra kernels.  SEG = false: one CTA per (unit, millisecond i).  SEG = true (semi-coherent grids): one
+// CTA per (unit, segment i) of a.T milliseconds, whose wiped-off milliseconds are summed before the one boxcar and forward
+// transform -- the correlation is linear and the code repeats every millisecond, so the transform of the sum is the coherent
+// sum of the T millisecond transforms.
+template <int S, bool SEG>
+__device__ __forceinline__ void doppler_spectra_body(const SpectraArgs& a) {
     constexpr int kSpecWarps = spec_warps(S);
     constexpr int kSpecThreads = kSpecWarps * 32;
     extern __shared__ __align__(16) float2 smem[];
@@ -120,7 +124,6 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_
     // correct.)
     const double f = a.doppler[d];
     if (isnan(f)) return;  // slot switched off by the on-device search planner
-    const float2* __restrict__ src = a.iq + static_cast<size_t>(b) * a.block_stride + static_cast<size_t>(i) * a.N;
     const int tid = threadIdx.x;
 
     // Carrier exp(-j 2 pi f (n + i N)/fs) (utils.py:93-96) as coarse[n / T] * fine[n % T]: both factors get an
@@ -131,6 +134,8 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_
     // coalesced float2 loads of the 1-ms IQ vector, ALL issued before the carrier set-up and the first use (the loop form
     // stalls on every load); from S = 5 on the samples past the first 16 per thread go through the tail loop below
     constexpr int kBatch = kIter < 16 ? kIter : 16;
+    if constexpr (!SEG) {
+    const float2* __restrict__ src = a.iq + static_cast<size_t>(b) * a.block_stride + static_cast<size_t>(i) * a.N;
     float2 v[kBatch];
 #pragma unroll
     for (int k = 0; k < kBatch; ++k) {
@@ -149,6 +154,41 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_
     }
     for (int k = kBatch, n = tid + kBatch * kSpecThreads; n < a.N; ++k, n += kSpecThreads)
         ypoly[(n % S) * kFft + zpos(n / S)] = cmul(src[n], cmul(coarse[k], fine));
+    } else {
+    // Segment i is milliseconds i*T .. i*T + T - 1 of the block, each wiped off with its own carrier (continuous phase over
+    // the block, as above) and summed into the polyphase rows.  Every thread owns the same row entries in every millisecond,
+    // so only the coarse carrier table needs a barrier between milliseconds.
+    if (a.pfa) stage_row31(coef);
+    const float2 fine = carrier_at(f, static_cast<double>(tid), a.inv_fs);
+    const float2* __restrict__ blk = a.iq + static_cast<size_t>(b) * a.block_stride;
+    for (int t = 0; t < a.T; ++t) {
+        const int ms = i * a.T + t;
+        const float2* __restrict__ src = blk + static_cast<size_t>(ms) * a.N;
+        float2 v[kBatch];
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const int n = tid + k * kSpecThreads;
+            v[k] = n < kChips * S ? src[n] : make_float2(0.f, 0.f);
+        }
+        if (t > 0) __syncthreads();  // every thread is done with the previous millisecond's coarse table
+        if (tid < kIter) coarse[tid] = carrier_at(f, static_cast<double>(tid * kSpecThreads + ms * a.N), a.inv_fs);
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const int n = tid + k * kSpecThreads;
+            if (n < kChips * S) {
+                float2& y = ypoly[(n % S) * kFft + zpos(n / S)];
+                const float2 w = cmul(v[k], cmul(coarse[k], fine));
+                y = t > 0 ? c_add(y, w) : w;
+            }
+        }
+        for (int k = kBatch, n = tid + kBatch * kSpecThreads; n < a.N; ++k, n += kSpecThreads) {
+            float2& y = ypoly[(n % S) * kFft + zpos(n / S)];
+            const float2 w = cmul(src[n], cmul(coarse[k], fine));
+            y = t > 0 ? c_add(y, w) : w;
+        }
+    }
+    }
     __syncthreads();
     if (tid < S) ypoly[tid * kFft + zpos(kFft - 1)] = ypoly[tid * kFft + zpos(0)];
     __syncthreads();
@@ -206,6 +246,20 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_
         __syncwarp();
         store_vec(x, lane, dst0 + static_cast<size_t>(task) * kFft);
     }
+}
+
+// 2.046 Msps: a register cap of four CTAs per SM (128 registers).  The cap of five (96 registers) spilled 216 B per thread, and
+// the benchmark's 256-block launch took 0.214 ms against 0.168 ms at four (H100, DESIGN.md section 4).
+template <int S>
+__global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_spectra(const SpectraArgs a) {
+    doppler_spectra_body<S, false>(a);
+}
+
+// Semi-coherent grids: one CTA per (unit, segment of a.T milliseconds), a.M segments per block.  Same shared memory and
+// register cap as k_doppler_spectra.
+template <int S>
+__global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_segment_spectra(const SpectraArgs a) {
+    doppler_spectra_body<S, true>(a);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -759,7 +813,10 @@ bool spectra_supports(int s) {
 
 template <int S>
 static cudaError_t spectra_attr() {
-    return cudaFuncSetAttribute(k_doppler_spectra<S>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    const cudaError_t e = cudaFuncSetAttribute(k_doppler_spectra<S>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               static_cast<int>(spectra_smem_bytes(S)));
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(k_segment_spectra<S>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(spectra_smem_bytes(S)));
 }
 cudaError_t configure_kernels() {
@@ -791,7 +848,11 @@ cudaError_t launch_doppler_spectra(const SpectraArgs& a, cudaStream_t st) {
     const int grid = a.n_units * a.M;
     const size_t sm = spectra_smem_bytes(a.s);
     switch (a.s) {
-#define GB_CASE(S) case S: k_doppler_spectra<S><<<grid, spec_warps(S) * 32, sm, st>>>(a); break;
+#define GB_CASE(S)                                                                \
+    case S:                                                                       \
+        if (a.T > 1) k_segment_spectra<S><<<grid, spec_warps(S) * 32, sm, st>>>(a); \
+        else k_doppler_spectra<S><<<grid, spec_warps(S) * 32, sm, st>>>(a);       \
+        break;
         GB_FOR_EACH_RATE(GB_CASE)
 #undef GB_CASE
         default: return cudaErrorInvalidValue;

@@ -8,17 +8,19 @@ namespace gb {
 constexpr int kKindCoherent = 1;     // utils.py:23-25: IntegrationType.Coherent = auto() -> 1
 constexpr int kKindNonCoherent = 2;  // IntegrationType.NonCoherent -> 2
 
-// doppler_spectra: one CTA per (unique Doppler u, millisecond i).
+// doppler_spectra: one CTA per (unique Doppler u, millisecond i); with T > 1 (segment_spectra) one per (u, segment i of T
+// milliseconds), M being the segments per block.
 struct SpectraArgs {
     const float2* iq;        // complex64 samples, block b starts at b * block_stride
     const double* doppler;   // [n_doppler] Hz
     float2* spec;            // [n_blocks*n_doppler][M][s][2][1024]
     const float2* tw1;       // [32][32]  exp(-2 pi i lane k1 / 1024)
     const float2* tw2;       // [1024]    exp(-2 pi i n / 2048)
-    long long block_stride;  // samples between consecutive blocks (= M*N)
+    long long block_stride;  // samples between consecutive blocks (= M*N, or M*T*N with segments)
     int pfa;                 // spectra for k_correlate_pfa: DFT1023(z_r) per branch r (warp_pfa.cuh order) in [r][0]; else both halves
     double inv_fs;
     int N, s, M, n_doppler, n_units;  // n_units = n_blocks * n_doppler
+    int T;                   // milliseconds per coherent segment; T > 1 selects segment_spectra
 };
 
 // correlate_cells: one warp (k_correlate_pfa) or warp pair (k_correlate_cells) per (cell, r-range); every slot of a CTA

@@ -120,6 +120,29 @@ int gb200_acquire_grid_best(gb200_engine* e, int n_blocks, int ms_per_block, con
 int gb200_acquire_grid_best_device(gb200_engine* e, int n_blocks, int ms_per_block, const int32_t* prn_idx, int n_prn,
                                    const double* doppler_hz, int n_doppler, int integration_type, void* out_device);
 
+/* Semi-coherent grid for weak signals (no counterpart in the reference, which offers only its two IntegrationTypes):
+ * each block's ms_per_block milliseconds are cut into K = ms_per_block / coherent_ms segments, each segment's 1-ms
+ * correlations are summed coherently, and the K magnitudes are added:  profile = sum_k |sum_{t<T} corr(k*T + t)|.
+ * A segment gains 10*log10(T) dB of SNR before its magnitude is taken, and needs Doppler bins of about 1/(2T) s
+ * (50 Hz at T = 10 ms).  Records, best records and the layouts of out are those of the gb200_acquire_grid* quartet
+ * above over that profile, with the same strength formula.  Rules: coherent_ms >= 1, ms_per_block a multiple of it
+ * (a partial segment is GB200_EINVAL, never dropped), and every rule of gb200_acquire_grid; nothing is launched on an
+ * error.  coherent_ms == 1 is gb200_acquire_grid(..., GB200_NON_COHERENT), byte for byte.
+ * Not handled: a navigation data bit edge inside a segment (every 20 ms) cancels part of that segment, up to all of
+ * it; code Doppler smears the peak by |f| / 1540 chips per second, as in the non-coherent grid.  There is no
+ * detection threshold: the reference's strength threshold was set for its own statistic.                          */
+int gb200_acquire_grid_semicoherent(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms, const int32_t* prn_idx,
+                                    int n_prn, const double* doppler_hz, int n_doppler, gb200_cell_record* out_host);
+int gb200_acquire_grid_semicoherent_device(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms,
+                                           const int32_t* prn_idx, int n_prn, const double* doppler_hz, int n_doppler,
+                                           void* out_device);
+int gb200_acquire_grid_semicoherent_best(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms,
+                                         const int32_t* prn_idx, int n_prn, const double* doppler_hz, int n_doppler,
+                                         gb200_best_record* out_host);
+int gb200_acquire_grid_semicoherent_best_device(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms,
+                                                const int32_t* prn_idx, int n_prn, const double* doppler_hz, int n_doppler,
+                                                void* out_device);
+
 /* acquisition.py:154-190 get_best_doppler_shift_estimation / :122-136: an arbitrary list of (prn, Doppler)
  * cells over the first n_ms milliseconds of the loaded IQ.  probe_idx (may be NULL) gives, per cell, the
  * profile index whose complex value is wanted for coherent integration, or -1.                      */

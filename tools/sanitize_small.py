@@ -28,6 +28,8 @@ for n, m in ((2046, 2), (4092, 1)):
         big = eng.acquire_grid(2, 1, np.arange(32), np.linspace(-10000, 10000, 161))  # full 32-PRN grid, 12-warp one-warp build
         r = eng.detect([24, 2], m)
         assert int(big["argmax"][0, 24, int(np.argmax(big["peak"][0, 24]))]) == 777 and int(r["code_phase"][0]) == 777
+        sg = eng.acquire_grid_semicoherent(1, m, 2, [24, 0, 5], dop)  # k_segment_spectra<2>, one segment of two ms
+        assert int(sg["argmax"][0, 0, 7]) == 777
         xs = to.synth_tracking_iq(3, n, 12, fs, [(25, 1500.3, 0.0, 777, 0.3, 0.004)])
         eng.upload_iq(xs)
         t = _native.Tracker(eng, [24, 6], [1500.0, -100.0], [0.0, 0.0], [777, 5])
@@ -146,6 +148,10 @@ for n in (5115, 12276):
     for m in (1, 2):
         g = eng.acquire_grid(1, m, [24, 0, 5], dop)
         assert int(g["argmax"][0, 0, 7]) == n - 1
+    # semi-coherent grid: k_segment_spectra (two-millisecond segment sums, tail loop), then its best bins
+    sg = eng.acquire_grid_semicoherent(1, 2, 2, [24, 0, 5], dop)
+    sb = eng.acquire_grid_semicoherent_best(1, 2, 2, [24, 0, 5], dop)
+    assert int(sg["argmax"][0, 0, 7]) == n - 1 == int(sb["code_phase"][0, 0])
     c = eng.acquire_cells([24, 3, 24], [1500.0, 0.0, 1000.0], 2, _native.COHERENT, probe_idx=[n - 1, 0, n // 2])
     p = eng.correlation_profile(24, 1500.0, 2, _native.NON_COHERENT)
     r = eng.detect([24, 2], 2)
