@@ -53,6 +53,10 @@ SYMBOLS = {
     "gb200_acquire_grid_semicoherent_device": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
     "gb200_acquire_grid_semicoherent_best": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
     "gb200_acquire_grid_semicoherent_best_device": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
+    "gb200_acquire_grid_weak": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
+    "gb200_acquire_grid_weak_device": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
+    "gb200_acquire_grid_weak_best": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
+    "gb200_acquire_grid_weak_best_device": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, _P]),
     "gb200_ring_create": (C.c_int, [_P, C.c_int, C.POINTER(_P)]),
     "gb200_ring_destroy": (C.c_int, [_P]),
     "gb200_ring_append": (C.c_int, [_P, _P, C.c_int]),
@@ -347,6 +351,52 @@ class Engine:
             self._lib.gb200_acquire_grid_semicoherent_best_device(self._h, n_blocks, ms_per_block, coherent_ms, _ptr(prn),
                                                                   prn.size, _ptr(dop), dop.size, _P(out_device_ptr)),
             "gb200_acquire_grid_semicoherent_best_device",
+        )
+
+    def acquire_grid_weak(self, n_blocks: int, ms_per_block: int, coherent_ms: int, bit_phases: int, prn_idx, doppler_hz,
+                          out: np.ndarray | None = None) -> np.ndarray:
+        """Weak grid (gb200_acquire_grid_weak): per cell and bit phase j the semi-coherent profile of the segments starting
+        at millisecond j * coherent_ms / bit_phases, every millisecond realigned by its code Doppler, reduced to
+        RECORD_DTYPE [n_blocks, n_prn, bit_phases, n_doppler]."""
+        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
+        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
+        shape = (n_blocks, prn.size, bit_phases, dop.size)
+        out = _records_out(out, shape if min(shape) > 0 else (0,))
+        self._check(
+            self._lib.gb200_acquire_grid_weak(self._h, n_blocks, ms_per_block, coherent_ms, bit_phases, _ptr(prn), prn.size,
+                                              _ptr(dop), dop.size, _ptr(out)),
+            "gb200_acquire_grid_weak",
+        )
+        return out
+
+    def acquire_grid_weak_device(self, n_blocks, ms_per_block, coherent_ms, bit_phases, prn: np.ndarray, dop: np.ndarray,
+                                 out_device_ptr: int):
+        """prn (int32) / dop (float64) must be contiguous arrays kept alive by the caller; enqueue only."""
+        self._check(
+            self._lib.gb200_acquire_grid_weak_device(self._h, n_blocks, ms_per_block, coherent_ms, bit_phases, _ptr(prn),
+                                                     prn.size, _ptr(dop), dop.size, _P(out_device_ptr)),
+            "gb200_acquire_grid_weak_device",
+        )
+
+    def acquire_grid_weak_best(self, n_blocks: int, ms_per_block: int, coherent_ms: int, bit_phases: int, prn_idx,
+                               doppler_hz) -> np.ndarray:
+        """The weak grid's best folded bin per (block, prn) row: BEST_DTYPE [n_blocks, n_prn], bin = j * n_doppler + d."""
+        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
+        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
+        out = np.empty((max(n_blocks, 0), prn.size), dtype=BEST_DTYPE)
+        self._check(
+            self._lib.gb200_acquire_grid_weak_best(self._h, n_blocks, ms_per_block, coherent_ms, bit_phases, _ptr(prn),
+                                                   prn.size, _ptr(dop), dop.size, _ptr(out)),
+            "gb200_acquire_grid_weak_best",
+        )
+        return out
+
+    def acquire_grid_weak_best_device(self, n_blocks, ms_per_block, coherent_ms, bit_phases, prn: np.ndarray, dop: np.ndarray,
+                                      out_device_ptr: int):
+        self._check(
+            self._lib.gb200_acquire_grid_weak_best_device(self._h, n_blocks, ms_per_block, coherent_ms, bit_phases,
+                                                          _ptr(prn), prn.size, _ptr(dop), dop.size, _P(out_device_ptr)),
+            "gb200_acquire_grid_weak_best_device",
         )
 
     def acquire_cells(self, prn_idx, doppler_hz, n_ms: int, kind: int = NON_COHERENT, probe_idx=None) -> np.ndarray:

@@ -7,6 +7,7 @@ evaluation per (satellite, bin).
 from __future__ import annotations
 
 import logging
+import math
 from dataclasses import dataclass
 
 import numpy as np
@@ -33,6 +34,13 @@ class SatelliteAcquisitionAttemptResult:  # acquisition.py:35-41
     carrier_wave_phase_shift: float
     prn_phase_shift: int
     correlation_strength: float
+
+
+def code_shift(ms, n: int, doppler_hz):
+    """The weak grid's realignment of millisecond ms (from the block's first) at Doppler f, in samples: rint(ms * N * f /
+    f_L1), evaluated in the engine's order (kernels.cuh code_shift).  A closing satellite's code lag at that millisecond is
+    its lag at the first sample minus this."""
+    return np.rint(np.float64(ms) * n * np.asarray(doppler_hz, dtype=np.float64) / 1575.42e6)
 
 
 def doppler_search_bins(center: float, spread: float) -> range:
@@ -170,6 +178,66 @@ class GpsSatelliteDetector:
         best = eng.acquire_grid_semicoherent_best(1, n_ms, coherent_ms, prn_idx, bins)[0]
         rec = eng.acquire_cells(prn_idx, best["doppler"], coherent_ms, _native.COHERENT, probe_idx=best["code_phase"])
         phase = np.angle(rec["probe_re"].astype(np.float64) + 1j * rec["probe_im"].astype(np.float64))
+        return [
+            SatelliteAcquisitionAttemptResult(
+                satellite_id=sid, doppler_shift=float(best["doppler"][i]), carrier_wave_phase_shift=float(phase[i]),
+                prn_phase_shift=int(best["code_phase"][i]), correlation_strength=float(best["strength"][i]),
+            )
+            for i, sid in enumerate(satellite_ids)
+        ]
+
+    def search_weak_satellites(self, satellite_ids, antenna_data, stream_attributes, coherent_ms: int = 20,
+                               bit_phases: int = 4, doppler_spread: float = 7000.0, doppler_step: float | None = None
+                               ) -> list[SatelliteAcquisitionAttemptResult]:
+        """Weak-signal acquisition through navigation data bits and code Doppler: every satellite's semi-coherent profile
+        (segments of coherent_ms ms) at each of bit_phases segment offsets coherent_ms / bit_phases ms apart, with each
+        millisecond realigned by its code Doppler, on the Doppler bins arange(-spread, spread + step / 2, step) (step
+        500 / coherent_ms Hz by default), in one gb200_acquire_grid_weak_best call.  The window (uploaded samples or a
+        DeviceSampleRing window) is trimmed to the longest one the bit phases cover with whole segments.  Then one coherent
+        integration over the first segment of each satellite's best bit phase, which lies inside one data bit, gives the
+        carrier phase at its code phase, referred back to the window's first sample (modulo pi: the bit's sign is unknown).
+
+        One result per satellite, NOT thresholded: the reference's strength threshold was set for its own statistic."""
+        for name, v in (("coherent_ms", coherent_ms), ("bit_phases", bit_phases)):
+            if isinstance(v, bool) or int(v) != v or v < 1:
+                raise ValueError(f"{name} must be a positive whole number (got {v!r})")
+        coherent_ms, bit_phases = int(coherent_ms), int(bit_phases)
+        if coherent_ms % bit_phases:
+            raise ValueError(f"bit_phases ({bit_phases}) must divide coherent_ms ({coherent_ms})")
+        spread = float(doppler_spread)
+        step = 500.0 / coherent_ms if doppler_step is None else float(doppler_step)
+        if not (np.isfinite(spread) and spread >= 0.0):
+            raise ValueError(f"doppler_spread must be finite and >= 0 (got {doppler_spread!r})")
+        if not (np.isfinite(step) and step > 0.0):
+            raise ValueError(f"doppler_step must be finite and > 0 (got {doppler_step!r})")
+        if not satellite_ids:
+            return []
+        satellite_ids = list(satellite_ids)
+        eng, prn_idx, n, n_ms = self._prepare(satellite_ids, antenna_data, stream_attributes)
+        delta = coherent_ms // bit_phases
+        k = (n_ms - (bit_phases - 1) * delta) // coherent_ms
+        if k < 1:
+            raise ValueError(f"a {n_ms}-ms window holds no {coherent_ms}-ms segment at each of {bit_phases} bit phases "
+                             f"(needs {coherent_ms + (bit_phases - 1) * delta} ms)")
+        bins = np.arange(-spread, spread + step / 2, step)
+        best = eng.acquire_grid_weak_best(1, k * coherent_ms + (bit_phases - 1) * delta, coherent_ms, bit_phases, prn_idx,
+                                          bins)[0]
+        phase_of = best["bin"] // bins.size
+        phase = np.zeros(len(satellite_ids))
+        on_device = hasattr(antenna_data, "bind")
+        for j in np.unique(phase_of):
+            first = int(j) * delta  # the phase's first segment: milliseconds first .. first + coherent_ms - 1
+            if first and on_device:
+                antenna_data.ring.native.bind_newest(n_ms - first)
+            elif first:
+                eng.upload_iq(np.ascontiguousarray(antenna_data, dtype=np.complex64)[first * n:(first + coherent_ms) * n])
+            sel = np.flatnonzero(phase_of == j)
+            f = best["doppler"][sel]
+            # the code phase at the segment's first sample, where the probe's correlation peaks
+            probe = (best["code_phase"][sel] - code_shift(first, n, f).astype(np.int64)) % n
+            rec = eng.acquire_cells(np.asarray(prn_idx)[sel], f, coherent_ms, _native.COHERENT, probe_idx=probe)
+            z = rec["probe_re"].astype(np.float64) + 1j * rec["probe_im"].astype(np.float64)
+            phase[sel] = np.angle(z * np.exp(-1j * math.tau * f * first * 1e-3))
         return [
             SatelliteAcquisitionAttemptResult(
                 satellite_id=sid, doppler_shift=float(best["doppler"][i]), carrier_wave_phase_shift=float(phase[i]),

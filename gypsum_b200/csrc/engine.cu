@@ -64,10 +64,20 @@ int pick_rsplit(const gb200_engine* e, int slots, long long n_cells) {
 
 size_t unit_floats2(const gb200_engine* e, int M) { return static_cast<size_t>(M) * e->s * 2 * kFft; }
 
+// How a grid's milliseconds are integrated before their magnitudes are added: coherent segments of T milliseconds
+// (T = 1: the non-coherent grid), and for a weak grid (B >= 1) B bit phases T / B milliseconds apart, each millisecond
+// realigned by its code Doppler.  B = 0: the segments start at the block's first millisecond, with no realignment.
+struct Segments {
+    int T = 1, B = 0;
+    int step() const { return B > 0 ? T / B : 0; }
+    int count(int M) const { return (M - (B > 0 ? B - 1 : 0) * step()) / T; }  // K, spectra per unit
+};
+
 // doppler_spectra of n_units (block, Doppler) units, n_doppler per block, blocks of M milliseconds consecutive from iq.
-// pfa: for the one-warp correlate kernel (spectra_pfa).  T > 1: one spectrum per segment of T milliseconds (M / T per unit,
-// T divides M) instead of one per millisecond.
-int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int n_doppler, int n_units, bool pfa, int T = 1) {
+// pfa: for the one-warp correlate kernel (spectra_pfa).  seg.T > 1 or a weak grid: one spectrum per segment of T
+// milliseconds (seg.count(M) per unit) instead of one per millisecond; a weak grid's n_doppler folds its B bit phases.
+int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int n_doppler, int n_units, bool pfa,
+                Segments seg = {}) {
     SpectraArgs sa{};
     sa.iq = iq;
     sa.doppler = dop;
@@ -78,8 +88,11 @@ int run_spectra(gb200_engine* e, const float2* iq, int M, const double* dop, int
     sa.inv_fs = 1.0 / static_cast<double>(e->fs);
     sa.N = e->N;
     sa.s = e->s;
-    sa.M = M / T;
-    sa.T = T;
+    sa.M = seg.count(M);
+    sa.T = seg.T;
+    sa.align = seg.B > 0 ? 1 : 0;
+    sa.phase_step = seg.step();
+    sa.phase_dopplers = seg.B > 0 ? n_doppler / seg.B : 0;
     sa.n_doppler = n_doppler;
     sa.n_units = n_units;
     sa.pfa = pfa ? 1 : 0;
@@ -191,6 +204,27 @@ int check_segments(gb200_engine* e, int ms_per_block, int coherent_ms) {
     return GB200_OK;
 }
 
+// A weak grid: B bit phases T / B milliseconds apart, each summing the same K >= 1 whole segments of T milliseconds inside
+// the block, and B * D folded Doppler slots that fit an int.
+int check_weak(gb200_engine* e, int ms_per_block, int coherent_ms, int bit_phases, int D) {
+    if (coherent_ms < 1) GB_FAIL(e, GB200_EINVAL, "coherent_ms must be at least 1 (got %d)", coherent_ms);
+    if (bit_phases < 1 || coherent_ms % bit_phases != 0)
+        GB_FAIL(e, GB200_EINVAL, "bit_phases (%d) must be at least 1 and divide coherent_ms (%d)", bit_phases, coherent_ms);
+    const long long span = static_cast<long long>(bit_phases - 1) * (coherent_ms / bit_phases);  // last phase's offset
+    if (ms_per_block < coherent_ms + span || (ms_per_block - span) % coherent_ms != 0)
+        GB_FAIL(e, GB200_EINVAL, "ms_per_block (%d) is not %lld ms plus a whole number (>= 1) of %d-ms coherent segments",
+                ms_per_block, span, coherent_ms);
+    if (static_cast<long long>(bit_phases) * D > INT32_MAX) GB_FAIL(e, GB200_EINVAL, "bit_phases * n_doppler exceeds an int");
+    return GB200_OK;
+}
+
+// The weak grid's folded Doppler axis: slot j * D + d holds dop[d].
+std::vector<double> fold_dopplers(const double* dop, int D, int B) {
+    std::vector<double> folded(static_cast<size_t>(B) * D);
+    for (int j = 0; j < B; ++j) std::copy(dop, dop + D, folded.begin() + static_cast<size_t>(j) * D);
+    return folded;
+}
+
 // What every acquisition needs before its own arguments are looked at.
 int check_common(gb200_engine* e, int n_ms, int kind) {
     GB_TRY(check_kind(e, kind));
@@ -228,10 +262,11 @@ int upload_grid_axes(gb200_engine* e, const int32_t* prn_idx, int P, const doubl
 }
 
 // grid mode: all cells of n_blocks x prn list x doppler list; records written to rec_dev (device).  The caller has applied
-// check_grid.  T > 1 (non-coherent kind, check_segments applied): a semi-coherent grid, whose correlate launch is the
-// non-coherent one over the M / T segment spectra of each unit.
+// check_grid.  seg.T > 1 (non-coherent kind, check_segments applied): a semi-coherent grid, whose correlate launch is the
+// non-coherent one over the M / T segment spectra of each unit.  A weak grid (seg.B >= 1, check_weak applied) is the same
+// over its seg.count(M) segments, with dop the folded list of D = B * (caller's Dopplers) slots.
 int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D, int kind,
-             CellRecord* rec_dev, int T = 1) {
+             CellRecord* rec_dev, Segments seg = {}) {
     GB_TRY(check_common(e, M, kind));
     if (static_cast<int64_t>(n_blocks) * M * e->N > e->iq_samples)
         GB_FAIL(e, GB200_EINVAL, "grid needs %lld samples, %lld loaded", static_cast<long long>(n_blocks) * M * e->N,
@@ -239,7 +274,7 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
     GB_TRY(check_prns(e, prn_idx, P));
     GB_TRY(upload_grid_axes(e, prn_idx, P, dop, D));
 
-    const int K = M / T;  // spectra per unit
+    const int K = seg.count(M);  // spectra per unit
     const size_t unit = unit_floats2(e, K);
     const size_t per_block = unit * D;
     int nb = static_cast<int>(std::max<size_t>(1, e->spec_budget_bytes / (per_block * sizeof(float2))));
@@ -253,7 +288,7 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
         const int nbb = std::min(nb, n_blocks - b0);
         const int chunks = (nbb * D + cpg - 1) / cpg;  // groups per PRN: its nbb*D cells in chunks of cpg
         GB_TRY(run_spectra(e, e->iq + static_cast<size_t>(b0) * M * e->N, M, e->d_doppler.p, D, nbb * D, spectra_pfa(kind, false),
-                           T));
+                           seg));
 
         CorrelateArgs ca = correlate_args(e, K, kind, rsplit, rec_dev + static_cast<size_t>(b0) * P * D, nullptr);
         ca.n_groups = P * chunks;
@@ -382,13 +417,30 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
 }
 
 // The grid's records into d_records, after check_grid; with best, then each (block, PRN) row's best bin into best
-// (acquisition.py:179-189 on the device).  T as for run_grid.
+// (acquisition.py:179-189 on the device).  seg as for run_grid.
 int grid_records(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D, int kind,
-                 BestRecord* best, int T = 1) {
+                 BestRecord* best, Segments seg = {}) {
     GB_CUDA(e, e->d_records.ensure(static_cast<size_t>(n_blocks) * P * D));
-    GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p, T));
+    GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p, seg));
     if (best) GB_LAUNCH(e, -1, launch_best_bins(n_blocks * P, D, e->N, e->d_records.p, e->d_doppler.p, best, e->stream));
     return GB200_OK;
+}
+
+// A weak grid, every rule checked first: its records into rec (device) when given, else into d_records and, with best, each
+// (block, PRN) row's best folded bin into best; host_best: into d_best.
+int weak_grid(gb200_engine* e, int n_blocks, int M, int T, int B, const int32_t* prn_idx, int P, const double* dop, int D,
+              CellRecord* rec, BestRecord* best, bool host_best = false) {
+    GB_CUDA(e, cudaSetDevice(e->device));
+    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
+    GB_TRY(check_weak(e, M, T, B, D));
+    const std::vector<double> folded = fold_dopplers(dop, D, B);
+    const Segments seg{T, B};
+    if (rec) return run_grid(e, n_blocks, M, prn_idx, P, folded.data(), B * D, GB200_NON_COHERENT, rec, seg);
+    if (host_best) {
+        GB_CUDA(e, e->d_best.ensure(static_cast<size_t>(n_blocks) * P));
+        best = e->d_best.p;
+    }
+    return grid_records(e, n_blocks, M, prn_idx, P, folded.data(), B * D, GB200_NON_COHERENT, best, seg);
 }
 
 // Records to the caller (see download).
@@ -575,7 +627,7 @@ int gb200_acquire_grid_semicoherent(gb200_engine* e, int n_blocks, int M, int co
     GB_CUDA(e, cudaSetDevice(e->device));
     GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     GB_TRY(check_segments(e, M, coherent_ms));
-    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, nullptr, coherent_ms));
+    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, nullptr, Segments{coherent_ms}));
     return fetch_records(e, static_cast<size_t>(n_blocks) * P * D, out_host);
 }
 
@@ -587,7 +639,8 @@ int gb200_acquire_grid_semicoherent_device(gb200_engine* e, int n_blocks, int M,
     GB_TRY(check_common(e, M, GB200_NON_COHERENT));
     GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     GB_TRY(check_segments(e, M, coherent_ms));
-    return run_grid(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, static_cast<CellRecord*>(out_device), coherent_ms);
+    return run_grid(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, static_cast<CellRecord*>(out_device),
+                    Segments{coherent_ms});
 }
 
 int gb200_acquire_grid_semicoherent_best(gb200_engine* e, int n_blocks, int M, int coherent_ms, const int32_t* prn_idx, int P,
@@ -599,7 +652,7 @@ int gb200_acquire_grid_semicoherent_best(gb200_engine* e, int n_blocks, int M, i
     GB_TRY(check_segments(e, M, coherent_ms));
     const size_t n = static_cast<size_t>(n_blocks) * P;
     GB_CUDA(e, e->d_best.ensure(n));
-    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, e->d_best.p, coherent_ms));
+    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, e->d_best.p, Segments{coherent_ms}));
     return download(e, reinterpret_cast<BestRecord*>(out_host), e->d_best.p, n, e->h_best);
 }
 
@@ -611,7 +664,41 @@ int gb200_acquire_grid_semicoherent_best_device(gb200_engine* e, int n_blocks, i
     GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     GB_TRY(check_segments(e, M, coherent_ms));
     return grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, static_cast<BestRecord*>(out_device),
-                        coherent_ms);
+                        Segments{coherent_ms});
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// weak grids: the semi-coherent profile at each of bit_phases segment offsets, every millisecond realigned by its code
+// Doppler, over the Doppler axis folded as bit_phases * n_doppler bins (bin j * n_doppler + d: phase j, Doppler d).
+// ---------------------------------------------------------------------------------------------------------
+int gb200_acquire_grid_weak(gb200_engine* e, int n_blocks, int M, int coherent_ms, int bit_phases, const int32_t* prn_idx,
+                            int P, const double* dop, int D, gb200_cell_record* out_host) {
+    if (!e) return GB200_EINVAL;
+    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
+    GB_TRY(weak_grid(e, n_blocks, M, coherent_ms, bit_phases, prn_idx, P, dop, D, nullptr, nullptr));
+    return fetch_records(e, static_cast<size_t>(n_blocks) * P * bit_phases * D, out_host);
+}
+
+int gb200_acquire_grid_weak_device(gb200_engine* e, int n_blocks, int M, int coherent_ms, int bit_phases, const int32_t* prn_idx,
+                                   int P, const double* dop, int D, void* out_device) {
+    if (!e) return GB200_EINVAL;
+    if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
+    return weak_grid(e, n_blocks, M, coherent_ms, bit_phases, prn_idx, P, dop, D, static_cast<CellRecord*>(out_device), nullptr);
+}
+
+int gb200_acquire_grid_weak_best(gb200_engine* e, int n_blocks, int M, int coherent_ms, int bit_phases, const int32_t* prn_idx,
+                                 int P, const double* dop, int D, gb200_best_record* out_host) {
+    if (!e) return GB200_EINVAL;
+    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
+    GB_TRY(weak_grid(e, n_blocks, M, coherent_ms, bit_phases, prn_idx, P, dop, D, nullptr, nullptr, true));
+    return download(e, reinterpret_cast<BestRecord*>(out_host), e->d_best.p, static_cast<size_t>(n_blocks) * P, e->h_best);
+}
+
+int gb200_acquire_grid_weak_best_device(gb200_engine* e, int n_blocks, int M, int coherent_ms, int bit_phases,
+                                        const int32_t* prn_idx, int P, const double* dop, int D, void* out_device) {
+    if (!e) return GB200_EINVAL;
+    if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
+    return weak_grid(e, n_blocks, M, coherent_ms, bit_phases, prn_idx, P, dop, D, nullptr, static_cast<BestRecord*>(out_device));
 }
 
 // Host to host in one call.  The first call of a shape runs eagerly (it may have to upload the axes and grow buffers,

@@ -5,7 +5,8 @@
 //                     This half of utils.py:65 does not depend on the PRN, so it is computed once per Doppler
 //                     bin and shared by all PRNs instead of being redone per cell as the reference does.
 //                     segment_spectra is the same per (Doppler, segment of T ms) of a semi-coherent grid: the T
-//                     wiped-off milliseconds are summed before the one forward transform.
+//                     wiped-off milliseconds are summed before the one forward transform.  aligned_segment_spectra
+//                     (weak grids) also offsets the segment by its bit phase and realigns each ms by its code Doppler.
 //   correlate_cells   per (PRN, Doppler) cell: x conj(FFT(replica)) (utils.py:69, spectrum staged into shared
 //                     memory with a TMA bulk copy), inverse warp FFTs (utils.py:73), |.| accumulation over ms
 //                     (utils.py:102-104) in registers, peak/argmax/sum/count reduction with REDUX / warp shuffles
@@ -103,11 +104,12 @@ __host__ __device__ constexpr int spec_f2(int s) {  // float2 of rows + tiles
                          : s * kFft + spec_warps(s) * kSpecTileF2;
 }
 
-// The body of both spectra kernels.  SEG = false: one CTA per (unit, millisecond i).  SEG = true (semi-coherent grids): one
+// The body of the three spectra kernels.  SEG = false: one CTA per (unit, millisecond i).  SEG = true (semi-coherent grids): one
 // CTA per (unit, segment i) of a.T milliseconds, whose wiped-off milliseconds are summed before the one boxcar and forward
 // transform -- the correlation is linear and the code repeats every millisecond, so the transform of the sum is the coherent
-// sum of the T millisecond transforms.
-template <int S, bool SEG>
+// sum of the T millisecond transforms.  ALIGN (with SEG; weak grids): the segment starts at the bit phase's offset, and each
+// millisecond's samples are added at rows shifted by its code Doppler, so that the code lines up across the segment.
+template <int S, bool SEG, bool ALIGN = false>
 __device__ __forceinline__ void doppler_spectra_body(const SpectraArgs& a) {
     constexpr int kSpecWarps = spec_warps(S);
     constexpr int kSpecThreads = kSpecWarps * 32;
@@ -156,13 +158,18 @@ __device__ __forceinline__ void doppler_spectra_body(const SpectraArgs& a) {
         ypoly[(n % S) * kFft + zpos(n / S)] = cmul(src[n], cmul(coarse[k], fine));
     } else {
     // Segment i is milliseconds i*T .. i*T + T - 1 of the block, each wiped off with its own carrier (continuous phase over
-    // the block, as above) and summed into the polyphase rows.  Every thread owns the same row entries in every millisecond,
-    // so only the coarse carrier table needs a barrier between milliseconds.
+    // the block, as above) and summed into the polyphase rows.  Without ALIGN every thread owns the same row entries in every
+    // millisecond, so only the coarse carrier table needs a barrier between milliseconds.  With ALIGN the segment starts
+    // j * phase_step milliseconds later (bit phase j of the folded slot d), and sample n of millisecond ms goes to row
+    // position (n + shift) mod N, the shift being uniform over the CTA: within a millisecond n -> (n + shift) mod N is a
+    // bijection, so no two threads touch one entry, and across milliseconds the two barriers around the coarse table order
+    // every read-modify-write of an entry after the previous millisecond's write of it.
     if (a.pfa) stage_row31(coef);
     const float2 fine = carrier_at(f, static_cast<double>(tid), a.inv_fs);
     const float2* __restrict__ blk = a.iq + static_cast<size_t>(b) * a.block_stride;
+    const int ms0 = ALIGN ? (d / a.phase_dopplers) * a.phase_step : 0;
     for (int t = 0; t < a.T; ++t) {
-        const int ms = i * a.T + t;
+        const int ms = ms0 + i * a.T + t;
         const float2* __restrict__ src = blk + static_cast<size_t>(ms) * a.N;
         float2 v[kBatch];
 #pragma unroll
@@ -170,20 +177,29 @@ __device__ __forceinline__ void doppler_spectra_body(const SpectraArgs& a) {
             const int n = tid + k * kSpecThreads;
             v[k] = n < kChips * S ? src[n] : make_float2(0.f, 0.f);
         }
-        if (t > 0) __syncthreads();  // every thread is done with the previous millisecond's coarse table
+        int shift = 0;  // in [0, N)
+        if constexpr (ALIGN) {
+            shift = static_cast<int>(fmod(code_shift(ms, a.N, f), static_cast<double>(a.N)));
+            if (shift < 0) shift += a.N;
+        }
+        if (t > 0) __syncthreads();  // every thread is done with the previous millisecond's coarse table (and rows)
         if (tid < kIter) coarse[tid] = carrier_at(f, static_cast<double>(tid * kSpecThreads + ms * a.N), a.inv_fs);
         __syncthreads();
 #pragma unroll
         for (int k = 0; k < kBatch; ++k) {
             const int n = tid + k * kSpecThreads;
             if (n < kChips * S) {
-                float2& y = ypoly[(n % S) * kFft + zpos(n / S)];
+                int p = n + shift;
+                if (ALIGN && p >= kChips * S) p -= kChips * S;
+                float2& y = ypoly[(p % S) * kFft + zpos(p / S)];
                 const float2 w = cmul(v[k], cmul(coarse[k], fine));
                 y = t > 0 ? c_add(y, w) : w;
             }
         }
         for (int k = kBatch, n = tid + kBatch * kSpecThreads; n < a.N; ++k, n += kSpecThreads) {
-            float2& y = ypoly[(n % S) * kFft + zpos(n / S)];
+            int p = n + shift;
+            if (ALIGN && p >= a.N) p -= a.N;
+            float2& y = ypoly[(p % S) * kFft + zpos(p / S)];
             const float2 w = cmul(src[n], cmul(coarse[k], fine));
             y = t > 0 ? c_add(y, w) : w;
         }
@@ -260,6 +276,13 @@ __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_doppler_
 template <int S>
 __global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_segment_spectra(const SpectraArgs a) {
     doppler_spectra_body<S, true>(a);
+}
+
+// Weak grids: one CTA per (unit, segment of a.T milliseconds) of a folded (bit phase, Doppler) slot, a.M segments per
+// block, every millisecond realigned by its code Doppler; any T, T = 1 included.  Same shared memory and register cap.
+template <int S>
+__global__ void __launch_bounds__(spec_warps(S) * 32, S == 2 ? 4 : 1) k_aligned_segment_spectra(const SpectraArgs a) {
+    doppler_spectra_body<S, true, true>(a);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -813,11 +836,11 @@ bool spectra_supports(int s) {
 
 template <int S>
 static cudaError_t spectra_attr() {
-    const cudaError_t e = cudaFuncSetAttribute(k_doppler_spectra<S>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               static_cast<int>(spectra_smem_bytes(S)));
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(k_segment_spectra<S>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                static_cast<int>(spectra_smem_bytes(S)));
+    const int sm = static_cast<int>(spectra_smem_bytes(S));
+    cudaError_t e = cudaFuncSetAttribute(k_doppler_spectra<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_segment_spectra<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_aligned_segment_spectra<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm);
+    return e;
 }
 cudaError_t configure_kernels() {
     cudaError_t e;
@@ -850,7 +873,8 @@ cudaError_t launch_doppler_spectra(const SpectraArgs& a, cudaStream_t st) {
     switch (a.s) {
 #define GB_CASE(S)                                                                \
     case S:                                                                       \
-        if (a.T > 1) k_segment_spectra<S><<<grid, spec_warps(S) * 32, sm, st>>>(a); \
+        if (a.align) k_aligned_segment_spectra<S><<<grid, spec_warps(S) * 32, sm, st>>>(a); \
+        else if (a.T > 1) k_segment_spectra<S><<<grid, spec_warps(S) * 32, sm, st>>>(a); \
         else k_doppler_spectra<S><<<grid, spec_warps(S) * 32, sm, st>>>(a);       \
         break;
         GB_FOR_EACH_RATE(GB_CASE)

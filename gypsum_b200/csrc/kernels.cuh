@@ -8,8 +8,8 @@ namespace gb {
 constexpr int kKindCoherent = 1;     // utils.py:23-25: IntegrationType.Coherent = auto() -> 1
 constexpr int kKindNonCoherent = 2;  // IntegrationType.NonCoherent -> 2
 
-// doppler_spectra: one CTA per (unique Doppler u, millisecond i); with T > 1 (segment_spectra) one per (u, segment i of T
-// milliseconds), M being the segments per block.
+// doppler_spectra: one CTA per (unique Doppler u, millisecond i); with T > 1 (segment_spectra) or align (aligned_segment_spectra)
+// one per (u, segment i of T milliseconds), M being the segments per block.
 struct SpectraArgs {
     const float2* iq;        // complex64 samples, block b starts at b * block_stride
     const double* doppler;   // [n_doppler] Hz
@@ -21,7 +21,19 @@ struct SpectraArgs {
     double inv_fs;
     int N, s, M, n_doppler, n_units;  // n_units = n_blocks * n_doppler
     int T;                   // milliseconds per coherent segment; T > 1 selects segment_spectra
+    // Weak grids (align = 1 selects aligned_segment_spectra, at any T): the Doppler axis is folded as n_doppler =
+    // B * phase_dopplers slots, slot d being bit phase j = d / phase_dopplers, whose segment i starts at block millisecond
+    // j * phase_step + i * T.  Each millisecond m is realigned by its code Doppler (code_shift).
+    int align, phase_step, phase_dopplers;
 };
+
+// The whole-sample code-Doppler shift of block millisecond m at Doppler f (N samples per millisecond): the code of a
+// satellite closing at f runs fast by f / f_L1, so its lag at millisecond m is tau0 - m * N * f / f_L1 samples, and a
+// sample added at row position (n + shift) mod N lines its millisecond up with millisecond 0.  The float64 expression is
+// evaluated in this order on the host, in the kernel and in the tests' oracle.
+__host__ __device__ inline double code_shift(int m, int N, double f) {
+    return rint(static_cast<double>(m) * N * f / 1575.42e6);
+}
 
 // correlate_cells: one warp (k_correlate_pfa) or warp pair (k_correlate_cells) per (cell, r-range); every slot of a CTA
 // works on the same PRN.

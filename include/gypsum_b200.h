@@ -128,9 +128,10 @@ int gb200_acquire_grid_best_device(gb200_engine* e, int n_blocks, int ms_per_blo
  * above over that profile, with the same strength formula.  Rules: coherent_ms >= 1, ms_per_block a multiple of it
  * (a partial segment is GB200_EINVAL, never dropped), and every rule of gb200_acquire_grid; nothing is launched on an
  * error.  coherent_ms == 1 is gb200_acquire_grid(..., GB200_NON_COHERENT), byte for byte.
- * Not handled: a navigation data bit edge inside a segment (every 20 ms) cancels part of that segment, up to all of
- * it; code Doppler smears the peak by |f| / 1540 chips per second, as in the non-coherent grid.  There is no
- * detection threshold: the reference's strength threshold was set for its own statistic.                          */
+ * Not handled here (the weak grid below handles both): a navigation data bit edge inside a segment (every 20 ms)
+ * cancels part of that segment, up to all of it; code Doppler smears the peak by |f| / 1540 chips per second, as in
+ * the non-coherent grid.  There is no detection threshold: the reference's strength threshold was set for its own
+ * statistic.                                                                                                        */
 int gb200_acquire_grid_semicoherent(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms, const int32_t* prn_idx,
                                     int n_prn, const double* doppler_hz, int n_doppler, gb200_cell_record* out_host);
 int gb200_acquire_grid_semicoherent_device(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms,
@@ -142,6 +143,39 @@ int gb200_acquire_grid_semicoherent_best(gb200_engine* e, int n_blocks, int ms_p
 int gb200_acquire_grid_semicoherent_best_device(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms,
                                                 const int32_t* prn_idx, int n_prn, const double* doppler_hz, int n_doppler,
                                                 void* out_device);
+
+/* Weak grid: the semi-coherent grid searched over the navigation data bit phase, with each millisecond realigned by its
+ * code Doppler.  With T = coherent_ms, B = bit_phases, M = ms_per_block and the phase step d = T / B, bit phase j
+ * (0 <= j < B) sums the K = (M - (B-1)*d) / T segments of milliseconds j*d + k*T .. j*d + k*T + T - 1 of the block:
+ *     profile_j[n] = sum_{k<K} | sum_{t<T} corr_aligned(j*d + k*T + t)[n] |
+ * One of the B phases keeps every segment inside one 20-ms data bit (within d ms) when B divides T and T divides 20.
+ * corr_aligned(m) is millisecond m (counted from the block's first millisecond), wiped off at its own time as in every
+ * grid, with its samples moved to row position (n + s_m) mod N before the correlation, where
+ *     s_m = rint((double)m * N * f / 1575.42e6)        (evaluated in exactly this order)
+ * takes back the code Doppler of a satellite at Doppler f (its lag drifts by -m*N*f/f_L1 samples), so code phases are
+ * those of the block's first sample.
+ * out holds out[((block * n_prn + a) * B + j) * n_doppler + d]: the Doppler axis folded as B * n_doppler bins, each with
+ * the record and strength formula of gb200_acquire_grid.  The best records are the best of each (block, PRN) row's
+ * B * n_doppler folded bins: bin = j * n_doppler + d, doppler_hz = doppler_hz[d].
+ * Rules: coherent_ms >= 1, bit_phases >= 1 dividing coherent_ms, ms_per_block >= coherent_ms + (B-1)*d and
+ * ms_per_block - (B-1)*d a multiple of coherent_ms (a partial segment is GB200_EINVAL, never dropped), and every rule of
+ * gb200_acquire_grid; nothing is launched on an error.  With B = 1 on a grid where every s_m is 0, the records equal
+ * gb200_acquire_grid_semicoherent's byte for byte.  coherent_ms = 1 (B = 1) is a non-coherent grid with realignment.
+ * Not handled: a bit edge falls at the satellite's code epoch, inside a millisecond, so even the right phase has up to
+ * 1 ms of one segment with the other sign; s_m is a whole sample, which leaves up to 1/2 sample (1/2 chip at 1.023 Msps)
+ * of misalignment between milliseconds; there are no weak variants of gb200_acquire_grid_host, the grid streams, cell
+ * lists, gb200_detect or the sharded searches.  There is no detection threshold.                                     */
+int gb200_acquire_grid_weak(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms, int bit_phases,
+                            const int32_t* prn_idx, int n_prn, const double* doppler_hz, int n_doppler,
+                            gb200_cell_record* out_host);
+int gb200_acquire_grid_weak_device(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms, int bit_phases,
+                                   const int32_t* prn_idx, int n_prn, const double* doppler_hz, int n_doppler, void* out_device);
+int gb200_acquire_grid_weak_best(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms, int bit_phases,
+                                 const int32_t* prn_idx, int n_prn, const double* doppler_hz, int n_doppler,
+                                 gb200_best_record* out_host);
+int gb200_acquire_grid_weak_best_device(gb200_engine* e, int n_blocks, int ms_per_block, int coherent_ms, int bit_phases,
+                                        const int32_t* prn_idx, int n_prn, const double* doppler_hz, int n_doppler,
+                                        void* out_device);
 
 /* acquisition.py:154-190 get_best_doppler_shift_estimation / :122-136: an arbitrary list of (prn, Doppler)
  * cells over the first n_ms milliseconds of the loaded IQ.  probe_idx (may be NULL) gives, per cell, the

@@ -3,7 +3,10 @@ T = 10, K = 10, through gb200_acquire_grid_semicoherent_best_device; against it 
 grid over the same 281 bins and over 29 bins at 500 Hz, and config 2's grid (32 PRN x 41 Doppler x 1 ms, 256 blocks) for
 its per-transform rate.  Prints the card, its power limit and one JSON line per workload, then the noise-only strength
 distribution of the best bin of the main workload over 32 noise-only PRNs.
-usage: python tools/bench_semicoherent.py [--reps R]"""
+With --weak the main workload is the weak grid instead (gb200_acquire_grid_weak_best_device): one 995-ms window at
+2.046 Msps, 32 PRNs, +-7 kHz at 25 Hz (561 bins), T = 20 with B = 4 bit phases 5 ms apart (K = 49 segments per phase),
+with config 2's grid for its per-transform rate and the same noise-only distribution.
+usage: python tools/bench_semicoherent.py [--reps R] [--weak]"""
 import json
 import os
 import subprocess
@@ -59,6 +62,60 @@ def timed(eng, call, reps):
     return ms, ks / reps, kc / reps
 
 
+def config2_row(eng, prn):
+    """Config 2's grid: 256 one-millisecond blocks of 32 PRN x 41 Doppler."""
+    nb = 256
+    x2 = noise(nb * N, 2)
+    x2d = torch.from_numpy(x2).cuda()
+    dop2 = np.linspace(-10000, 10000, 41)
+    out2 = torch.empty(nb * 32 * 41 * 32, dtype=torch.uint8, device="cuda")
+    eng.bind_iq_device(x2d.data_ptr(), x2.size)
+    ms, ks, kc = timed(eng, lambda: eng.acquire_grid_device(nb, 1, prn, dop2, _native.NON_COHERENT, out2.data_ptr()), REPS)
+    t2 = nb * 32 * 41 * S
+    return dict(workload="config 2 grid, 256 blocks", call_ms=ms, spectra_ms=ks, correlate_ms=kc, inverse_transforms=t2,
+                forward_transforms=nb * 41 * S, inverse_per_s=t2 / (kc * 1e-3), call_transforms_per_s=t2 / (ms * 1e-3))
+
+
+def print_rows(rows):
+    for r in rows:
+        r["correlate_rate_vs_config2"] = r["inverse_per_s"] / rows[-1]["inverse_per_s"]
+        print(json.dumps(r), flush=True)
+
+
+def print_noise(best_strengths):
+    s = np.array(best_strengths)
+    print(json.dumps({"noise_only_best_strength": {"n": int(s.size), "mean": float(s.mean()), "p50": float(np.median(s)),
+                                                   "p99": float(np.quantile(s, 0.99)), "max": float(s.max())}}), flush=True)
+
+
+def weak(eng, prn):
+    t, b, m = 20, 4, 995
+    k = (m - (b - 1) * (t // b)) // t
+    x = noise(m * N, 1)
+    x += o.synth_iq(0, N, m, FS, [(25, 1234.0, 777, 0.3, 0.016)], sigma=0.0)  # 27.2 dB-Hz
+    xd = torch.from_numpy(x).cuda()
+    eng.bind_iq_device(xd.data_ptr(), x.size)
+    fine = np.arange(-7000.0, 7012.5, 25.0)
+    out = torch.empty(32 * 32, dtype=torch.uint8, device="cuda")
+    ms, ks, kc = timed(eng, lambda: eng.acquire_grid_weak_best_device(1, m, t, b, prn, fine, out.data_ptr()), REPS)
+    transforms = 32 * b * fine.size * k * S  # inverse DFT-1023 per (PRN, phase, bin, segment, branch)
+    row = dict(workload=f"weak T={t} B={b} K={k} M={m}, {fine.size} bins (best)", call_ms=ms, spectra_ms=ks, correlate_ms=kc,
+               inverse_transforms=transforms, forward_transforms=b * fine.size * k * S,
+               wiped_ms=b * fine.size * k * t, inverse_per_s=transforms / (kc * 1e-3),
+               call_transforms_per_s=transforms / (ms * 1e-3))
+    best = eng.acquire_grid_weak_best(1, m, t, b, prn, fine)[0]
+    row["sv25_found"] = [float(best["doppler"][24]), int(best["code_phase"][24]), int(best["bin"][24]) // fine.size,
+                         float(best["strength"][24])]
+    del xd
+    print_rows([row, config2_row(eng, prn)])
+    strengths = []
+    for seed in range(8):
+        xn = torch.from_numpy(noise(m * N, 100 + seed)).cuda()
+        eng.bind_iq_device(xn.data_ptr(), m * N)
+        strengths.extend(eng.acquire_grid_weak_best(1, m, t, b, prn, fine)[0]["strength"].tolist())
+    print_noise(strengths)
+
+
 def main():
     print(json.dumps({"card": card()}), flush=True)
     eng = _native.Engine(FS, N)
@@ -67,6 +124,11 @@ def main():
     torch.cuda.set_stream(st)
     eng.set_stream(st.cuda_stream)
     prn = np.arange(32, dtype=np.int32)
+    if "--weak" in sys.argv:
+        weak(eng, prn)
+        eng.set_stream(0)
+        eng.close()
+        return
     m = 100
     x = noise(m * N, 1)
     x += o.synth_iq(0, N, m, FS, [(25, 1234.0, 777, 0.3, 0.03)], sigma=0.0)  # 32.7 dB-Hz, 20-ms data bits off
@@ -93,29 +155,15 @@ def main():
                          inverse_per_s=transforms / (kc * 1e-3), call_transforms_per_s=transforms / (ms * 1e-3)))
     best = eng.acquire_grid_semicoherent_best(1, m, 10, prn, fine)[0]
     rows[0]["sv25_found"] = [float(best["doppler"][24]), int(best["code_phase"][24]), float(best["strength"][24])]
-    # config 2's grid: 256 one-millisecond blocks of 32 PRN x 41 Doppler
-    nb = 256
-    x2 = noise(nb * N, 2)
-    x2d = torch.from_numpy(x2).cuda()
-    dop2 = np.linspace(-10000, 10000, 41)
-    out2 = torch.empty(nb * 32 * 41 * 32, dtype=torch.uint8, device="cuda")
-    eng.bind_iq_device(x2d.data_ptr(), x2.size)
-    ms, ks, kc = timed(eng, lambda: eng.acquire_grid_device(nb, 1, prn, dop2, _native.NON_COHERENT, out2.data_ptr()), REPS)
-    t2 = nb * 32 * 41 * S
-    rows.append(dict(workload="config 2 grid, 256 blocks", call_ms=ms, spectra_ms=ks, correlate_ms=kc, inverse_transforms=t2,
-                     forward_transforms=nb * 41 * S, inverse_per_s=t2 / (kc * 1e-3), call_transforms_per_s=t2 / (ms * 1e-3)))
-    for r in rows:
-        r["correlate_rate_vs_config2"] = r["inverse_per_s"] / rows[-1]["inverse_per_s"]
-        print(json.dumps(r), flush=True)
+    rows.append(config2_row(eng, prn))
+    print_rows(rows)
     # noise-only strength of the main workload's best bin: 32 PRNs x 8 windows of pure noise
     strengths = []
     for seed in range(8):
         xn = torch.from_numpy(noise(m * N, 100 + seed)).cuda()
         eng.bind_iq_device(xn.data_ptr(), m * N)
         strengths.extend(eng.acquire_grid_semicoherent_best(1, m, 10, prn, fine)[0]["strength"].tolist())
-    s = np.array(strengths)
-    print(json.dumps({"noise_only_best_strength": {"n": int(s.size), "mean": float(s.mean()), "p50": float(np.median(s)),
-                                                   "p99": float(np.quantile(s, 0.99)), "max": float(s.max())}}), flush=True)
+    print_noise(strengths)
     eng.set_stream(0)
     eng.close()
 

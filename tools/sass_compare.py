@@ -24,7 +24,8 @@ def sass(lib: str) -> dict[str, str]:
         if m:
             cur = out.setdefault(m.group(1), [])
         elif cur is not None and "/*" in line:  # instructions and their encodings, not the section headers between kernels
-            cur.append(line.rstrip())
+            # cuobjdump pads every line to the widest instruction of the whole dump: compare the tokens, not the padding
+            cur.append(" ".join(line.split()))
     return {k: "\n".join(v) for k, v in out.items()}
 
 
