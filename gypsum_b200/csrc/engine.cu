@@ -1065,7 +1065,11 @@ int gb200_grid_stream_create(gb200_engine* e, int n_blocks, int M, const int32_t
     *out = nullptr;
     GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
     if (depth < 1 || depth > 8) GB_FAIL(e, GB200_EINVAL, "depth must be 1..8");
-    GB_TRY(check_common(e, M, kind));
+    // not check_common: the stream brings its own IQ (each submit binds a slot buffer and checks it), so the engine need
+    // not have any bound now -- on a fresh engine, or right after another stream took its slot buffers with it
+    GB_TRY(check_kind(e, kind));
+    GB_TRY(check_replicas(e));
+    if (M < 1) GB_FAIL(e, GB200_EINVAL, "need at least one whole millisecond of samples");
     GB_TRY(check_prns(e, prn_idx, P));
     GB_CUDA(e, cudaSetDevice(e->device));
     gb200_grid_stream* g = new gb200_grid_stream;

@@ -65,7 +65,11 @@ int gb200_set_stream(gb200_engine* e, void* cuda_stream);
 int gb200_set_replicas(gb200_engine* e, const uint8_t* chips, int n_prn);
 
 /* receiver.py:219 antenna_data: complex64[n_samples] (interleaved float32 I,Q -- the on-disk format of
- * antenna_sample_provider.py:112-119).  upload copies from the host; bind uses a device buffer in place.    */
+ * antenna_sample_provider.py:112-119).  upload copies from the host; bind uses a device buffer in place.
+ * A pageable iq_host is copied into a staging buffer before upload returns, so the caller may reuse it at once.  From a
+ * pinned iq_host the copy is only enqueued: the caller must not rewrite the buffer until a call that synchronises
+ * the engine's stream has returned (any call that hands results back to the host, e.g. gb200_acquire_grid).  The same
+ * holds for gb200_ring_append and gb200_grid_stream_submit; gb200_acquire_grid_host synchronises before it returns.  */
 int gb200_upload_iq(gb200_engine* e, const float* iq_host, int64_t n_samples);
 /* iq_device must be 16-byte aligned (the fused and tracking kernels stage it with bulk / cp.async copies). */
 int gb200_bind_iq_device(gb200_engine* e, const void* iq_device, int64_t n_samples);
@@ -77,7 +81,8 @@ int gb200_bind_iq_device(gb200_engine* e, const void* iq_device, int64_t n_sampl
 typedef struct gb200_ring gb200_ring;
 int gb200_ring_create(gb200_engine* e, int capacity_ms, gb200_ring** out);
 int gb200_ring_destroy(gb200_ring* r);
-/* Append n_ms whole milliseconds (complex64[n_ms * N]) from host memory. */
+/* Append n_ms whole milliseconds (complex64[n_ms * N]) from host memory.  A pinned iq_host is read after the call
+ * returns: do not rewrite it before a synchronising call (see gb200_upload_iq).                                  */
 int gb200_ring_append(gb200_ring* r, const float* iq_host, int n_ms);
 /* The engine's IQ binding := the newest n_ms milliseconds (zero copy); what gb200_detect / gb200_acquire_* /
  * gb200_tracker_process* then read.  n_ms <= min(capacity_ms, milliseconds appended so far).                          */
@@ -99,7 +104,8 @@ int gb200_acquire_grid_device(gb200_engine* e, int n_blocks, int ms_per_block, c
  * scan): copy-in, both kernels and copy-out are replayed as one CUDA graph per grid shape, one host synchronisation.
  * iq_host: complex64[n_blocks * ms_per_block * N].  Pageable and pinned buffers are both accepted; with pinned ones
  * (cudaHostAlloc / cudaHostRegister) inputs above 64 KB are read by the copy engine in place and small record sets
- * (<= 256 KB) are stored by the kernel straight into out_host, which saves the two staging copies.                    */
+ * (<= 256 KB) are stored by the kernel straight into out_host, which saves the two staging copies.  The call
+ * synchronises before it returns, so both buffers may be reused, a pinned iq_host rewritten, as soon as it has.      */
 int gb200_acquire_grid_host(gb200_engine* e, const float* iq_host, int n_blocks, int ms_per_block, const int32_t* prn_idx,
                             int n_prn, const double* doppler_hz, int n_doppler, int integration_type,
                             gb200_cell_record* out_host);
@@ -279,8 +285,10 @@ int gb200_tracker_undo_channel(gb200_tracker* t, int channel);
  * gb200_acquire_grid on it and sends the n_blocks*P*D records to out_host; `collect` waits for the OLDEST batch in
  * flight.  Up to `depth` batches are in flight: the host->device copy of batch k+1 and the device->host copy of batch
  * k-1 run on their own streams under the kernels of batch k.  iq_host / out_host are DMA'd directly when they are
- * pinned, staged otherwise; both must stay valid until the batch is collected.  While a stream exists it owns the
- * engine's IQ binding (gb200_upload_iq / gb200_bind_iq_device must be called again before other acquire calls). */
+ * pinned, staged otherwise; both must stay valid, and a pinned iq_host unchanged, until the batch is collected.  While
+ * a stream exists it owns the engine's IQ binding (gb200_upload_iq / gb200_bind_iq_device must be called again before
+ * other acquire calls).  A stream needs no IQ bound to be created: each submit binds its own.  destroy waits for the
+ * batches in flight; their records are in a pinned out_host by then, and a staged batch's are dropped uncollected.  */
 typedef struct gb200_grid_stream gb200_grid_stream;
 int gb200_grid_stream_create(gb200_engine* e, int n_blocks, int n_ms, const int32_t* prn_idx, int n_prn,
                              const double* doppler_hz, int n_doppler, int kind, int depth, gb200_grid_stream** out);
