@@ -236,19 +236,31 @@ class Engine:
         self.iq_tag = tag
 
     # -- the hot path --------------------------------------------------------------------------------------
+    def _grid(self, name: str, n_blocks: int, ms_per_block: int, prn_idx, doppler_hz, out, segments: tuple = (),
+              kind: int | None = None):
+        """Every grid method but acquire_grid_host: gb200_<name> over int32 PRN rows and float64 Dopplers with the family's
+        arguments (kind, or segments: (coherent_ms,) or (coherent_ms, bit_phases)).  out: a _device call's device address
+        (returns None), else the records, RECORD_DTYPE [n_blocks, n_prn, (bit_phases,) n_doppler] or (0,) for a grid with no
+        cells, made when None; best records (BEST_DTYPE [n_blocks, n_prn]) are always made.  Returns them."""
+        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
+        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
+        ret = None
+        if name.endswith("_best"):
+            ret = np.empty((max(n_blocks, 0), prn.size), dtype=BEST_DTYPE)
+        elif not name.endswith("_device"):
+            shape = (n_blocks, prn.size, *segments[1:], dop.size)  # a weak grid's bit phases fold into the bins
+            ret = _records_out(out, shape if min(shape) > 0 else (0,))
+        tail = () if kind is None else (kind,)
+        rc = getattr(self._lib, "gb200_" + name)(self._h, n_blocks, ms_per_block, *segments, _ptr(prn), prn.size, _ptr(dop),
+                                                 dop.size, *tail, _P(out) if ret is None else _ptr(ret))
+        self._check(rc, "gb200_" + name)
+        return ret
+
     def acquire_grid(self, n_blocks: int, ms_per_block: int, prn_idx, doppler_hz, kind: int = NON_COHERENT,
                      out: np.ndarray | None = None) -> np.ndarray:
         """out: optional preallocated RECORD_DTYPE array [n_blocks, n_prn, n_doppler]; if it lives in pinned memory
         (e.g. a view of a torch pinned tensor) the records are DMA'd straight into it."""
-        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
-        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
-        out = _records_out(out, (n_blocks, prn.size, dop.size))
-        self._check(
-            self._lib.gb200_acquire_grid(self._h, n_blocks, ms_per_block, _ptr(prn), prn.size, _ptr(dop), dop.size, kind,
-                                         _ptr(out)),
-            "gb200_acquire_grid",
-        )
-        return out
+        return self._grid("acquire_grid", n_blocks, ms_per_block, prn_idx, doppler_hz, out, kind=kind)
 
     def acquire_grid_host(self, iq, n_blocks: int, ms_per_block: int, prn_idx, doppler_hz, kind: int = NON_COHERENT,
                           out: np.ndarray | None = None) -> np.ndarray:
@@ -284,120 +296,56 @@ class Engine:
 
     def acquire_grid_best(self, n_blocks: int, ms_per_block: int, prn_idx, doppler_hz, kind: int = NON_COHERENT) -> np.ndarray:
         """acquisition.py:179-189 per (block, prn) row: BEST_DTYPE [n_blocks, n_prn]."""
-        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
-        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
-        out = np.empty((n_blocks, prn.size), dtype=BEST_DTYPE)
-        self._check(
-            self._lib.gb200_acquire_grid_best(self._h, n_blocks, ms_per_block, _ptr(prn), prn.size, _ptr(dop), dop.size, kind,
-                                              _ptr(out)),
-            "gb200_acquire_grid_best",
-        )
-        return out
+        return self._grid("acquire_grid_best", n_blocks, ms_per_block, prn_idx, doppler_hz, None, kind=kind)
 
     def acquire_grid_best_device(self, n_blocks, ms_per_block, prn: np.ndarray, dop: np.ndarray, kind: int, out_device_ptr: int):
-        self._check(
-            self._lib.gb200_acquire_grid_best_device(self._h, n_blocks, ms_per_block, _ptr(prn), prn.size, _ptr(dop), dop.size,
-                                                     kind, _P(out_device_ptr)),
-            "gb200_acquire_grid_best_device",
-        )
+        self._grid("acquire_grid_best_device", n_blocks, ms_per_block, prn, dop, out_device_ptr, kind=kind)
 
     def acquire_grid_device(self, n_blocks, ms_per_block, prn: np.ndarray, dop: np.ndarray, kind: int, out_device_ptr: int):
-        """prn (int32) / dop (float64) must be contiguous arrays kept alive by the caller; enqueue only."""
-        self._check(
-            self._lib.gb200_acquire_grid_device(self._h, n_blocks, ms_per_block, _ptr(prn), prn.size, _ptr(dop), dop.size,
-                                                kind, _P(out_device_ptr)),
-            "gb200_acquire_grid_device",
-        )
+        """Enqueue only: the records reach out_device_ptr in the engine's stream order."""
+        self._grid("acquire_grid_device", n_blocks, ms_per_block, prn, dop, out_device_ptr, kind=kind)
 
     def acquire_grid_semicoherent(self, n_blocks: int, ms_per_block: int, coherent_ms: int, prn_idx, doppler_hz,
                                   out: np.ndarray | None = None) -> np.ndarray:
         """Semi-coherent grid (gb200_acquire_grid_semicoherent): per cell the profile sum_k |coherent sum of milliseconds
         k*coherent_ms .. (k+1)*coherent_ms - 1|, reduced to RECORD_DTYPE [n_blocks, n_prn, n_doppler]."""
-        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
-        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
-        out = _records_out(out, (n_blocks, prn.size, dop.size))
-        self._check(
-            self._lib.gb200_acquire_grid_semicoherent(self._h, n_blocks, ms_per_block, coherent_ms, _ptr(prn), prn.size,
-                                                      _ptr(dop), dop.size, _ptr(out)),
-            "gb200_acquire_grid_semicoherent",
-        )
-        return out
+        return self._grid("acquire_grid_semicoherent", n_blocks, ms_per_block, prn_idx, doppler_hz, out, (coherent_ms,))
 
     def acquire_grid_semicoherent_device(self, n_blocks, ms_per_block, coherent_ms, prn: np.ndarray, dop: np.ndarray,
                                          out_device_ptr: int):
-        """prn (int32) / dop (float64) must be contiguous arrays kept alive by the caller; enqueue only."""
-        self._check(
-            self._lib.gb200_acquire_grid_semicoherent_device(self._h, n_blocks, ms_per_block, coherent_ms, _ptr(prn), prn.size,
-                                                             _ptr(dop), dop.size, _P(out_device_ptr)),
-            "gb200_acquire_grid_semicoherent_device",
-        )
+        """Enqueue only: the records reach out_device_ptr in the engine's stream order."""
+        self._grid("acquire_grid_semicoherent_device", n_blocks, ms_per_block, prn, dop, out_device_ptr, (coherent_ms,))
 
     def acquire_grid_semicoherent_best(self, n_blocks: int, ms_per_block: int, coherent_ms: int, prn_idx,
                                        doppler_hz) -> np.ndarray:
         """The semi-coherent grid's best bin per (block, prn) row: BEST_DTYPE [n_blocks, n_prn]."""
-        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
-        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
-        out = np.empty((n_blocks, prn.size), dtype=BEST_DTYPE)
-        self._check(
-            self._lib.gb200_acquire_grid_semicoherent_best(self._h, n_blocks, ms_per_block, coherent_ms, _ptr(prn), prn.size,
-                                                           _ptr(dop), dop.size, _ptr(out)),
-            "gb200_acquire_grid_semicoherent_best",
-        )
-        return out
+        return self._grid("acquire_grid_semicoherent_best", n_blocks, ms_per_block, prn_idx, doppler_hz, None, (coherent_ms,))
 
     def acquire_grid_semicoherent_best_device(self, n_blocks, ms_per_block, coherent_ms, prn: np.ndarray, dop: np.ndarray,
                                               out_device_ptr: int):
-        self._check(
-            self._lib.gb200_acquire_grid_semicoherent_best_device(self._h, n_blocks, ms_per_block, coherent_ms, _ptr(prn),
-                                                                  prn.size, _ptr(dop), dop.size, _P(out_device_ptr)),
-            "gb200_acquire_grid_semicoherent_best_device",
-        )
+        self._grid("acquire_grid_semicoherent_best_device", n_blocks, ms_per_block, prn, dop, out_device_ptr, (coherent_ms,))
 
     def acquire_grid_weak(self, n_blocks: int, ms_per_block: int, coherent_ms: int, bit_phases: int, prn_idx, doppler_hz,
                           out: np.ndarray | None = None) -> np.ndarray:
         """Weak grid (gb200_acquire_grid_weak): per cell and bit phase j the semi-coherent profile of the segments starting
         at millisecond j * coherent_ms / bit_phases, every millisecond realigned by its code Doppler, reduced to
         RECORD_DTYPE [n_blocks, n_prn, bit_phases, n_doppler]."""
-        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
-        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
-        shape = (n_blocks, prn.size, bit_phases, dop.size)
-        out = _records_out(out, shape if min(shape) > 0 else (0,))
-        self._check(
-            self._lib.gb200_acquire_grid_weak(self._h, n_blocks, ms_per_block, coherent_ms, bit_phases, _ptr(prn), prn.size,
-                                              _ptr(dop), dop.size, _ptr(out)),
-            "gb200_acquire_grid_weak",
-        )
-        return out
+        return self._grid("acquire_grid_weak", n_blocks, ms_per_block, prn_idx, doppler_hz, out, (coherent_ms, bit_phases))
 
     def acquire_grid_weak_device(self, n_blocks, ms_per_block, coherent_ms, bit_phases, prn: np.ndarray, dop: np.ndarray,
                                  out_device_ptr: int):
-        """prn (int32) / dop (float64) must be contiguous arrays kept alive by the caller; enqueue only."""
-        self._check(
-            self._lib.gb200_acquire_grid_weak_device(self._h, n_blocks, ms_per_block, coherent_ms, bit_phases, _ptr(prn),
-                                                     prn.size, _ptr(dop), dop.size, _P(out_device_ptr)),
-            "gb200_acquire_grid_weak_device",
-        )
+        """Enqueue only: the records reach out_device_ptr in the engine's stream order."""
+        self._grid("acquire_grid_weak_device", n_blocks, ms_per_block, prn, dop, out_device_ptr, (coherent_ms, bit_phases))
 
     def acquire_grid_weak_best(self, n_blocks: int, ms_per_block: int, coherent_ms: int, bit_phases: int, prn_idx,
                                doppler_hz) -> np.ndarray:
         """The weak grid's best folded bin per (block, prn) row: BEST_DTYPE [n_blocks, n_prn], bin = j * n_doppler + d."""
-        prn = np.ascontiguousarray(prn_idx, dtype=np.int32)
-        dop = np.ascontiguousarray(doppler_hz, dtype=np.float64)
-        out = np.empty((max(n_blocks, 0), prn.size), dtype=BEST_DTYPE)
-        self._check(
-            self._lib.gb200_acquire_grid_weak_best(self._h, n_blocks, ms_per_block, coherent_ms, bit_phases, _ptr(prn),
-                                                   prn.size, _ptr(dop), dop.size, _ptr(out)),
-            "gb200_acquire_grid_weak_best",
-        )
-        return out
+        return self._grid("acquire_grid_weak_best", n_blocks, ms_per_block, prn_idx, doppler_hz, None, (coherent_ms, bit_phases))
 
     def acquire_grid_weak_best_device(self, n_blocks, ms_per_block, coherent_ms, bit_phases, prn: np.ndarray, dop: np.ndarray,
                                       out_device_ptr: int):
-        self._check(
-            self._lib.gb200_acquire_grid_weak_best_device(self._h, n_blocks, ms_per_block, coherent_ms, bit_phases,
-                                                          _ptr(prn), prn.size, _ptr(dop), dop.size, _P(out_device_ptr)),
-            "gb200_acquire_grid_weak_best_device",
-        )
+        self._grid("acquire_grid_weak_best_device", n_blocks, ms_per_block, prn, dop, out_device_ptr,
+                   (coherent_ms, bit_phases))
 
     def acquire_cells(self, prn_idx, doppler_hz, n_ms: int, kind: int = NON_COHERENT, probe_idx=None) -> np.ndarray:
         prn = np.ascontiguousarray(prn_idx, dtype=np.int32)

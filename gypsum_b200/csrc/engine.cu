@@ -218,13 +218,6 @@ int check_weak(gb200_engine* e, int ms_per_block, int coherent_ms, int bit_phase
     return GB200_OK;
 }
 
-// The weak grid's folded Doppler axis: slot j * D + d holds dop[d].
-std::vector<double> fold_dopplers(const double* dop, int D, int B) {
-    std::vector<double> folded(static_cast<size_t>(B) * D);
-    for (int j = 0; j < B; ++j) std::copy(dop, dop + D, folded.begin() + static_cast<size_t>(j) * D);
-    return folded;
-}
-
 // What every acquisition needs before its own arguments are looked at.
 int check_common(gb200_engine* e, int n_ms, int kind) {
     GB_TRY(check_kind(e, kind));
@@ -261,20 +254,34 @@ int upload_grid_axes(gb200_engine* e, const int32_t* prn_idx, int P, const doubl
     return GB200_OK;
 }
 
-// grid mode: all cells of n_blocks x prn list x doppler list; records written to rec_dev (device).  The caller has applied
-// check_grid.  seg.T > 1 (non-coherent kind, check_segments applied): a semi-coherent grid, whose correlate launch is the
-// non-coherent one over the M / T segment spectra of each unit.  A weak grid (seg.B >= 1, check_weak applied) is the same
-// over its seg.count(M) segments, with dop the folded list of D = B * (caller's Dopplers) slots.
-int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D, int kind,
-             CellRecord* rec_dev, Segments seg = {}) {
+// One grid call: n_blocks blocks of M milliseconds x P PRN rows x D Dopplers, each block's milliseconds summed as seg says.
+// weak: seg.B is the caller's bit_phases, held to check_weak (B = 0 included).  A weak grid has bins() = B * D folded bins,
+// and run_grid reads dop as that folded list.
+struct GridCall {
+    int n_blocks, M;
+    const int32_t* prn;
+    int P;
+    const double* dop;
+    int D, kind;
+    Segments seg;
+    bool weak;
+    int bins() const { return D * std::max(seg.B, 1); }
+    size_t rows() const { return static_cast<size_t>(n_blocks) * P; }  // (block, PRN) rows
+};
+
+// grid mode: all cells of g, records written to rec_dev (device).  The caller has applied check_grid and the segment rule
+// (check_segments or check_weak).  seg.T > 1 or a weak grid: the correlate launch is the non-coherent one over the
+// seg.count(M) segment spectra of each (block, bin) unit.
+int run_grid(gb200_engine* e, const GridCall& g, CellRecord* rec_dev) {
+    const int n_blocks = g.n_blocks, M = g.M, P = g.P, D = g.bins(), kind = g.kind;  // D: the (folded) bins
     GB_TRY(check_common(e, M, kind));
     if (static_cast<int64_t>(n_blocks) * M * e->N > e->iq_samples)
         GB_FAIL(e, GB200_EINVAL, "grid needs %lld samples, %lld loaded", static_cast<long long>(n_blocks) * M * e->N,
                 static_cast<long long>(e->iq_samples));
-    GB_TRY(check_prns(e, prn_idx, P));
-    GB_TRY(upload_grid_axes(e, prn_idx, P, dop, D));
+    GB_TRY(check_prns(e, g.prn, P));
+    GB_TRY(upload_grid_axes(e, g.prn, P, g.dop, D));
 
-    const int K = seg.count(M);  // spectra per unit
+    const int K = g.seg.count(M);  // spectra per unit
     const size_t unit = unit_floats2(e, K);
     const size_t per_block = unit * D;
     int nb = static_cast<int>(std::max<size_t>(1, e->spec_budget_bytes / (per_block * sizeof(float2))));
@@ -288,7 +295,7 @@ int run_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P
         const int nbb = std::min(nb, n_blocks - b0);
         const int chunks = (nbb * D + cpg - 1) / cpg;  // groups per PRN: its nbb*D cells in chunks of cpg
         GB_TRY(run_spectra(e, e->iq + static_cast<size_t>(b0) * M * e->N, M, e->d_doppler.p, D, nbb * D, spectra_pfa(kind, false),
-                           seg));
+                           g.seg));
 
         CorrelateArgs ca = correlate_args(e, K, kind, rsplit, rec_dev + static_cast<size_t>(b0) * P * D, nullptr);
         ca.n_groups = P * chunks;
@@ -416,36 +423,37 @@ int run_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, const double
     return GB200_OK;
 }
 
-// The grid's records into d_records, after check_grid; with best, then each (block, PRN) row's best bin into best
-// (acquisition.py:179-189 on the device).  seg as for run_grid.
-int grid_records(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D, int kind,
-                 BestRecord* best, Segments seg = {}) {
-    GB_CUDA(e, e->d_records.ensure(static_cast<size_t>(n_blocks) * P * D));
-    GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_records.p, seg));
-    if (best) GB_LAUNCH(e, -1, launch_best_bins(n_blocks * P, D, e->N, e->d_records.p, e->d_doppler.p, best, e->stream));
-    return GB200_OK;
-}
+// Where a grid call's output goes: its records, or each (block, PRN) row's best bin (acquisition.py:179-189 on the
+// device), into the caller's device buffer or to the host.
+enum class GridOut { records_device, records_host, best_device, best_host };
 
-// A weak grid, every rule checked first: its records into rec (device) when given, else into d_records and, with best, each
-// (block, PRN) row's best folded bin into best; host_best: into d_best.
-int weak_grid(gb200_engine* e, int n_blocks, int M, int T, int B, const int32_t* prn_idx, int P, const double* dop, int D,
-              CellRecord* rec, BestRecord* best, bool host_best = false) {
+// Every gb200_acquire_grid* entry point but gb200_acquire_grid_host: the argument rules in the header's order (nothing is
+// launched on an error), the grid, then its output.
+int acquire_grid(gb200_engine* e, GridCall g, GridOut to, void* out) {
+    if (!e) return GB200_EINVAL;
+    if (!out) GB_FAIL(e, GB200_EINVAL, "null output");
     GB_CUDA(e, cudaSetDevice(e->device));
-    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    GB_TRY(check_weak(e, M, T, B, D));
-    const std::vector<double> folded = fold_dopplers(dop, D, B);
-    const Segments seg{T, B};
-    if (rec) return run_grid(e, n_blocks, M, prn_idx, P, folded.data(), B * D, GB200_NON_COHERENT, rec, seg);
-    if (host_best) {
-        GB_CUDA(e, e->d_best.ensure(static_cast<size_t>(n_blocks) * P));
+    GB_TRY(check_grid(e, g.n_blocks, g.P, g.D, g.prn, g.dop));
+    GB_TRY(g.weak ? check_weak(e, g.M, g.seg.T, g.seg.B, g.D) : check_segments(e, g.M, g.seg.T));
+    std::vector<double> folded;  // a weak grid's Doppler axis: bin j * D + d holds dop[d]
+    if (g.weak) {
+        for (int j = 0; j < g.seg.B; ++j) folded.insert(folded.end(), g.dop, g.dop + g.D);
+        g.dop = folded.data();
+    }
+    if (to == GridOut::records_device) return run_grid(e, g, static_cast<CellRecord*>(out));
+    const size_t n_rec = g.rows() * g.bins();
+    GB_CUDA(e, e->d_records.ensure(n_rec));
+    BestRecord* best = static_cast<BestRecord*>(out);
+    if (to == GridOut::best_host) {
+        GB_CUDA(e, e->d_best.ensure(g.rows()));
         best = e->d_best.p;
     }
-    return grid_records(e, n_blocks, M, prn_idx, P, folded.data(), B * D, GB200_NON_COHERENT, best, seg);
-}
-
-// Records to the caller (see download).
-int fetch_records(gb200_engine* e, size_t n, gb200_cell_record* out_host) {
-    return download(e, reinterpret_cast<CellRecord*>(out_host), e->d_records.p, n, e->h_records);
+    GB_TRY(run_grid(e, g, e->d_records.p));
+    if (to == GridOut::records_host) return download(e, static_cast<CellRecord*>(out), e->d_records.p, n_rec, e->h_records);
+    GB_LAUNCH(e, -1, launch_best_bins(static_cast<int>(g.rows()), g.bins(), e->N, e->d_records.p, e->d_doppler.p, best,
+                                      e->stream));
+    if (to == GridOut::best_device) return GB200_OK;
+    return download(e, static_cast<BestRecord*>(out), best, g.rows(), e->h_best);
 }
 
 }  // namespace
@@ -577,43 +585,22 @@ int gb200_bind_iq_device(gb200_engine* e, const void* iq_device, int64_t n_sampl
 
 int gb200_acquire_grid_device(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D,
                               int kind, void* out_device) {
-    if (!e) return GB200_EINVAL;
-    if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
-    GB_CUDA(e, cudaSetDevice(e->device));
-    GB_TRY(check_common(e, M, kind));
-    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    return run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, static_cast<CellRecord*>(out_device));
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, kind}, GridOut::records_device, out_device);
 }
 
 int gb200_acquire_grid(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D,
                        int kind, gb200_cell_record* out_host) {
-    if (!e) return GB200_EINVAL;
-    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
-    GB_CUDA(e, cudaSetDevice(e->device));
-    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, kind, nullptr));
-    return fetch_records(e, static_cast<size_t>(n_blocks) * P * D, out_host);
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, kind}, GridOut::records_host, out_host);
 }
 
 int gb200_acquire_grid_best_device(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D,
                                    int kind, void* out_device) {
-    if (!e) return GB200_EINVAL;
-    if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
-    GB_CUDA(e, cudaSetDevice(e->device));
-    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    return grid_records(e, n_blocks, M, prn_idx, P, dop, D, kind, static_cast<BestRecord*>(out_device));
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, kind}, GridOut::best_device, out_device);
 }
 
 int gb200_acquire_grid_best(gb200_engine* e, int n_blocks, int M, const int32_t* prn_idx, int P, const double* dop, int D,
                             int kind, gb200_best_record* out_host) {
-    if (!e) return GB200_EINVAL;
-    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
-    GB_CUDA(e, cudaSetDevice(e->device));
-    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    const size_t n = static_cast<size_t>(n_blocks) * P;
-    GB_CUDA(e, e->d_best.ensure(n));
-    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, kind, e->d_best.p));
-    return download(e, reinterpret_cast<BestRecord*>(out_host), e->d_best.p, n, e->h_best);
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, kind}, GridOut::best_host, out_host);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -622,49 +609,23 @@ int gb200_acquire_grid_best(gb200_engine* e, int n_blocks, int M, const int32_t*
 // ---------------------------------------------------------------------------------------------------------
 int gb200_acquire_grid_semicoherent(gb200_engine* e, int n_blocks, int M, int coherent_ms, const int32_t* prn_idx, int P,
                                     const double* dop, int D, gb200_cell_record* out_host) {
-    if (!e) return GB200_EINVAL;
-    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
-    GB_CUDA(e, cudaSetDevice(e->device));
-    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    GB_TRY(check_segments(e, M, coherent_ms));
-    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, nullptr, Segments{coherent_ms}));
-    return fetch_records(e, static_cast<size_t>(n_blocks) * P * D, out_host);
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, {coherent_ms}}, GridOut::records_host, out_host);
 }
 
 int gb200_acquire_grid_semicoherent_device(gb200_engine* e, int n_blocks, int M, int coherent_ms, const int32_t* prn_idx, int P,
                                            const double* dop, int D, void* out_device) {
-    if (!e) return GB200_EINVAL;
-    if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
-    GB_CUDA(e, cudaSetDevice(e->device));
-    GB_TRY(check_common(e, M, GB200_NON_COHERENT));
-    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    GB_TRY(check_segments(e, M, coherent_ms));
-    return run_grid(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, static_cast<CellRecord*>(out_device),
-                    Segments{coherent_ms});
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, {coherent_ms}}, GridOut::records_device,
+                        out_device);
 }
 
 int gb200_acquire_grid_semicoherent_best(gb200_engine* e, int n_blocks, int M, int coherent_ms, const int32_t* prn_idx, int P,
                                          const double* dop, int D, gb200_best_record* out_host) {
-    if (!e) return GB200_EINVAL;
-    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
-    GB_CUDA(e, cudaSetDevice(e->device));
-    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    GB_TRY(check_segments(e, M, coherent_ms));
-    const size_t n = static_cast<size_t>(n_blocks) * P;
-    GB_CUDA(e, e->d_best.ensure(n));
-    GB_TRY(grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, e->d_best.p, Segments{coherent_ms}));
-    return download(e, reinterpret_cast<BestRecord*>(out_host), e->d_best.p, n, e->h_best);
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, {coherent_ms}}, GridOut::best_host, out_host);
 }
 
 int gb200_acquire_grid_semicoherent_best_device(gb200_engine* e, int n_blocks, int M, int coherent_ms, const int32_t* prn_idx,
                                                 int P, const double* dop, int D, void* out_device) {
-    if (!e) return GB200_EINVAL;
-    if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
-    GB_CUDA(e, cudaSetDevice(e->device));
-    GB_TRY(check_grid(e, n_blocks, P, D, prn_idx, dop));
-    GB_TRY(check_segments(e, M, coherent_ms));
-    return grid_records(e, n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, static_cast<BestRecord*>(out_device),
-                        Segments{coherent_ms});
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, {coherent_ms}}, GridOut::best_device, out_device);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -673,32 +634,26 @@ int gb200_acquire_grid_semicoherent_best_device(gb200_engine* e, int n_blocks, i
 // ---------------------------------------------------------------------------------------------------------
 int gb200_acquire_grid_weak(gb200_engine* e, int n_blocks, int M, int coherent_ms, int bit_phases, const int32_t* prn_idx,
                             int P, const double* dop, int D, gb200_cell_record* out_host) {
-    if (!e) return GB200_EINVAL;
-    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
-    GB_TRY(weak_grid(e, n_blocks, M, coherent_ms, bit_phases, prn_idx, P, dop, D, nullptr, nullptr));
-    return fetch_records(e, static_cast<size_t>(n_blocks) * P * bit_phases * D, out_host);
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, {coherent_ms, bit_phases}, true},
+                        GridOut::records_host, out_host);
 }
 
 int gb200_acquire_grid_weak_device(gb200_engine* e, int n_blocks, int M, int coherent_ms, int bit_phases, const int32_t* prn_idx,
                                    int P, const double* dop, int D, void* out_device) {
-    if (!e) return GB200_EINVAL;
-    if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
-    return weak_grid(e, n_blocks, M, coherent_ms, bit_phases, prn_idx, P, dop, D, static_cast<CellRecord*>(out_device), nullptr);
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, {coherent_ms, bit_phases}, true},
+                        GridOut::records_device, out_device);
 }
 
 int gb200_acquire_grid_weak_best(gb200_engine* e, int n_blocks, int M, int coherent_ms, int bit_phases, const int32_t* prn_idx,
                                  int P, const double* dop, int D, gb200_best_record* out_host) {
-    if (!e) return GB200_EINVAL;
-    if (!out_host) GB_FAIL(e, GB200_EINVAL, "null output");
-    GB_TRY(weak_grid(e, n_blocks, M, coherent_ms, bit_phases, prn_idx, P, dop, D, nullptr, nullptr, true));
-    return download(e, reinterpret_cast<BestRecord*>(out_host), e->d_best.p, static_cast<size_t>(n_blocks) * P, e->h_best);
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, {coherent_ms, bit_phases}, true},
+                        GridOut::best_host, out_host);
 }
 
 int gb200_acquire_grid_weak_best_device(gb200_engine* e, int n_blocks, int M, int coherent_ms, int bit_phases,
                                         const int32_t* prn_idx, int P, const double* dop, int D, void* out_device) {
-    if (!e) return GB200_EINVAL;
-    if (!out_device) GB_FAIL(e, GB200_EINVAL, "null output");
-    return weak_grid(e, n_blocks, M, coherent_ms, bit_phases, prn_idx, P, dop, D, nullptr, static_cast<BestRecord*>(out_device));
+    return acquire_grid(e, {n_blocks, M, prn_idx, P, dop, D, GB200_NON_COHERENT, {coherent_ms, bit_phases}, true},
+                        GridOut::best_device, out_device);
 }
 
 // Host to host in one call.  The first call of a shape runs eagerly (it may have to upload the axes and grow buffers,
@@ -751,7 +706,7 @@ int gb200_acquire_grid_host(gb200_engine* e, const float* iq_host, int n_blocks,
     const bool same = g.seen && g.key == key();
     auto enqueue = [&]() -> int {
         GB_CUDA(e, cudaMemcpyAsync(e->iq_own.p, h2d_src, n_iq * sizeof(float2), cudaMemcpyHostToDevice, e->stream));
-        GB_TRY(run_grid(e, n_blocks, M, prn_idx, P, dop, D, kind, rec_target));
+        GB_TRY(run_grid(e, {n_blocks, M, prn_idx, P, dop, D, kind}, rec_target));
         if (!direct)
             GB_CUDA(e, cudaMemcpyAsync(e->h_records.p, e->d_records.p, n_rec * sizeof(CellRecord), cudaMemcpyDeviceToHost, e->stream));
         return GB200_OK;
@@ -877,7 +832,7 @@ int gb200_acquire_cells(gb200_engine* e, int n_cells, const int32_t* prn_idx, co
     if (n_cells < 1) GB_FAIL(e, GB200_EINVAL, "empty cell list");
     GB_CUDA(e, e->d_records.ensure(n_cells));
     GB_TRY(run_cells(e, n_cells, prn_idx, dop, probe, n_ms, kind, e->d_records.p, nullptr));
-    return fetch_records(e, n_cells, out_host);
+    return download(e, reinterpret_cast<CellRecord*>(out_host), e->d_records.p, n_cells, e->h_records);
 }
 
 int gb200_correlation_profile(gb200_engine* e, int prn, double dop, int n_ms, int kind, float* out_host) {
@@ -1120,7 +1075,7 @@ int gb200_grid_stream_submit(gb200_grid_stream* g, const float* iq_host, gb200_c
     GB_CUDA(e, cudaEventRecord(sl.h2d, g->s_in));
     GB_CUDA(e, cudaStreamWaitEvent(e->stream, sl.h2d, 0));
     bind_iq(e, sl.iq.p, static_cast<int64_t>(n_iq));
-    GB_TRY(run_grid(e, g->n_blocks, g->M, g->prn.data(), g->P, g->dop.data(), g->D, g->kind, sl.rec.p));
+    GB_TRY(run_grid(e, {g->n_blocks, g->M, g->prn.data(), g->P, g->dop.data(), g->D, g->kind}, sl.rec.p));
     GB_CUDA(e, cudaEventRecord(sl.done, e->stream));
     GB_CUDA(e, cudaStreamWaitEvent(g->s_out, sl.done, 0));
     GB_CUDA(e, cudaMemcpyAsync(sl.staged_out ? reinterpret_cast<gb200_cell_record*>(sl.h_rec.p) : out_host, sl.rec.p,

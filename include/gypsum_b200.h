@@ -95,7 +95,11 @@ int gb200_ring_appended(const gb200_ring* r, int64_t* total_ms);
  * out[(block*n_prn + a)*n_doppler + b].
  * Every Doppler a caller passes -- to the grid calls below, gb200_grid_stream_create, gb200_acquire_cells and both
  * gb200_correlation_profile calls -- must be finite: NaN or +-inf is GB200_EINVAL naming the first such index, and
- * nothing is launched (the reference's profile of such a cell is all NaN, which no record can stand for).          */
+ * nothing is launched (the reference's profile of such a cell is all NaN, which no record can stand for).
+ * Every gb200_acquire_grid* call but gb200_acquire_grid_host checks its rules in one order and reports the first one
+ * broken: a null output, then an empty grid and the Dopplers, then the segment rules of the semi-coherent and weak
+ * grids, then the integration type, the replicas, the bound IQ, the milliseconds and samples asked of it, and the PRN
+ * range; nothing is launched on an error.                                                                           */
 int gb200_acquire_grid(gb200_engine* e, int n_blocks, int ms_per_block, const int32_t* prn_idx, int n_prn,
                        const double* doppler_hz, int n_doppler, int integration_type, gb200_cell_record* out_host);
 int gb200_acquire_grid_device(gb200_engine* e, int n_blocks, int ms_per_block, const int32_t* prn_idx, int n_prn,
@@ -132,8 +136,8 @@ int gb200_acquire_grid_best_device(gb200_engine* e, int n_blocks, int ms_per_blo
  * A segment gains 10*log10(T) dB of SNR before its magnitude is taken, and needs Doppler bins of about 1/(2T) s
  * (50 Hz at T = 10 ms).  Records, best records and the layouts of out are those of the gb200_acquire_grid* quartet
  * above over that profile, with the same strength formula.  Rules: coherent_ms >= 1, ms_per_block a multiple of it
- * (a partial segment is GB200_EINVAL, never dropped), and every rule of gb200_acquire_grid; nothing is launched on an
- * error.  coherent_ms == 1 is gb200_acquire_grid(..., GB200_NON_COHERENT), byte for byte.
+ * (a partial segment is GB200_EINVAL, never dropped), and every rule of gb200_acquire_grid, in the order given above.
+ * coherent_ms == 1 is gb200_acquire_grid(..., GB200_NON_COHERENT), byte for byte.
  * Not handled here (the weak grid below handles both): a navigation data bit edge inside a segment (every 20 ms)
  * cancels part of that segment, up to all of it; code Doppler smears the peak by |f| / 1540 chips per second, as in
  * the non-coherent grid.  There is no detection threshold: the reference's strength threshold was set for its own
@@ -165,7 +169,7 @@ int gb200_acquire_grid_semicoherent_best_device(gb200_engine* e, int n_blocks, i
  * B * n_doppler folded bins: bin = j * n_doppler + d, doppler_hz = doppler_hz[d].
  * Rules: coherent_ms >= 1, bit_phases >= 1 dividing coherent_ms, ms_per_block >= coherent_ms + (B-1)*d and
  * ms_per_block - (B-1)*d a multiple of coherent_ms (a partial segment is GB200_EINVAL, never dropped), and every rule of
- * gb200_acquire_grid; nothing is launched on an error.  With B = 1 on a grid where every s_m is 0, the records equal
+ * gb200_acquire_grid, in the order given above.  With B = 1 on a grid where every s_m is 0, the records equal
  * gb200_acquire_grid_semicoherent's byte for byte.  coherent_ms = 1 (B = 1) is a non-coherent grid with realignment.
  * Not handled: a bit edge falls at the satellite's code epoch, inside a millisecond, so even the right phase has up to
  * 1 ms of one segment with the other sign; s_m is a whole sample, which leaves up to 1/2 sample (1/2 chip at 1.023 Msps)

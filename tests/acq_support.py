@@ -83,8 +83,26 @@ def _vector_cols(x, fs, n, svs, dop, kind, probe):
     return peak, arg, total, count, val
 
 
-def _vector_worker(args):
-    return _vector_cols(*args)
+def _apply(args):
+    fn, fn_args = args
+    return fn(*fn_args)
+
+
+def by_doppler_column(cols, n_dop, work, part_args):
+    """cols(*part_args(p)) over the Doppler columns p of an n_dop-column grid, each result an array whose last axis is the
+    Doppler.  Large grids (work: distinct SVs x columns x samples, times the bit phases of a weak grid) are spread over the
+    host's cores (fork pool) by Doppler column and put back together."""
+    procs = max(1, min(n_dop, os.cpu_count() or 1, work // (1 << 24)))
+    if procs == 1:
+        return cols(*part_args(slice(None)))
+    parts = [np.arange(i, n_dop, procs) for i in range(procs)]
+    with _pool(procs) as pool:
+        res = pool.map(_apply, [(cols, part_args(p)) for p in parts])
+    out = [np.zeros(a.shape[:-1] + (n_dop,), a.dtype) for a in res[0]]
+    for p, r in zip(parts, res):
+        for o_, a in zip(out, r):
+            o_[..., p] = a
+    return tuple(out)
 
 
 def vector_grid(x, fs, n, svs, dop, kind=o.NON_COHERENT, probe=None):
@@ -92,40 +110,37 @@ def vector_grid(x, fs, n, svs, dop, kind=o.NON_COHERENT, probe=None):
     with conj(FFT(replica)) of every SV at once and one batched inverse FFT; repeated SVs and bit-equal Doppler entries are
     computed once.  Returns (peak, argmax, sum, count, probe values), each [len(svs), len(dop)]: probe values are the
     coherent (complex) or non-coherent profile at the lag probe[a, b], zeros without probe.  Large grids are spread over
-    the host's cores (fork pool) by Doppler column."""
+    the host's cores by Doppler column (by_doppler_column)."""
     dop = np.asarray(dop, dtype=np.float64)
-    work = len(set(svs)) * dop.size * len(x)
-    procs = max(1, min(dop.size, os.cpu_count() or 1, work // (1 << 24)))
-    if procs == 1:
-        return _vector_cols(x, fs, n, list(svs), dop, kind, probe)
-    parts = [np.arange(i, dop.size, procs) for i in range(procs)]
-    with _pool(procs) as pool:
-        res = pool.map(_vector_worker, [(x, fs, n, list(svs), dop[p], kind,
-                                         None if probe is None else np.asarray(probe)[:, p]) for p in parts])
-    out = [np.zeros((len(svs), dop.size), a.dtype) for a in res[0]]
-    for p, r in zip(parts, res):
-        for o_, a in zip(out, r):
-            o_[:, p] = a
-    return tuple(out)
+    return by_doppler_column(_vector_cols, dop.size, len(set(svs)) * dop.size * len(x), lambda p: (
+        x, fs, n, list(svs), dop[p], kind, None if probe is None else np.asarray(probe)[:, p]))
 
 
-def check_grid(rec, x, fs, n, svs, dop, what, kind=o.NON_COHERENT, ref=None):
-    """Every record of a (SV x Doppler) grid against the oracle: peak, sum and strength within the tolerance, count exact,
-    argmax exact bar near-ties proved on the float64 profile.  ref: the oracle's (peak, argmax, sum, count) of the grid
-    when the caller has them (vector_grid), else o.grid_cells runs here.  Returns the number of near-tie proofs."""
-    peak, arg, total, count = ref if ref is not None else oracle_grid(x, fs, n, svs, dop, kind)
-    assert rec.shape == peak.shape
+def check_records(rec, ref, n, profile, what):
+    """The tolerances of DESIGN.md section 6 on a grid's records against the oracle's ref = (peak, argmax, sum, count), of
+    the same shape: peak and sum within MAG_TOL of the largest, count exact, argmax exact bar near-ties proved on the
+    float64 profile(idx) of the cell at index idx, strength within 1e-4.  Returns the number of near-tie proofs."""
+    peak, arg, total, count = ref
+    assert rec.shape == peak.shape, what
     assert np.abs(rec["peak"] - peak).max() <= MAG_TOL * peak.max(), what
     assert np.abs(rec["sum"] - total).max() <= MAG_TOL * total.max(), what
     assert np.array_equal(rec["count"], count), what
     bad = np.argwhere(rec["argmax"] != arg)
-    for a, b in bad:  # a different index is only acceptable where the float64 profile itself ties to within the tolerance
-        prof = np.abs(o.integrate(kind, x, fs, n, dop[b], o.replica(svs[a], n)))
-        assert prof.max() - prof[rec["argmax"][a, b]] <= MAG_TOL * prof.max(), (what, a, b)
-    strength = rec["peak"].astype(np.float64) / ((rec["sum"] - rec["count"] * rec["peak"].astype(np.float64)) / (n - rec["count"]))
-    ref_strength = peak / ((total - count * peak) / (n - count))
+    for idx in map(tuple, bad):  # a different index is only acceptable where the float64 profile itself ties within the tolerance
+        prof = profile(idx)
+        assert prof.max() - prof[rec["argmax"][idx]] <= MAG_TOL * prof.max(), (what, *idx)
+    strength = o.strength_from_record(rec["peak"].astype(np.float64), rec["sum"], rec["count"], n)
+    ref_strength = o.strength_from_record(peak, total, count, n)
     assert np.abs(strength - ref_strength).max() <= 1e-4 * ref_strength.max(), what
     return len(bad)
+
+
+def check_grid(rec, x, fs, n, svs, dop, what, kind=o.NON_COHERENT, ref=None):
+    """check_records on a (SV x Doppler) grid.  ref: the oracle's (peak, argmax, sum, count) of the grid when the caller
+    has them (vector_grid), else o.grid_cells runs here.  Returns the number of near-tie proofs."""
+    ref = ref if ref is not None else oracle_grid(x, fs, n, svs, dop, kind)
+    return check_records(rec, ref, n, lambda i: np.abs(o.integrate(kind, x, fs, n, dop[i[1]], o.replica(svs[i[0]], n))),
+                         what)
 
 
 def _cells_cols(x, fs, n, svs, dop, kind, probe, cols):

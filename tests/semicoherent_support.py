@@ -7,11 +7,10 @@ milliseconds add exact zeros.  vector_semicoherent is the same arithmetic batche
 acq_support.vector_grid: per (Doppler, segment) the wiped-off milliseconds' forward FFTs are summed and one batched inverse
 FFT runs over every SV."""
 import math
-import os
 
 import numpy as np
 
-from acq_support import MAG_TOL, _pool, _replica_spectrum
+from acq_support import _replica_spectrum, by_doppler_column, check_records
 from oracle import gypsum_oracle as o
 
 
@@ -51,44 +50,19 @@ def _semi_cols(x, fs, n, svs, dop, coherent_ms):
     return peak, arg, total, count
 
 
-def _semi_worker(args):
-    return _semi_cols(*args)
-
-
 def vector_semicoherent(x, fs, n, svs, dop, coherent_ms):
     """(peak, argmax, sum, count) of every (SV, Doppler) cell of one block's semi-coherent grid, each [len(svs),
     len(dop)].  Large grids are spread over the host's cores by Doppler column."""
     dop = np.asarray(dop, dtype=np.float64)
-    work = len(set(svs)) * dop.size * len(x)
-    procs = max(1, min(dop.size, os.cpu_count() or 1, work // (1 << 24)))
-    if procs == 1:
-        return _semi_cols(x, fs, n, list(svs), dop, coherent_ms)
-    parts = [np.arange(i, dop.size, procs) for i in range(procs)]
-    with _pool(procs) as pool:
-        res = pool.map(_semi_worker, [(x, fs, n, list(svs), dop[p], coherent_ms) for p in parts])
-    out = [np.zeros((len(svs), dop.size), a.dtype) for a in res[0]]
-    for p, r in zip(parts, res):
-        for o_, a in zip(out, r):
-            o_[:, p] = a
-    return tuple(out)
+    return by_doppler_column(_semi_cols, dop.size, len(set(svs)) * dop.size * len(x),
+                             lambda p: (x, fs, n, list(svs), dop[p], coherent_ms))
 
 
 def check_semicoherent(rec, x, fs, n, svs, dop, coherent_ms, what, ref=None):
-    """acq_support.check_grid for one block of a semi-coherent grid: peak and sum within MAG_TOL of the largest, count
-    exact, strength within 1e-4, argmax exact bar near-ties proved on the float64 profile.  Returns the near-tie proofs."""
-    peak, arg, total, count = ref if ref is not None else vector_semicoherent(x, fs, n, svs, dop, coherent_ms)
-    assert rec.shape == peak.shape, what
-    assert np.abs(rec["peak"] - peak).max() <= MAG_TOL * peak.max(), what
-    assert np.abs(rec["sum"] - total).max() <= MAG_TOL * total.max(), what
-    assert np.array_equal(rec["count"], count), what
-    bad = np.argwhere(rec["argmax"] != arg)
-    for a, b in bad:
-        prof = integrate_semicoherent(x, fs, n, dop[b], o.replica(svs[a], n), coherent_ms)
-        assert prof.max() - prof[rec["argmax"][a, b]] <= MAG_TOL * prof.max(), (what, a, b)
-    strength = o.strength_from_record(rec["peak"].astype(np.float64), rec["sum"], rec["count"], n)
-    ref_strength = o.strength_from_record(peak, total, count, n)
-    assert np.abs(strength - ref_strength).max() <= 1e-4 * ref_strength.max(), what
-    return len(bad)
+    """acq_support.check_records for one block of a semi-coherent grid.  Returns the near-tie proofs."""
+    ref = ref if ref is not None else vector_semicoherent(x, fs, n, svs, dop, coherent_ms)
+    return check_records(rec, ref, n, lambda i: integrate_semicoherent(x, fs, n, dop[i[1]], o.replica(svs[i[0]], n),
+                                                                       coherent_ms), what)
 
 
 def best_bins(peak):

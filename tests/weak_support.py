@@ -7,11 +7,10 @@ j * T / B + k * T.  vector_weak is the same arithmetic batched for grids, in the
 semicoherent_support.vector_semicoherent.  synth_weak_iq plants satellites whose code runs at (1 + f / f_L1) * 1.023 MHz
 and whose +-1 data bits change at their own code epochs."""
 import math
-import os
 
 import numpy as np
 
-from acq_support import MAG_TOL, _pool, _replica_spectrum
+from acq_support import _replica_spectrum, by_doppler_column, check_records
 from oracle import gypsum_oracle as o
 
 F_L1 = 1575.42e6
@@ -76,45 +75,19 @@ def _weak_cols(x, fs, n, svs, dop, coherent_ms, bit_phases):
     return peak, arg, total, count
 
 
-def _weak_worker(args):
-    return _weak_cols(*args)
-
-
 def vector_weak(x, fs, n, svs, dop, coherent_ms, bit_phases):
     """(peak, argmax, sum, count) of every (SV, bit phase, Doppler) cell of one block's weak grid, each [len(svs),
     bit_phases, len(dop)].  Large grids are spread over the host's cores by Doppler column."""
     dop = np.asarray(dop, dtype=np.float64)
-    work = len(set(svs)) * dop.size * len(x) * bit_phases
-    procs = max(1, min(dop.size, os.cpu_count() or 1, work // (1 << 24)))
-    if procs == 1:
-        return _weak_cols(x, fs, n, list(svs), dop, coherent_ms, bit_phases)
-    parts = [np.arange(i, dop.size, procs) for i in range(procs)]
-    with _pool(procs) as pool:
-        res = pool.map(_weak_worker, [(x, fs, n, list(svs), dop[p], coherent_ms, bit_phases) for p in parts])
-    out = [np.zeros((len(svs), bit_phases, dop.size), a.dtype) for a in res[0]]
-    for p, r in zip(parts, res):
-        for o_, a in zip(out, r):
-            o_[:, :, p] = a
-    return tuple(out)
+    return by_doppler_column(_weak_cols, dop.size, len(set(svs)) * dop.size * len(x) * bit_phases,
+                             lambda p: (x, fs, n, list(svs), dop[p], coherent_ms, bit_phases))
 
 
 def check_weak(rec, x, fs, n, svs, dop, coherent_ms, bit_phases, what, ref=None):
-    """The tolerances of DESIGN.md section 6 on one block's weak records [n_svs, B, D]: peak and sum within MAG_TOL of
-    the largest, count exact, strength within 1e-4, argmax exact bar near-ties proved on the float64 profile.  Returns
-    the number of near-tie proofs."""
-    peak, arg, total, count = ref if ref is not None else vector_weak(x, fs, n, svs, dop, coherent_ms, bit_phases)
-    assert rec.shape == peak.shape, what
-    assert np.abs(rec["peak"] - peak).max() <= MAG_TOL * peak.max(), what
-    assert np.abs(rec["sum"] - total).max() <= MAG_TOL * total.max(), what
-    assert np.array_equal(rec["count"], count), what
-    bad = np.argwhere(rec["argmax"] != arg)
-    for a, j, b in bad:
-        prof = integrate_weak(x, fs, n, dop[b], o.replica(svs[a], n), coherent_ms, bit_phases)[j]
-        assert prof.max() - prof[rec["argmax"][a, j, b]] <= MAG_TOL * prof.max(), (what, a, j, b)
-    strength = o.strength_from_record(rec["peak"].astype(np.float64), rec["sum"], rec["count"], n)
-    ref_strength = o.strength_from_record(peak, total, count, n)
-    assert np.abs(strength - ref_strength).max() <= 1e-4 * ref_strength.max(), what
-    return len(bad)
+    """acq_support.check_records on one block's weak records [n_svs, B, D].  Returns the number of near-tie proofs."""
+    ref = ref if ref is not None else vector_weak(x, fs, n, svs, dop, coherent_ms, bit_phases)
+    return check_records(rec, ref, n, lambda i: integrate_weak(x, fs, n, dop[i[2]], o.replica(svs[i[0]], n), coherent_ms,
+                                                               bit_phases)[i[1]], what)
 
 
 def best_folded(peak):
